@@ -1,17 +1,19 @@
 #!/usr/bin/env python
-"""Headline benchmark: tokens/sec of LLaMA-7B int4 g128 batch-1 decode on B200 (BASELINE.json metric),
+"""Headline benchmark: tokens/sec of LLaMA-7B int4 g128 batch-1 decode on H100 (BASELINE.json metric),
 plus the roofline of the dominant kernel and the CPU baseline, as ONE JSON line on rank 0.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config 7b|13b-int3|65b|prefill]   # our arm
-    python bench.py --impl reference [--steps K] [--warmup W]                                  # the reference's arithmetic on the host cores
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config 7b|13b-int3|65b|prefill] [--dump-outputs DIR]   # our arm
+    python bench.py --impl reference [--steps K] [--warmup W]                                                      # the reference's arithmetic on the host cores
 
 A "step" is one decoded token: one replay of the captured CUDA graph of gptq_llama_decode_step (ONE persistent kernel) over a
-random-init LLaMA-7B-shaped GPTQ model (32 distinct layers, 3.6 GB of packed weights per step, i.e. far larger than the 126 MB
+random-init LLaMA-7B-shaped GPTQ model (32 distinct layers, 3.6 GB of packed weights per step, i.e. far larger than the 50 MB
 L2, so every step streams from HBM) at context position seq-1 = 2047.
 N > 1 (torchrun): the path does not shard at this size ("replicas only", DESIGN.md): every rank decodes its own sequence on its
 own GPU, no data-path collective; value = total tokens/s, scaling = weak.
 --config selects the other BASELINE.json configurations (13b-int3 = config 4, 65b = the config-5 model on one GPU, prefill = config 3);
 the default is config 2, the one the metric is quoted on.
+--dump-outputs DIR writes what the timed path computed in its last step as DIR/<name>.npy (float32); every input is generated from
+fixed seeds, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -37,18 +39,16 @@ def _host_threads():
 if '--impl' in sys.argv and 'reference' in sys.argv:
     # the CPU arm sets its thread count itself (torchrun exports OMP_NUM_THREADS=1, which must not leak into it), before torch / libgomp
     # are loaded.  32 threads: the restatement is bound by its bit-unpacking loop per 32-column block and two OpenMP runtimes are alive in
-    # the process (torch's and the oracle's); with all 128 hardware threads of the B200 hosts spinning in both, a token took 3.5 - 13.8 s from
-    # run to run, with 8 threads of the build container 4.6 s.  Passive waiting keeps idle workers off the cores.
+    # the process (torch's and the oracle's); with every hardware thread of a large host spinning in both, token times varied several-fold
+    # from run to run.  Passive waiting keeps idle workers off the cores.
     os.environ['OMP_NUM_THREADS'] = os.environ.get('BENCH_CPU_THREADS', str(min(32, _host_threads())))
     os.environ['OMP_WAIT_POLICY'] = 'passive' 
 
 import torch  # noqa: E402
 
-METRIC = 'tokens/sec LLaMA-7B int4 g128 batch=1; matvec HBM GB/s vs 8 TB/s roofline'
+METRIC = 'tokens/sec LLaMA-7B int4 g128 batch=1; matvec HBM GB/s vs 3.35 TB/s roofline'
 SEQ = 2048
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of llama_decode_mega_kernel on the 32-layer model at context 2047
-# (ncu --set full, profiles/r2_mega_summary.txt, profiles/r2_mega_final.ncu-rep)
-NCU_TRAFFIC_BYTES = {'7b': 4737481728}  # 4.7074 GB read + 30.1 MB written (algorithmic: 4.7084 GB)
+DUMP_ROWS = 128  # rows of each prefill output written by --dump-outputs (a fixed, seeded sample of the 65536)
 CONFIGS = {  # name -> (size, bits, act_order, BASELINE.json config)
     '7b': ('7b', 4, False, 'LLaMA-7B int4 g128 batch=1 decode'),
     '13b-int3': ('13b', 3, True, 'LLaMA-13B int3 g128 act-order batch=1 decode'),
@@ -64,12 +64,28 @@ def alg_bytes_qlinear(K, N, bits, M=1, gs=GROUP):
     return K * N * bits // 8 + G * N * 2 + G * N * bits // 8 + 4 * K + 2 * M * K + 2 * M * N
 
 
-def measured_peaks():
-    path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(path):
-        d = json.load(open(path))
-        return d.get('hbm_gbs', 6650.0), d.get('bf16_tflops', 1590.0), d.get('bf16_tflops_sustained', 1400.0), 'measured (MEASURED_PEAKS.json)'
-    return 6650.0, 1590.0, 1400.0, 'fallback (B200_PROFILING.md)'
+def datasheet_peaks():
+    """HBM GB/s and dense fp16 TFLOP/s of the H100 SXM (NVIDIA data sheet, 700 W); a card with a lower power limit reaches less."""
+    return 3350.0, 989.0, 'NVIDIA H100 SXM data sheet (700 W)'
+
+
+def gpu_identity(index):
+    """Name and power limit of the card the numbers were taken on."""
+    try:
+        out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader', '-i', str(index)], capture_output=True, text=True,
+                             timeout=30).stdout.strip()
+        name, limit = [f.strip() for f in out.split(',')]
+        return {'name': name, 'power_limit': limit}
+    except (OSError, ValueError, subprocess.SubprocessError):
+        return {'name': torch.cuda.get_device_name(index), 'power_limit': None}
+
+
+def dump_outputs(dirname, arrays):
+    """Write each array as dirname/<name>.npy in float32."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(dirname, f'{name}.npy'), t.detach().float().cpu().numpy())
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -242,8 +258,9 @@ def run_decode(args):
     else:
         dec = engine.synthetic_llama(size, bits=bits, groupsize=GROUP, act_order=act, device=str(dev), seed=rank, max_seq=SEQ)
     # synthetic context: the cache holds seq-1 = 2047 tokens of random K/V; the step decodes token 2048
-    dec.k_cache.normal_(0, 0.5)
-    dec.v_cache.normal_(0, 0.5)
+    gen = torch.Generator(device=dev).manual_seed(1000 + rank)
+    dec.k_cache.normal_(0, 0.5, generator=gen)
+    dec.v_cache.normal_(0, 0.5, generator=gen)
     pos = SEQ - 1
     dec.positions.fill_(pos)
     dec.tokens.fill_(1)
@@ -255,6 +272,8 @@ def run_decode(args):
     assert bool(torch.isfinite(dec.logits).all()), 'non-finite logits'
     sampler = ClockSampler(local) if rank == 0 else None
     t_dev = timed(dec.step, steps, dist_on)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {'logits': dec.logits, 'next_tokens': dec.next_tokens})
 
     # ---- end-to-end arm: host token in -> H2D -> step -> D2H logits, every step -----------------------
     tok_host = torch.ones(1, dtype=torch.int32).pin_memory()
@@ -297,7 +316,7 @@ def run_decode(args):
         reps = 10
         t_k = timed(graph.replay, reps, False) / (reps * len(gates))
         kbytes = 2 * alg_bytes_qlinear(dec.hidden, dec.intermediate, bits) - 2 * dec.hidden  # two weights, x read once
-    peak, _, _, peak_src = measured_peaks()
+    peak, _, peak_src = datasheet_peaks()
 
     # max over ranks, whole-job aggregate
     tt = torch.tensor([t_dev, t_e2e], device=dev, dtype=torch.float64)
@@ -320,7 +339,7 @@ def run_decode(args):
                 'workload': f'{title}, context {pos} (seq={SEQ}), {L} layers, random-init packed weights',
                 'parallelism': (f'tp{world}: heads / MLP columns sharded, o_proj and down_proj partial sums RED-added into every rank over NVLink inside the kernel' if tp else
                                 'replicas only (one independent sequence per GPU, no data-path collective)' if world > 1 else 'single GPU'),
-                'l2': f'each step streams {L * per_layer / 1e9:.1f} GB of weights + {kv / 1e9:.2f} GB of KV cache (inputs >> 126 MB L2); no explicit flush needed',
+                'l2': f'each step streams {L * per_layer / 1e9:.1f} GB of weights + {kv / 1e9:.2f} GB of KV cache (inputs >> 50 MB L2); no explicit flush needed',
                 'arithmetic': 'raw int4 nibbles x fp16 activations on the tensor pipe (mma.sync, exact products, fp32 accumulate), fp16 scale and zero applied once per '
                               'quantisation group on the fp32 accumulator, fp16 store; within 1e-3 of the reference kernel (tests/)',
             },
@@ -328,6 +347,7 @@ def run_decode(args):
                     'note': 'host token+position (pinned) -> H2D -> CUDA-graph decode step -> D2H fp16 logits, synchronised every step'},
             'gpu_launches': dec.launches_per_step() * steps,
             'roofline': None,
+            'gpu': gpu_identity(local),
             'clocks': clocks,
         }
         assert dec.launches_per_step() == 1, 'the persistent kernel must be the measured path'
@@ -335,21 +355,11 @@ def run_decode(args):
         line['roofline'] = {'bound': 'hbm', 'kernel': 'llama_decode_mega_kernel (persistent decode step: all quantized matvecs + attention + lm_head of a token)',
                             'achieved': step_bytes / t_step / 1e9 / (world if tp else 1), 'peak': peak, 'unit': 'GB/s',
                             'frac': step_bytes / t_step / 1e9 / peak / (world if tp else 1), 'peak_source': peak_src + (' per GPU' if tp else ''),
-                            'bytes_per_launch': step_bytes, 'us_per_launch': t_step * 1e6, 'frac_of_8TBs': step_bytes / t_step / 8e12,
-                            'traffic': NCU_TRAFFIC_BYTES.get(args.config), 'traffic_source': 'dram__bytes_read.sum + dram__bytes_write.sum, ncu --set full, profiles/'}
+                            'bytes_per_launch': step_bytes, 'us_per_launch': t_step * 1e6, 'traffic': None}
         if mlp is None and bits == 4 and not act and not tp:
             ach = kbytes / t_k / 1e9
             line['roofline']['standalone_fused_mlp'] = {'kernel': 'qmatvec_int4_kernel<dual> (standalone gptq_fused_mlp_fwd, timed alone over the layers\' distinct weights)',
                                                         'achieved': ach, 'frac': ach / peak, 'bytes_per_launch': kbytes, 'us_per_launch': t_k * 1e6}
-        ref_path = os.path.join(ROOT, 'profiles', 'r2_reference_triton_decode.json')
-        if args.config == '7b' and os.path.exists(ref_path):
-            try:
-                rt = json.loads(open(ref_path).readline())
-                line['reference_triton'] = {'tokens_per_s': rt['tokens_per_s'], 'ms_per_token': rt['ms_per_token'],
-                                            'source': 'profiles/r2_reference_triton_decode.json: the unmodified reference modules (Triton kernels) on a B200 of this pool, '
-                                                      'measured separately by tools/refshim/ref_decode_bench.py; not re-measured in this run'}
-            except (ValueError, KeyError):
-                pass
         if base is not None:
             line['cpu_baseline'] = base
         print(json.dumps(line))
@@ -359,7 +369,7 @@ def run_decode(args):
 
 def run_prefill(args):
     """BASELINE.json config 3: LLaMA-7B int4 g128 prefill, batch 32 x seq 2048 (M = 65536): a step = the quantized linears of one decoder
-    layer on the tcgen05 GEMM path (qkv, o, fused gate/up + SwiGLU, down); tokens/s counts the 32 layers' linears only."""
+    layer on the wgmma GEMM path (qkv, o, fused gate/up + SwiGLU, down); tokens/s counts the 32 layers' linears only."""
     from gptq_b200 import engine, ops
     dev = torch.device('cuda', int(os.environ.get('LOCAL_RANK', '0')))
     torch.cuda.set_device(dev)
@@ -369,28 +379,33 @@ def run_prefill(args):
     t4 = lambda w: (w.qweight, w.scales, w.qzeros, w.g_idx)
     x = torch.randn(M, H, device=dev, generator=gen).half()
 
-    def layer():
-        ops.matmul248(x, *t4(L['qkv']), 4, None, groupsize=GROUP)
-        ops.matmul248(x, *t4(L['o']), 4, None, groupsize=GROUP)
-        h = ops.fused_mlp(x, t4(L['gate']), t4(L['up']), 4, GROUP)
-        ops.matmul248(h, *t4(L['down']), 4, None, groupsize=GROUP)
+    outs = {}
 
-    steps, warm = max(1, min(args.steps, 20)), max(3, min(args.warmup, 5))
+    def layer():
+        outs['qkv'] = ops.matmul248(x, *t4(L['qkv']), 4, None, groupsize=GROUP)
+        outs['o'] = ops.matmul248(x, *t4(L['o']), 4, None, groupsize=GROUP)
+        outs['mlp'] = h = ops.fused_mlp(x, t4(L['gate']), t4(L['up']), 4, GROUP)
+        outs['down'] = ops.matmul248(h, *t4(L['down']), 4, None, groupsize=GROUP)
+
+    steps, warm = max(1, args.steps), max(3, min(args.warmup, 5))
     for _ in range(warm):
         layer()
     sampler = ClockSampler(dev.index)
     t = timed(layer, steps, False) / steps
     clocks = sampler.stop()
+    if args.dump_outputs:
+        rows = torch.randperm(M, generator=torch.Generator().manual_seed(0))[:DUMP_ROWS].sort().values.to(dev)
+        dump_outputs(args.dump_outputs, {k: v.index_select(0, rows) for k, v in outs.items()} | {'rows': rows})
     flops = 2 * M * (H * 3 * H + H * H + 2 * H * I + I * H)
-    _, burst, sustained, src = measured_peaks()
+    _, peak, src = datasheet_peaks()
     print(json.dumps({
-        'metric': 'prefill tokens/sec LLaMA-7B int4 g128 batch=32 seq=2048 (quantized linears, tcgen05 GEMM path)', 'value': M / (t * 32), 'unit': 'tokens/s', 'n_gpus': 1,
+        'metric': 'prefill tokens/sec LLaMA-7B int4 g128 batch=32 seq=2048 (quantized linears, wgmma GEMM path)', 'value': M / (t * 32), 'unit': 'tokens/s', 'n_gpus': 1,
         'steps': steps, 'warmup': warm, 'ms_per_step': t * 1e3, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f16', 'data': 'synthetic',
         'config': {'workload': 'LLaMA-7B int4 g128 prefill batch 32 x seq 2048 (M=65536): the 4 quantized linears of one decoder layer per step; tokens/s = M / (32 x step)',
-                   'l2': 'activations 0.5-1.4 GB per operand (>> 126 MB L2)'},
-        'gpu_launches': 4 * steps, 'clocks': clocks,
-        'roofline': {'bound': 'tensor', 'kernel': 'qgemm_tcgen05_kernel', 'achieved': flops / t / 1e12, 'peak': sustained, 'unit': 'TFLOP/s', 'frac': flops / t / 1e12 / sustained,
-                     'frac_of_burst': flops / t / 1e12 / burst, 'peak_source': src + ' (sustained cuBLAS bf16)', 'traffic': None},
+                   'l2': 'activations 0.5-1.4 GB per operand (>> 50 MB L2)'},
+        'gpu_launches': 4 * steps, 'gpu': gpu_identity(dev.index), 'clocks': clocks,
+        'roofline': {'bound': 'tensor', 'kernel': 'qgemm_wgmma_kernel', 'achieved': flops / t / 1e12, 'peak': peak, 'unit': 'TFLOP/s', 'frac': flops / t / 1e12 / peak,
+                     'peak_source': src + ', dense fp16', 'traffic': None},
     }))
 
 
@@ -401,6 +416,7 @@ def main():
     ap.add_argument('--warmup', type=int, default=10)
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--config', default='7b', choices=sorted(CONFIGS) + ['prefill'])
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None, help='write the last timed step\'s outputs as DIR/<name>.npy (float32)')
     args = ap.parse_args()
     if args.impl == 'reference':
         run_reference(args)

@@ -43,7 +43,7 @@ const char* gptq_strerror(int status) {
         case GPTQ_ERR_NULL: return "required pointer is NULL";
         case GPTQ_ERR_ALIGN: return "pointer or leading dimension is misaligned";
         case GPTQ_ERR_WORKSPACE: return "workspace too small (see gptq_qlinear_workspace_bytes)";
-        case GPTQ_ERR_CUDA: return "CUDA runtime error (launch failed; is this an sm_100a device?)";
+        case GPTQ_ERR_CUDA: return "CUDA runtime error (launch failed; is this an sm_90a device?)";
         case GPTQ_ERR_UNSUPPORTED: return "request not supported by this build";
     }
     return "unknown gptq status";

@@ -1,4 +1,4 @@
-// Shared device helpers for libgptq_b200 (sm_100a only).
+// Shared device helpers for libgptq_b200 (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -12,7 +12,7 @@
 
 namespace gptq {
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 __host__ __device__ constexpr int ceil_div(int a, int b) { return (a + b - 1) / b; }
 

@@ -1,6 +1,6 @@
 // Persistent decode step: ONE cooperative kernel per token (batch 1, int4 kernel-form layers; optionally one tensor-parallel shard).
 //
-// One CTA per SM (148 on B200), each with two consumer TEAMS of 8 warps and one producer warp per team.
+// One CTA per SM (132 on H100 SXM), each with two consumer TEAMS of 8 warps and one producer warp per team.
 // Everything a token reads from HBM -- packed weights with their scales/zeros, the KV cache, the fp16 lm_head --
 // is streamed by the producer warps through the TMA unit (cp.async.bulk.tensor / cp.async.bulk) into a per-team ring of 17 KB stages in
 // shared memory, in one fixed order per team for the whole token, so the producers run ahead across operations

@@ -1,6 +1,6 @@
 // Generic CUDA-core kernels: every bit width in {2,3,4,8}, arbitrary g_idx (act-order), any M.
 // They are the correctness backbone (and the only path for shapes the tuned kernels reject);
-// the tuned int4 matvec / tcgen05 GEMM live in their own files and are dispatched from capi.cu.
+// the tuned int4 matvec / wgmma GEMM live in their own files and are dispatched from capi.cu.
 //
 // Arithmetic follows matmul_248_kernel (quant/quant_linear.py:84-137 of the reference):
 //   W[k,n] = fp16( fp16(q[k,n] - (z[g_idx[k],n] + 1)) * s[g_idx[k],n] ),  out = fp16( sum_k fp32(x*W) ) (+ bias in fp16)

@@ -40,7 +40,7 @@ size_t skinny_workspace_bytes(int M, int K, int N, bool dual);
 bool skinny_supported(const QLinearArgs& a);
 cudaError_t launch_qlinear_skinny(const QLinearArgs& a, bool pdl);
 
-// qgemm_tcgen05.cu -- batched (prefill) int4 GEMM on tcgen05 tensor cores, M > 8
+// qgemm_wgmma.cu -- batched (prefill) int4 GEMM on wgmma tensor cores, M > 8
 bool gemm_tc_supported(const QLinearArgs& a);
 cudaError_t launch_qlinear_gemm_tc(const QLinearArgs& a);
 

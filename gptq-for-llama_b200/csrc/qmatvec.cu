@@ -5,7 +5,7 @@
 //
 // Design (HBM-bound: 0.53 B/weight, ~2.8 issue slots per weight at 100 % of HBM):
 //  * Work = units of 4 packed rows (32 k) x 256 columns (4 KB of qweight, 1 KB contiguous per row).
-//    Units are numbered slab-major (slab = 256 columns) and split evenly over min(296, units) CTAs
+//    Units are numbered slab-major (slab = 256 columns) and split evenly over min(2 x 132 SMs, units) CTAs
 //    ("stream-K"): every SM streams the same number of bytes whatever the layer shape.
 //  * Each of the 8 warps owns a 32-column stripe of the slab and walks the k-steps of its CTA's range.
 //    Weights are staged global -> shared memory by 16-byte asynchronous copies (cp.async / LDGSTS, L1 bypass):

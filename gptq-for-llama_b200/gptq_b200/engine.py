@@ -1,7 +1,7 @@
 """Decode engine host side: a GPTQ LLaMA decoded token by token on a static KV cache, the whole step
 captured once in a CUDA graph (gptq_llama_decode_step in include/gptq_b200.h).
 
-This is the B200-native replacement for the reference's per-token loop (llama.py:419-433 /
+This is the H100-native replacement for the reference's per-token loop (llama.py:419-433 /
 model.generate in llama_inference.py:120): ~480 Python-dispatched launches and an O(n) torch.cat of
 the KV cache per token become one graph replay.  torch is used for device memory, streams and graph
 capture only.
@@ -281,7 +281,7 @@ class LlamaDecoder:
     @torch.no_grad()
     def prefill(self, prompt_ids):
         """Batched pass over the first len(prompt) - 1 prompt tokens that fills the static KV cache (batch 1): per layer the quantized linears on
-        the tcgen05 GEMM path (gptq_qlinear_fwd / gptq_fused_mlp_fwd with M = tokens), the RoPE and RMSNorm kernels, torch SDPA for the causal
+        the wgmma GEMM path (gptq_qlinear_fwd / gptq_fused_mlp_fwd with M = tokens), the RoPE and RMSNorm kernels, torch SDPA for the causal
         attention (as the reference's QuantLlamaAttention does, quant/fused_attn.py:154-155); keys are cached after RoPE.  The LAST prompt token then
         goes through the decode step like every generated one (it produces the first logits).  Returns the number of cached positions."""
         assert self.batch == 1 and self.tp is None
@@ -306,7 +306,7 @@ class LlamaDecoder:
 
     @torch.no_grad()
     def generate(self, prompt_ids, max_new_tokens, prefill=True):
-        """Greedy decode (batch 1).  One engine, two phases: the prompt is prefilled in one batched pass (tcgen05 GEMM path) into the static KV
+        """Greedy decode (batch 1).  One engine, two phases: the prompt is prefilled in one batched pass (wgmma GEMM path) into the static KV
         cache, then the persistent decode kernel takes over token by token; prefill=False feeds the prompt through the decode step instead."""
         assert self.batch == 1
         if len(prompt_ids) < 1 or len(prompt_ids) + max_new_tokens > self.max_seq + 1:

@@ -224,7 +224,7 @@ def unpack_qzeros(qzeros, bits):
 
 
 def kernel_form(qweight, scales, qzeros, g_idx, bits, groupsize, allow_perm=True):
-    """Load-time derived buffers that let the tuned int4 kernels (matvec, tcgen05 GEMM, persistent decode kernel)
+    """Load-time derived buffers that let the tuned int4 kernels (matvec, wgmma GEMM, persistent decode kernel)
     serve a layer they would otherwise leave to the generic kernel.  The stored tensors are not touched.
 
     * act-order (arbitrary g_idx, gptq.py:210-216) with equal-sized groups: the packed rows are regrouped so that every

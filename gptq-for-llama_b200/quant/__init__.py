@@ -1,5 +1,5 @@
 """Drop-in replacement for the reference's ``quant`` package (quant/__init__.py:1-5 of
-qwopqwop200/GPTQ-for-LLaMa, triton branch), backed by hand-written sm_100a CUDA in
+qwopqwop200/GPTQ-for-LLaMa, triton branch), backed by hand-written sm_90a CUDA in
 libgptq_b200.so instead of Triton.  Same public names; ``make_quant`` is the older alias of
 ``make_quant_linear``.
 """

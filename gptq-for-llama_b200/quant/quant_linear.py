@@ -1,4 +1,4 @@
-"""QuantLinear: packed-weight linear layer on hand-written sm_100a CUDA.
+"""QuantLinear: packed-weight linear layer on hand-written sm_90a CUDA.
 
 Mirrors the module surface of the reference's quant/quant_linear.py (QuantLinear :304-377,
 matmul248 :263-269, transpose_matmul248 :272-279, QuantLinearFunction :282-301,
@@ -6,7 +6,7 @@ make_quant_linear :380-390, autotune_warmup_linear :393-423): same constructor, 
 shapes and dtypes (so existing .pt/.safetensors checkpoints load), same exceptions.
 Differences, all additive: 3-bit is accepted (the reference commit raises for it), ``make_quant``
 aliases ``make_quant_linear``, bias is fused into the kernel epilogue, and the autotune warm-up
-is a cheap load-time preparation pass because dispatch is static (matvec vs tcgen05 GEMM by M).
+is a cheap load-time preparation pass because dispatch is static (matvec vs wgmma GEMM by M).
 """
 import math
 

@@ -1,5 +1,5 @@
 /*
- * gptq_b200.h -- C ABI of libgptq_b200.so: the B200 (sm_100a) implementation of the
+ * gptq_b200.h -- C ABI of libgptq_b200.so: the H100 (sm_90a) implementation of the
  * GPTQ-for-LLaMa quantized-linear inference hot path.
  *
  * The reference (qwopqwop200/GPTQ-for-LLaMa, triton branch) has no FFI layer: its boundary is

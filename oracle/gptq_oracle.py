@@ -7,7 +7,7 @@ no CPU fallback.
 
 It is a plain numpy / torch-CPU restatement of the arithmetic of the reference's
 Triton kernels (which cannot run without a GPU) and of its CPU ``pack()``.
-Every function cites the reference lines (relative to /root/reference) it follows.
+Every function cites the reference lines (relative to the reference checkout) it follows.
 
 Pinning status
 --------------

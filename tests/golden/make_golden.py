@@ -1,9 +1,9 @@
-"""Generate the golden pack() fixtures by running the UNMODIFIED reference in the build container.
+"""Generate the golden pack() fixtures by running the UNMODIFIED reference.
 
-    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py REFERENCE_CHECKOUT
 
-Imports ``quant`` from /root/reference (read-only; it does not exist on the GPU box, so
-the outputs are committed as small .npz files next to this script).  For every case:
+Imports ``quant`` from a checkout of the reference (the tests do not need it: the outputs are
+committed as small .npz files next to this script).  For every case:
 random fp weights -> per-group ``Quantizer`` (quant/quantizer.py, configured as in
 gptq.py:185-194) -> on-grid weights Q -> the reference's own ``QuantLinear.pack``
 (quant/quant_linear.py:325-371).  Stored: the inputs and the packed tensors the
@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 sys.dont_write_bytecode = True
-sys.path.insert(0, '/root/reference')
+sys.path.insert(0, sys.argv[1])
 import quant as refquant  # noqa: E402  (the reference package)
 import torch.nn as nn  # noqa: E402
 

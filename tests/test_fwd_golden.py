@@ -1,5 +1,5 @@
 """The forward arithmetic against OUTPUTS OF THE REFERENCE'S OWN TRITON KERNELS (tests/golden/fwd_ref_triton.npz, generated on a
-B200 from the unmodified reference by tests/golden/make_fwd_golden.py): matmul248 (+bias), the fused SwiGLU MLP kernel,
+GPU from the unmodified reference by tests/golden/make_fwd_golden.py): matmul248 (+bias), the fused SwiGLU MLP kernel,
 triton_rotate_half_ and TritonLlamaRMSNorm.
 
   * CPU: the oracle (oracle/gptq_oracle.py, and its C restatement) reproduces the reference outputs within 1e-3 -- this is what
@@ -83,7 +83,7 @@ def test_cuda_matmul248_matches_reference_triton():
         qw, sc, qz, gi, bias = _fixture_tensors(fx)
         x = G.x_for(G.name_seed(name), M, int(fx['K']))
         out = ops.matmul248(x.to(dev), qw.to(dev), sc.to(dev), qz.to(dev), gi.to(dev), int(fx['bits']), bias=bias.to(dev) if bias is not None else None)
-        assert_rel_close(out, ref(f'pack/{name}/M{M}'), rel=1e-3 if M <= 8 else 2e-3, what=f'pack/{name}/M{M}')  # M > 8: tcgen05 accumulation is not IEEE per add
+        assert_rel_close(out, ref(f'pack/{name}/M{M}'), rel=1e-3 if M <= 8 else 2e-3, what=f'pack/{name}/M{M}')  # M > 8: tensor-core accumulation is not IEEE per add
     for name, K, N, bits, gs, act, seed, Ms in G.RANDOM_CASES:
         qw, sc, qz, gi, _ = O.random_packed(K, N, bits, gs, seed=seed, act_order=act)
         for M in Ms:

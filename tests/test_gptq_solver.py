@@ -1,95 +1,62 @@
-"""SURVEY.md 8(f) rank 4: the GPTQ solver (`gptq.GPTQ`, drop-in for the reference module) against the reference's own `gptq.py`, imported
-unmodified (its table-printing dependency `texttable` and the SNR helper it pulls from `utils` are stubbed: neither touches the result), on
-the same layers and calibration batches: scales, zeros, g_idx and the on-grid weights must agree.  CPU, runs where the reference exists."""
-import importlib
+"""SURVEY.md 8(f) rank 4: the GPTQ solver (`gptq.GPTQ`, drop-in for the reference module) against what the reference's own `gptq.py`
+computes on the same layers and calibration batches (stored in tests/golden/solver_ref.npz by tests/golden/make_solver_golden.py):
+scales, zeros, g_idx and the on-grid weights must agree."""
+import importlib.util
 import os
 import sys
-import types
 
+import numpy as np
 import pytest
 import torch
 import torch.nn as nn
 
-REF = '/root/reference'
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(REF, 'gptq.py')), reason='reference checkout not present')
+HERE = os.path.dirname(os.path.abspath(__file__))
+spec = importlib.util.spec_from_file_location('make_solver_golden', os.path.join(HERE, 'golden', 'make_solver_golden.py'))
+G = importlib.util.module_from_spec(spec)
+spec.loader.exec_module(G)
+REF = dict(np.load(G.OUT))
 
 
-def _reference_gptq():
-    import quant  # this repo's package: its Quantizer reproduces the reference's bit for bit (tests/test_host_modules.py)
-    import utils as ours
-    tt = types.ModuleType('texttable')
-
-    class Texttable:  # only used to print one line per layer
-        def header(self, *a): pass
-        def set_cols_dtype(self, *a): pass
-        def add_row(self, *a): pass
-        def draw(self): return 'a\nb\nc'
-    tt.Texttable = Texttable
-    shim = types.ModuleType('utils')
-    shim.find_layers, shim.DEV = ours.find_layers, ours.DEV
-    shim.torch_snr_error = lambda a, b, reduction='mean': ((a - b)**2 / (b**2 + 1e-12)).mean()
-    saved = {k: sys.modules.get(k) for k in ('texttable', 'utils', 'gptq')}
-    sys.modules.update(texttable=tt, utils=shim)
-    sys.modules.pop('gptq', None)
-    sys.dont_write_bytecode = True
-    sys.path.insert(0, REF)
-    try:
-        ref = importlib.import_module('gptq')
-        assert ref.__file__.startswith(REF)
-    finally:
-        sys.path.remove(REF)
-        for k, v in saved.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
-    sync = torch.cuda.synchronize
-    torch.cuda.synchronize = lambda *a, **k: None  # the reference synchronises unconditionally (gptq.py:205); there is no GPU here
-    return ref, sync
-
-
-@pytest.mark.parametrize('K,N,bits,groupsize,actorder', [(256, 96, 4, 64, False), (256, 96, 4, 128, True), (192, 64, 3, -1, False), (256, 64, 8, 128, False),
-                                                      (256, 96, 2, 32, True)])
+@pytest.mark.parametrize('K,N,bits,groupsize,actorder', G.CASES)
 def test_solver_matches_reference_gptq(K, N, bits, groupsize, actorder):
-    ref_mod, sync = _reference_gptq()
+    import gptq as ours_mod
+    assert 'gptq-for-llama_b200' in ours_mod.__file__
+    n = G.case_name(K, N, bits, groupsize, actorder)
+    ga, sa, za, ea = (torch.from_numpy(REF[f'{n}/{k}']) for k in ('g_idx', 'scale', 'zero', 'err'))
+    ea = float(ea)
+    Wa = sa[:, ga.long()] * (torch.from_numpy(REF[f'{n}/codes']).float() - za[:, ga.long()])  # the reference's on-grid weights, exactly
+    sync = torch.cuda.synchronize
+    torch.cuda.synchronize = lambda *a, **k: None  # the solver mirrors the reference's unconditional synchronise (gptq.py:205); there may be no GPU
     try:
-        import gptq as ours_mod
-        assert 'gptq-for-llama_b200' in ours_mod.__file__
-        g = torch.Generator().manual_seed(K + N + bits)
-        lin_a, lin_b = nn.Linear(K, N, bias=True), nn.Linear(K, N, bias=True)
-        lin_a.weight.data = torch.randn(N, K, generator=g) * 0.05
-        lin_b.load_state_dict(lin_a.state_dict())
-        # correlated calibration inputs with a few dominant (and one dead) features, so that act-order actually reorders
-        mix = torch.randn(K, K, generator=g) * 0.2 + torch.eye(K)
-        gain = torch.rand(K, generator=g) * 3 + 0.1
-        gain[5] = 0.0
-        batches = [(torch.randn(2, 24, K, generator=g) @ mix) * gain for _ in range(3)]
-        a, b = ref_mod.GPTQ(lin_a), ours_mod.GPTQ(lin_b)
-        for s in (a, b):
-            s.quantizer.configure(bits, perchannel=True, sym=False, mse=False)
+        weight, batches = G.make_inputs(K, N, bits)
+        lin_b = nn.Linear(K, N, bias=True)
+        lin_b.weight.data = weight.clone()
+        b = ours_mod.GPTQ(lin_b)
+        b.quantizer.configure(bits, perchannel=True, sym=False, mse=False)
         for x in batches:
-            a.add_batch(x, None)
             b.add_batch(x, None)
-        assert torch.allclose(a.H, b.H, rtol=1e-5, atol=1e-6)
-        sa, za, ga, ea = a.fasterquant(blocksize=128, percdamp=.01, groupsize=groupsize, actorder=actorder, name='t')
+        r, c = G.h_sample(K)
+        assert torch.allclose(torch.diagonal(b.H), torch.from_numpy(REF[f'{n}/H_diag']), rtol=1e-5, atol=1e-6)
+        assert torch.allclose(b.H[r, c], torch.from_numpy(REF[f'{n}/H_sample']), rtol=1e-5, atol=1e-6)
         sb, zb, gb, eb = b.fasterquant(blocksize=128, percdamp=.01, groupsize=groupsize, actorder=actorder, name='t')
-        assert torch.equal(ga.cpu(), gb.cpu()) and sa.shape == sb.shape and za.shape == zb.shape
-        if actorder:
-            assert not torch.equal(gb.cpu(), (torch.arange(K) // (groupsize if groupsize != -1 else K)).int())  # the fixture really exercises the permutation
-        # the same algorithm in fp32 with a different operation order: scales / zeros agree closely, a handful of weights may land on a neighbouring grid point
-        assert torch.allclose(sa, sb, rtol=1e-4, atol=1e-7)
-        assert (za != zb).float().mean().item() < 0.01
-        Wa, Wb = lin_a.weight.data, lin_b.weight.data
-        step = sb.mean().item()
-        differing = ((Wa - Wb).abs() > 0.5 * step).float().mean().item()
-        assert differing < 0.01, f'{differing:.2%} of the quantised weights differ'
-        assert abs(ea - eb) <= 0.02 * abs(ea) + 1e-9
-        # and the point of the exercise: the layer output error stays small and comparable
-        x = batches[0].reshape(-1, K)
-        assert torch.allclose(x @ Wa.t(), x @ Wb.t(), rtol=0, atol=0.05 * (x @ Wa.t()).abs().mean().item() + 1e-6)
     finally:
         torch.cuda.synchronize = sync
-        sys.modules.pop('gptq', None)
+    assert torch.equal(ga, gb.cpu().to(ga.dtype)) and sa.shape == sb.shape and za.shape == zb.shape
+    if actorder:
+        assert not torch.equal(gb.cpu(), (torch.arange(K) // (groupsize if groupsize != -1 else K)).int())  # the fixture really exercises the permutation
+    # the same algorithm in fp32 with a different operation order: scales / zeros agree closely, a handful of weights may land on a neighbouring grid point
+    sb, zb = sb.cpu(), zb.cpu()
+    assert torch.allclose(sa, sb, rtol=1e-4, atol=1e-7)
+    assert (za != zb).float().mean().item() < 0.01
+    Wb = lin_b.weight.data
+    step = sb.mean().item()
+    differing = ((Wa - Wb).abs() > 0.5 * step).float().mean().item()
+    assert differing < 0.01, f'{differing:.2%} of the quantised weights differ'
+    assert abs(ea - eb) <= 0.02 * abs(ea) + 1e-9
+    # and the point of the exercise: the layer output error stays small and comparable
+    x = batches[0].reshape(-1, K)
+    assert torch.allclose(x @ Wa.t(), x @ Wb.t(), rtol=0, atol=0.05 * (x @ Wa.t()).abs().mean().item() + 1e-6)
+    sys.modules.pop('gptq', None)
 
 
 def test_quantize_linears_drives_a_block_with_bias_layers():

@@ -143,7 +143,7 @@ def test_host_rejects_positions_and_tokens_outside_the_cache_and_vocabulary():
 
 @pytest.mark.parametrize('size', ['tiny', 'tiny256'])
 def test_prefill_then_decode_matches_token_by_token(size):
-    """One engine, two phases: the batched prefill (tcgen05 GEMM path + SDPA, filling the static KV cache) followed by the decode kernel gives the
+    """One engine, two phases: the batched prefill (wgmma GEMM path + SDPA, filling the static KV cache) followed by the decode kernel gives the
     same cache rows and the same next-token logits as feeding the prompt token by token through the decode step."""
     from gptq_b200 import engine
     dec = engine.synthetic_llama(size, bits=4, groupsize=64, vocab=300, seed=5, max_seq=96)

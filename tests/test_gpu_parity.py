@@ -175,10 +175,10 @@ def test_error_mapping_on_device(ops):
         ops.matmul248(torch.zeros(1, 128).half(), qw, s, qz, g, 4, 15)
 
 
-# ----------------------------------------------------------------------------- batched (prefill) path: tcgen05 GEMM
+# ----------------------------------------------------------------------------- batched (prefill) path: wgmma GEMM
 @pytest.mark.parametrize('M,K,N,gs', [(16, 512, 256, 128), (100, 1024, 384, 64), (128, 256, 128, 128), (300, 2048, 512, 128), (129, 128, 128, 64)])
 def test_prefill_gemm_vs_oracle(ops, M, K, N, gs):
-    """M > 8, int4, no act-order: tcgen05 GEMM (qgemm_tcgen05.cu) against the CPU oracle."""
+    """M > 8, int4, no act-order: wgmma GEMM (qgemm_wgmma.cu) against the CPU oracle."""
     qw, s, qz, g, b = O.random_packed(K, N, 4, gs, seed=M + K, bias=(M % 2 == 0))
     x = torch.randn(M, K, generator=torch.Generator().manual_seed(M)).half()
     ref = O.qlinear_fwd(x, qw, s, qz, g, 4, b)
@@ -188,7 +188,7 @@ def test_prefill_gemm_vs_oracle(ops, M, K, N, gs):
 
 
 def test_prefill_gemm_full_size_matches_dequant_matmul(ops):
-    """LLaMA-7B layer size, M = 512: tcgen05 GEMM == fp32 matmul over the device-dequantised weight; exact homogeneity."""
+    """LLaMA-7B layer size, M = 512: wgmma GEMM == fp32 matmul over the device-dequantised weight; exact homogeneity."""
     K, N, M = 4096, 4096, 512
     qw, s, qz, g, _ = cuda(*O.random_packed(K, N, 4, 128, seed=3))
     x = torch.randn(M, K, generator=torch.Generator().manual_seed(0)).half().cuda()
@@ -204,7 +204,7 @@ def test_prefill_gemm_full_size_matches_dequant_matmul(ops):
 
 @pytest.mark.parametrize('M', [24, 200])
 def test_prefill_fused_mlp_vs_oracle(ops, M):
-    """Fused SwiGLU MLP at M > 8: dual-accumulator tcgen05 GEMM, silu*mul on the fp32 accumulators in the epilogue."""
+    """Fused SwiGLU MLP at M > 8: dual-accumulator wgmma GEMM, silu*mul on the fp32 accumulators in the epilogue."""
     K, N, gs = 512, 384, 128
     gate = O.random_packed(K, N, 4, gs, seed=1)[:4]
     up = O.random_packed(K, N, 4, gs, seed=2)[:4]

@@ -1,7 +1,7 @@
-// Grid-barrier latency on B200 under HBM load: one CTA per SM, thread 0 of every CTA synchronises ROUNDS times; the other
+// Grid-barrier latency on H100 under HBM load: one CTA per SM, thread 0 of every CTA synchronises ROUNDS times; the other
 // warps stream a large buffer (background traffic like the decode kernel's weight stream).  Per variant: time from the LAST
 // arrival to the median / last release, in ns (globaltimer).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o barrier barrier.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o barrier barrier.cu
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
@@ -30,10 +30,10 @@ __global__ void __launch_bounds__(576, 1) k_bar(unsigned long long* bar, unsigne
 #pragma unroll
             for (int u = 0; u < 8; ++u) {
                 uint4 v;
-                asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(big + (i + u * 544 * 148) % big_n));
+                asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(big + (i + u * 544 * 132) % big_n));
                 acc.x ^= v.x; acc.y ^= v.y; acc.z ^= v.z; acc.w ^= v.w;
             }
-            i = (i + 8ull * 544 * 148 + 1) % big_n;
+            i = (i + 8ull * 544 * 132 + 1) % big_n;
         }
         if (acc.x == 0x12345) sink[tid] = (float)acc.y;
         return;

@@ -1,6 +1,6 @@
-// Microbenchmark of the decode matvec's per-stage inner loop on sm_100a: 16 warps per CTA (4 per scheduler), one CTA per SM,
+// Microbenchmark of the decode matvec's per-stage inner loop on sm_90a: 16 warps per CTA (4 per scheduler), one CTA per SM,
 // every warp runs `iters` stages of 4 k-steps from shared memory.  Prints cycles per stage per warp for a few instruction mixes.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o loop loop.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o loop loop.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -203,7 +203,7 @@ void run(const char* name, float* out, long long* cyc, int nb) {
 }
 
 int main() {
-    int nb = 148;
+    int nb = 132;
     cudaDeviceProp pr;
     cudaGetDeviceProperties(&pr, 0);
     nb = pr.multiProcessorCount;

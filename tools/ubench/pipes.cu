@@ -1,4 +1,4 @@
-// Issue-rate / latency microbenchmark for the instruction mix of the int4 decode matvec on sm_100a:
+// Issue-rate / latency microbenchmark for the instruction mix of the int4 decode matvec on sm_90a:
 // legacy HMMA.16816 (mma.sync), HFMA2, LOP3.  Prints cycles per warp-instruction per SM sub-partition.
 #include <cstdio>
 #include <cstdint>
@@ -112,14 +112,14 @@ __global__ void k_mix(float* out, long long* cyc, int iters) {
 
 template <typename K>
 void run_mix(const char* name, K kern, int threads, int iters, float* out, long long* cyc) {
-    kern<<<148, threads>>>(out, cyc, iters);
-    kern<<<148, threads>>>(out, cyc, iters);
+    kern<<<132, threads>>>(out, cyc, iters);
+    kern<<<132, threads>>>(out, cyc, iters);
     cudaDeviceSynchronize();
-    long long h[148];
+    long long h[132];
     cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
     double avg = 0;
-    for (int i = 0; i < 148; ++i) avg += (double)h[i];
-    avg /= 148;
+    for (int i = 0; i < 132; ++i) avg += (double)h[i];
+    avg /= 132;
     const int wps = threads / 128;
     printf("MIX %-34s warps/SMSP %d: %.1f cycles per iteration per warp -> %.1f per SMSP per warp-iteration (%s)\n", name, wps, avg / iters, avg / iters / wps,
            cudaGetErrorString(cudaGetLastError()));
@@ -127,14 +127,14 @@ void run_mix(const char* name, K kern, int threads, int iters, float* out, long 
 
 template <typename K>
 void run(const char* name, K kern, int chains, int threads, int iters, float* out, long long* cyc) {
-    kern<<<148, threads>>>(out, cyc, iters);
-    kern<<<148, threads>>>(out, cyc, iters);
+    kern<<<132, threads>>>(out, cyc, iters);
+    kern<<<132, threads>>>(out, cyc, iters);
     cudaDeviceSynchronize();
-    long long h[148];
+    long long h[132];
     cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
     double avg = 0;
-    for (int i = 0; i < 148; ++i) avg += (double)h[i];
-    avg /= 148;
+    for (int i = 0; i < 132; ++i) avg += (double)h[i];
+    avg /= 132;
     const int warps_per_smsp = threads / 32 / 4 > 0 ? threads / 32 / 4 : 1;
     const double per_warp_instr = avg / ((double)iters * chains);
     printf("%-8s chains %d warps/SMSP %d%s: %.2f cycles per warp-instr per warp -> %.2f cycles per instr per SMSP (%s)\n", name, chains, warps_per_smsp,
@@ -144,8 +144,8 @@ void run(const char* name, K kern, int chains, int threads, int iters, float* ou
 int main() {
     float* out;
     long long* cyc;
-    cudaMalloc(&out, 148 * 1024 * 4);
-    cudaMalloc(&cyc, 148 * 8);
+    cudaMalloc(&out, 132 * 1024 * 4);
+    cudaMalloc(&cyc, 132 * 8);
     const int it = 4096;
     run("HMMA", k_hmma<1>, 1, 32, it, out, cyc);   // latency (1 dependent chain, 1 warp)
     run("HMMA", k_hmma<2>, 2, 32, it, out, cyc);
