@@ -347,7 +347,7 @@ ScratchLayout scratch_layout(const gptq_llama_model& m, int batch, int max_seq) 
     ws = max(ws, skinny_workspace_bytes(batch, m.intermediate, m.hidden, false));
     L.ws_bytes = ws;
     L.ws = take(ws);
-    L.mega = take(mega_scratch_bytes(m, max_seq));
+    L.mega = take(mega_scratch_bytes(m, batch, max_seq));
     L.total = off;
     return L;
 }

@@ -1,4 +1,4 @@
-// Persistent decode step: ONE cooperative kernel per token (batch 1, int4 kernel-form layers; optionally one tensor-parallel shard).
+// Persistent decode step: ONE cooperative kernel per token (batch 1 to 8, int4 kernel-form layers; at batch 1 optionally one tensor-parallel shard).
 //
 // One CTA per SM (132 on H100 SXM), each with two consumer TEAMS of 8 warps and one producer warp per team.
 // Everything a token reads from HBM -- packed weights with their scales/zeros, the KV cache, the fp16 lm_head --
@@ -32,6 +32,12 @@
 // rounds to fp16 exactly where the reference rounds (a QuantLinear output is fp16); each vector is re-zeroed
 // one operation after its last reader.  Only the fp32 summation order of those partials is unordered.
 // Tensor parallelism (gptq_llama_tp): the o_proj / down_proj sums also go to the peer GPUs' accumulators (NVLink, see MegaParams).
+//
+// Batch B = 2..8 (the BATCH instantiation): the eight columns of the B operand carry up to eight DIFFERENT sequences (lane group g
+// reads sequence min(g, B - 1)), so one weight stream, one dequantisation and one HMMA per packed word serve the whole batch.  Every
+// per-sequence vector (residual stream, accumulators, staged x and its step sums, RoPE angles, logits) gets a [B] dimension; the
+// attention teams are dealt to (sequence, head) pairs in proportion to each sequence's context (seq_teams).  Batch 1 is the
+// !BATCH instantiation, whose code is the single-sequence kernel unchanged.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
@@ -64,6 +70,7 @@ constexpr int kMaxLayers = 80;
 constexpr int kMaxStages = 8;
 constexpr int kTeamScratch = 4224;     // per-team scratch (attention merge buffers / lm_head partials)
 constexpr int kLmStageBytes = 16384;   // lm_head bytes per stage (whole rows)
+constexpr int kMaxBatch = 8;           // sequences of one step (the columns of the mma B operand)
 
 #ifdef GPTQ_DQ_EXACT_INT
 constexpr bool kSubnormal = false;
@@ -167,6 +174,10 @@ struct MegaParams {
     unsigned long long* xbar_peer[kMaxTP];
     LayerDesc layers[kMaxLayers];
     CUtensorMap tmaps[6];  // [class]: 16-row boxes (a full stage), [3 + class]: 4-row boxes (one k-step)
+    // BATCH instantiation only: sequences of the step, and halves between the sequences' rows of the staged x (H + 32: a stride of
+    // 64 mod 128 bytes puts the two lane groups of a quarter-warp on different banks).  Per-sequence vectors are [batch][n] with
+    // n = H, 3 Hq, I, V or 128 (rope_cs); resid, acc_* and rope_cs are sized for the batch.
+    int batch, xs_stride;
 };
 
 // ---- work split ------------------------------------------------------------------------------------------------
@@ -210,6 +221,51 @@ __device__ __forceinline__ int stage_steps(int gpos, int gs_steps, int left) { r
 
 // position of this step, clamped to the cache (the host rejects pos >= max_seq; the kernel must not write outside)
 __device__ __forceinline__ int step_pos(const MegaParams& p) { return min(max(p.positions[0], 0), p.max_seq - 1); }
+__device__ __forceinline__ int step_pos(const MegaParams& p, int s) { return min(max(p.positions[s], 0), p.max_seq - 1); }
+
+// Batched attention: sequence s is served by teams [first, first + count): n_heads teams plus a share of the other nb - batch * n_heads
+// teams in proportion to its 32-key units (cumulative rounding: the shares add up to nb exactly).  Inside a sequence the teams are
+// dealt to its heads as in batch 1 (attn_range / head_teams with count teams).  mega_plan guarantees batch * n_heads <= nb.
+__device__ __forceinline__ HeadTeams seq_teams(const MegaParams& p, int s, unsigned nb) {
+    int before = 0, mine = 0, tot = 0;
+#pragma unroll 1
+    for (int i = 0; i < p.batch; ++i) {
+        const int units = step_pos(p, i) / kKeysPerUnit + 1;
+        before += i < s ? units : 0;
+        mine = i == s ? units : mine;
+        tot += units;
+    }
+    const long long extra = (long long)nb - (long long)p.batch * p.n_heads;
+    HeadTeams h;
+    h.first = s * p.n_heads + (int)(extra * before / tot);
+    h.count = (s + 1) * p.n_heads + (int)(extra * (before + mine) / tot) - h.first;
+    return h;
+}
+// sequence of team T and that sequence's teams
+__device__ __forceinline__ int team_seq(const MegaParams& p, unsigned T, unsigned nb, HeadTeams& st) {
+    int s = 0;
+#pragma unroll 1
+    for (;; ++s) {
+        st = seq_teams(p, s, nb);
+        if ((int)T < st.first + st.count || s == p.batch - 1) return s;
+    }
+}
+// (sequence, head, unit range [b0, b1)) of team T; pos = that sequence's position, Tlen = pos + 1 keys
+template <bool BATCH>
+__device__ __forceinline__ int attn_work(const MegaParams& p, unsigned T, unsigned nb, int& pos, int& Tlen, int& head, int& b0, int& b1) {
+    int s = 0;
+    HeadTeams st{0, (int)nb};
+    if constexpr (BATCH) {
+        s = team_seq(p, T, nb, st);
+        pos = step_pos(p, s);
+    } else {
+        pos = step_pos(p);
+    }
+    Tlen = pos + 1;
+    const int upb = (Tlen + kKeysPerUnit - 1) / kKeysPerUnit;
+    attn_range(T - st.first, p.n_heads, st.count, upb, head, b0, b1);
+    return s;
+}
 
 // ---- team / CTA synchronisation ------------------------------------------------------------------------------------
 __device__ __forceinline__ void team_sync(int team) { asm volatile("bar.sync %0, 256;" ::"r"(team + 1) : "memory"); }
@@ -290,17 +346,16 @@ __device__ void produce_matvec(ProdRing& r, const MegaParams& p, const MatDesc* 
     }
 }
 
+template <bool BATCH>
 __device__ void produce_kv(ProdRing& r, const MegaParams& p, int layer, unsigned T, unsigned nb) {
-    const int Tlen = step_pos(p) + 1;
-    const int upb = (Tlen + kKeysPerUnit - 1) / kKeysPerUnit;
-    int head, b, b1;
-    attn_range(T, p.n_heads, nb, upb, head, b, b1);
+    int pos, Tlen, head, b, b1;
+    const int seq = attn_work<BATCH>(p, T, nb, pos, Tlen, head, b, b1);
     const __half* kc = p.k_cache + layer * p.layer_stride;
     const __half* vc = p.v_cache + layer * p.layer_stride;
 #pragma unroll 1
     for (; b < b1; ++b) {
         const int nrows = min(kKeysPerUnit, Tlen - b * kKeysPerUnit);
-        const size_t off = ((size_t)head * p.max_seq + (size_t)b * kKeysPerUnit) * kHD;
+        const size_t off = ((size_t)(seq * p.n_heads + head) * p.max_seq + (size_t)b * kKeysPerUnit) * kHD;
         uint32_t bar;
         const uint32_t dst = prod_acquire(r, bar);
         mbar_expect_tx(bar, nrows * 512);
@@ -327,6 +382,7 @@ __device__ void produce_lm_head(ProdRing& r, const MegaParams& p, unsigned T, un
     }
 }
 
+template <bool BATCH>
 __device__ void producer_loop(const MegaParams& p, ProdRing r, unsigned T, unsigned nb) {
 #pragma unroll 1
     for (int l = 0; l < p.n_layers; ++l) {
@@ -335,7 +391,7 @@ __device__ void producer_loop(const MegaParams& p, ProdRing r, unsigned T, unsig
             const MatDesc* const md[1] = {&L.qkv};
             produce_matvec<1>(r, p, md, p.H, 3 * p.Hq, T, nb);
         }
-        produce_kv(r, p, l, T, nb);
+        produce_kv<BATCH>(r, p, l, T, nb);
         {
             const MatDesc* const md[1] = {&L.o};
             produce_matvec<1>(r, p, md, p.Hq, p.H, T, nb);
@@ -643,6 +699,39 @@ struct TeamCtx {
     uint8_t* scratch;          // kTeamScratch bytes
 };
 
+// softmax merge of dimension d of the partial records of teams [ht.first, ht.first + ht.count), NB records per round trip
+template <int NB>
+__device__ __forceinline__ float merge_records(const MegaParams& p, const HeadTeams& ht, int d) {
+    float M = -INFINITY, Ls = 0.f, O = 0.f;
+#pragma unroll 1
+    for (int ib = 0; ib < ht.count; ib += NB) {
+        float mv[NB], lv[NB], ov[NB];
+#pragma unroll
+        for (int i = 0; i < NB; ++i) {  // all loads of the batch are in flight together
+            const bool on = ib + i < ht.count;
+            const float* rc = p.part + (size_t)(ht.first + (on ? ib + i : 0)) * kRec;
+            const float m = ld_cg(rc), l = ld_cg(rc + 1), o = ld_cg(rc + 4 + d);
+            mv[i] = on ? m : -INFINITY;
+            lv[i] = on ? l : 0.f;
+            ov[i] = on ? o : 0.f;
+        }
+        float Mb = M;
+#pragma unroll
+        for (int i = 0; i < NB; ++i) Mb = fmaxf(Mb, mv[i]);
+        const float w0 = (M == -INFINITY) ? 0.f : expf(M - Mb);
+        Ls *= w0;
+        O *= w0;
+#pragma unroll
+        for (int i = 0; i < NB; ++i) {
+            const float w = (mv[i] == -INFINITY) ? 0.f : expf(mv[i] - Mb);
+            Ls = fmaf(lv[i], w, Ls);
+            O = fmaf(ov[i], w, O);
+        }
+        M = Mb;
+    }
+    return O / Ls;
+}
+
 
 // Input of o_proj (XMODE == X_ATTN) / down_proj (X_SWIGLU) for the team's WHOLE unit range [u0, u1) (units = k-steps of 32, numbered
 // slab-major; the range wraps at most once from the end of one slab's k-range to the start of the next): staged once, in unit order,
@@ -742,7 +831,7 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
                 }
                 const int head = k / kHD, d = k - head * kHD;
                 const HeadTeams ht = head_teams(head, p.n_heads, tc.nb);
-                float M = -INFINITY, Ls = 0.f, O = 0.f;
+                float M = -INFINITY, Ls = 0.f, O = 0.f;  // (merge_records, written out: this is the code batch 1 has always compiled to)
 #pragma unroll 1
                 for (int ib = 0; ib < ht.count; ib += kBatch) {
                     float mv[kBatch], lv[kBatch], ov[kBatch];
@@ -778,9 +867,64 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
     team_sync(tc.team);
 }
 
+// The same staging for a batch: sequence s of the team's range goes to xseg + s * xs_stride, its step sums to xsum_seg + s * H / 32.
+template <int XMODE, bool ACT>
+__device__ void stage_range_batch(const MegaParams& p, const TeamCtx& tc, int nk, int u0, int u1, const int32_t* perm) {
+    const int nun = u1 - u0, nfeat = nun * 32, B = p.batch;
+    const int ksb = u0 % nk;
+    auto k_of = [&](int e) {
+        int ks = ksb + (e >> 5);
+        if (ks >= nk) ks -= nk;
+        return ks * 32 + (e & 31);
+    };
+    team_sync(tc.team);
+    if constexpr (XMODE == X_SWIGLU) {
+        const int N = p.I;
+        for (int c = tc.ttid; c < nun * 4 * B; c += kTeamThreads) {
+            const int s = c / (nun * 4), cs = c - s * (nun * 4);
+            const int k = k_of(cs * 8);
+            const float* ag = p.acc_g + (size_t)s * N + k;
+            const float* au = p.acc_u + (size_t)s * N + k;
+            const float4 g0 = ld_cg4(ag), g1 = ld_cg4(ag + 4);
+            const float4 a0 = ld_cg4(au), a1 = ld_cg4(au + 4);
+            const uint32_t o0 = h2_as_u32(__floats2half2_rn(swiglu(g0.x, a0.x), swiglu(g0.y, a0.y)));
+            const uint32_t o1 = h2_as_u32(__floats2half2_rn(swiglu(g0.z, a0.z), swiglu(g0.w, a0.w)));
+            const uint32_t o2 = h2_as_u32(__floats2half2_rn(swiglu(g1.x, a1.x), swiglu(g1.y, a1.y)));
+            const uint32_t o3 = h2_as_u32(__floats2half2_rn(swiglu(g1.z, a1.z), swiglu(g1.w, a1.w)));
+            *reinterpret_cast<uint4*>(tc.xseg + (size_t)s * p.xs_stride + cs * 8) = perm8(o0, o1, o2, o3);
+        }
+    } else {
+        // attention output of sequence s: the records of (s, head) are those of the head's teams inside the sequence's teams
+#pragma unroll 1
+        for (int s = 0; s < B; ++s) {
+            const HeadTeams st = seq_teams(p, s, tc.nb);
+            __half* xseg = tc.xseg + (size_t)s * p.xs_stride;
+            for (int e = tc.ttid; e < nfeat; e += kTeamThreads) {
+                int k = k_of(e);
+                if constexpr (ACT) {
+                    if (perm != nullptr) k = perm[k];
+                }
+                const int head = k / kHD, d = k - head * kHD;
+                HeadTeams ht = head_teams(head, p.n_heads, st.count);
+                ht.first += st.first;
+                __half hv = __float2half_rn(merge_records<12>(p, ht, d));
+                const int j8 = e & 7;
+                if (perm_scaled(j8)) hv = __hmul(hv, __float2half_rn(0.0625f));
+                xseg[(e & ~7) + perm_pos(j8)] = hv;
+            }
+        }
+    }
+    team_sync(tc.team);
+#pragma unroll 1
+    for (int s = 0; s < B; ++s) compute_xsum(tc.xseg + (size_t)s * p.xs_stride, nun, tc.xsum_seg + s * (p.H / 32), tc.ttid, kTeamThreads);
+    team_sync(tc.team);
+}
+
 // One matvec op for this team: consume the stages of its unit range from the ring, RED the results.
 // NM = 2: gate|up as one virtual matrix (out0 = gate accumulators, out1 = up accumulators).
-template <int NM, int XMODE, bool ACT = false>
+// BATCH: B operand column g is sequence min(g, B - 1); lane (g, t) finishes columns 4 cg .. 4 cg + 3 of sequences 2t and 2t + 1 (the C
+// fragment columns), and out0 / out1 are [B][N].
+template <int NM, int XMODE, bool ACT = false, bool BATCH = false>
 __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& tc, int gs_steps, int K, int N, float* out0, float* out1, const __half* xs_full,
                            const float* xsum_full, const int32_t* perm = nullptr, float* const* peers = nullptr) {
     const int lane = tc.lane, g = lane >> 2, t = lane & 3;
@@ -800,13 +944,20 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
     const uint32_t lane_z = (uint32_t)(kZeroOff + (tc.wt * 4 + (cg >> 1)) * 4);    // the qzeros word holding its zero
     const int zshift = (cg & 1) * 16 + t * 4;
     const float unit = kSubnormal ? 16777216.0f : 1.0f;  // the accumulators are in units of 2^-24
+    // BATCH: lane group g feeds sequence min(g, B - 1) to the tensor pipe and the lane finishes sequences 2t and 2t + 1 (clamped: lanes
+    // past the batch read sequence B - 1 and drop their results); xsum_hi = offset of the step sums of sequence 2t + 1 from those of 2t
+    const int B = p.batch;
+    const int xsum_hi = BATCH ? (min(2 * t + 1, B - 1) - min(2 * t, B - 1)) * (p.H / 32) : 0;
     const int u_begin = u;
     if constexpr (XMODE != X_FULL) {
         if (u < u_end) {
 #ifdef GPTQ_TRACE
             const long long stg0 = clock64();
 #endif
-            stage_range<XMODE, ACT>(p, tc, nk, u, u_end, perm);
+            if constexpr (BATCH)
+                stage_range_batch<XMODE, ACT>(p, tc, nk, u, u_end, perm);
+            else
+                stage_range<XMODE, ACT>(p, tc, nk, u, u_end, perm);
 #ifdef GPTQ_TRACE
             if (g_mega_trace != nullptr && threadIdx.x == 0) g_mega_trace[blockIdx.x * 64 + 36 + XMODE] += (unsigned long long)(clock64() - stg0);
 #endif
@@ -830,6 +981,13 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
             xaddr = smem_u32(tc.xseg) + ((u - u_begin) * 32 + t * 8) * 2;
             xsum = tc.xsum_seg + (u - u_begin);
         }
+        float totb[4][2];  // BATCH: [column 4 cg + i][sequence 2t, 2t + 1]
+        if constexpr (BATCH) {
+            xaddr += (uint32_t)(min(g, B - 1) * p.xs_stride * 2);
+            xsum += min(2 * t, B - 1) * (p.H / 32);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) totb[i][0] = totb[i][1] = 0.f;
+        }
 
         float tot = 0.f;  // lane (g, t) finishes column 4g + t of the warp's stripe
         int left = nseg, gpos = ks0 % gs_steps;
@@ -838,7 +996,7 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
             const int n = stage_steps(gpos, gs_steps, left);
             const uint32_t st = cons_wait(ring);
             float acc0[4], acc1[4];
-            float xs4;
+            float xs4, xs4b;  // xs4b: sum of x of sequence 2t + 1 (BATCH)
             if (n == kStageSteps) {
                 uint4 q[4], xf[4];
 #pragma unroll
@@ -850,22 +1008,39 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
                 step_mma<false>(q[2], xf[2], acc0, acc1);
                 step_mma<false>(q[3], xf[3], acc0, acc1);
                 xs4 = (xsum[0] + xsum[1]) + (xsum[2] + xsum[3]);
+                if constexpr (BATCH) xs4b = (xsum[xsum_hi] + xsum[xsum_hi + 1]) + (xsum[xsum_hi + 2] + xsum[xsum_hi + 3]);
             } else {
                 {
                     const uint4 q = lds128(st + lane_b), xf = lds128(xaddr);
                     step_mma<true>(q, xf, acc0, acc1);
                     xs4 = xsum[0];
+                    if constexpr (BATCH) xs4b = xsum[xsum_hi];
                 }
 #pragma unroll 1
                 for (int j = 1; j < n; ++j) {
                     const uint4 q = lds128(st + lane_b + j * kStepBytes), xf = lds128(xaddr + j * 64);
                     step_mma<false>(q, xf, acc0, acc1);
                     xs4 += xsum[j];
+                    if constexpr (BATCH) xs4b += xsum[xsum_hi + j];
                 }
             }
             // group epilogue: tot += s * (acc * unit - z * sum(x))   (z = stored zero + 1, quant/quant_linear.py:120-121).
-            // All four t lanes hold the same four column sums (the batch columns of B are copies): lane t finishes column 4g + t.
-            {
+            if constexpr (BATCH) {
+                // acc0[0..1] / acc0[2..3] / acc1[0..1] / acc1[2..3]: columns 4 cg + 0 / 1 / 2 / 3 of sequences 2t, 2t + 1
+                uint32_t s01, s23, zw;
+                asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(s01), "=r"(s23) : "r"(st + (uint32_t)(kScaleOff + (tc.wt * 32 + 4 * cg) * 2)));
+                asm volatile("ld.shared.u32 %0, [%1];" : "=r"(zw) : "r"(st + lane_z));
+                const float2 sa = __half22float2(u32_as_h2(s01)), sb = __half22float2(u32_as_h2(s23));
+                const float sc[4] = {sa.x, sa.y, sb.x, sb.y};
+                const float av[4][2] = {{acc0[0], acc0[1]}, {acc0[2], acc0[3]}, {acc1[0], acc1[1]}, {acc1[2], acc1[3]}};
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float z = (float)(((zw >> ((cg & 1) * 16 + 4 * i)) & 15u) + 1u);
+                    totb[i][0] = fmaf(sc[i], fmaf(av[i][0], unit, -z * xs4), totb[i][0]);
+                    totb[i][1] = fmaf(sc[i], fmaf(av[i][1], unit, -z * xs4b), totb[i][1]);
+                }
+            } else {
+                // All four t lanes hold the same four column sums (the batch columns of B are copies): lane t finishes column 4g + t.
                 uint32_t sh, zw;
                 asm volatile("ld.shared.u16 %0, [%1];" : "=r"(sh) : "r"(st + lane_s));
                 asm volatile("ld.shared.u32 %0, [%1];" : "=r"(zw) : "r"(st + lane_z));
@@ -880,7 +1055,16 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
             gpos += n;
             if (gpos == gs_steps) gpos = 0;
         }
-        if (peers == nullptr) {
+        if constexpr (BATCH) {  // the four columns of each of the lane's sequences: one 16-byte vector RED
+            float* outq = (mi ? out1 : out0) + (slab_v - mi * nslab) * kSlabCols + tc.wt * 32 + 4 * cg;
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                if (2 * t + j < B)
+                    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(outq + (size_t)(2 * t + j) * N), "f"(totb[0][j]), "f"(totb[1][j]),
+                                 "f"(totb[2][j]), "f"(totb[3][j])
+                                 : "memory");
+            }
+        } else if (peers == nullptr) {
             asm volatile("red.global.add.f32 [%0], %1;" ::"l"(outp), "f"(tot) : "memory");  // the warp's 32 columns: one 128-byte line
         } else {  // tensor parallelism, direct mode: the partial sum goes into out0's counterpart on every rank
             const size_t off = (size_t)(outp - out0);
@@ -893,11 +1077,11 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
 // ---- attention ----------------------------------------------------------------------------------------------------------
 // Work units (head, 32 keys); a team serves one head (attn_range); one unit = one ring stage (K rows, V rows).  The team writes
 // one partial record (m, l, o[128]) to p.part[T].
+// BATCH: the team serves one (sequence, head) pair (attn_work), at that sequence's position, in that sequence's cache slot.
+template <bool BATCH>
 __device__ void run_attention(const MegaParams& p, ConsRing& ring, const TeamCtx& tc, int layer) {
-    const int pos = step_pos(p), Tlen = pos + 1;
-    const int upb = (Tlen + kKeysPerUnit - 1) / kKeysPerUnit;
-    int head, b0, b_end;
-    attn_range(tc.T, p.n_heads, tc.nb, upb, head, b0, b_end);
+    int pos, Tlen, head, b0, b_end;
+    const int seq = attn_work<BATCH>(p, tc.T, tc.nb, pos, Tlen, head, b0, b_end);
     float* red_o = reinterpret_cast<float*>(tc.scratch);                 // [8][128]  end of a segment
     float* red_ml = reinterpret_cast<float*>(tc.scratch + 4096);         // [8][2]
     float* q_s = reinterpret_cast<float*>(tc.scratch);                   // [128]     start of a segment (aliases red_o)
@@ -923,8 +1107,8 @@ __device__ void run_attention(const MegaParams& p, ConsRing& ring, const TeamCtx
         if (ttid < kHD) {
             const int i = ttid & 63;
             const bool hi = ttid >= 64;
-            const float c = ld_cg(p.rope_cs + i), s = ld_cg(p.rope_cs + 64 + i);
-            const float* aq = p.acc_qkv + head * kHD;
+            const float c = ld_cg(p.rope_cs + seq * kHD + i), s = ld_cg(p.rope_cs + seq * kHD + 64 + i);
+            const float* aq = p.acc_qkv + (size_t)seq * 3 * p.Hq + head * kHD;
             const float qx = __half2float(__float2half_rn(ld_cg(aq + i))), qy = __half2float(__float2half_rn(ld_cg(aq + i + 64)));  // the qkv projection output is fp16
             const float qr = hi ? __fadd_rn(__fmul_rn(qx, s), __fmul_rn(qy, c)) : __fsub_rn(__fmul_rn(qx, c), __fmul_rn(qy, s));
             q_s[ttid] = __half2float(__float2half_rn(qr));
@@ -936,7 +1120,7 @@ __device__ void run_attention(const MegaParams& p, ConsRing& ring, const TeamCtx
                 const __half kh = __float2half_rn(kr), vh = __float2half_rn(ld_cg(av + ttid));
                 knew[ttid] = kh;
                 vnew[ttid] = vh;
-                const size_t off = ((size_t)head * p.max_seq + pos) * kHD + ttid;
+                const size_t off = ((size_t)(seq * p.n_heads + head) * p.max_seq + pos) * kHD + ttid;
                 kc_l[off] = kh;
                 vc_l[off] = vh;
             }
@@ -1114,7 +1298,104 @@ __device__ void run_lm_head(const MegaParams& p, ConsRing& ring, const TeamCtx& 
     }
 }
 
-template <bool ACT>
+// The same for a batch: x of sequence s is read from shared memory (xs + s * xs_stride, natural order) for every row, because the 32
+// registers per sequence that batch 1 spends on it would not fit eight sequences; each weight chunk is loaded once for all of them.
+// mega_plan keeps 2 * lm_rows * batch * kTeamWarps floats within the team scratch.
+__device__ void run_lm_head_batch(const MegaParams& p, ConsRing& ring, const TeamCtx& tc, const __half* xs_plain) {
+    const int R = p.lm_rows, H = p.H, nch = H / 8, B = p.batch;
+    int u, u_end;
+    team_range(tc.T, (unsigned)((p.V + R - 1) / R), tc.nb, u, u_end);
+    float* part_s = reinterpret_cast<float*>(tc.scratch);  // [2][R][B][8]
+    const uint32_t xbase = smem_u32(xs_plain);
+    int buf = 0;
+#pragma unroll 1
+    for (; u < u_end; ++u) {
+        const int nrows = min(R, p.V - u * R);
+        const uint32_t st = cons_wait(ring);
+        float* ps = part_s + buf * (R * B * kTeamWarps);
+#pragma unroll 1
+        for (int r = 0; r < nrows; ++r) {
+            float a[kMaxBatch];
+#pragma unroll
+            for (int s = 0; s < kMaxBatch; ++s) a[s] = 0.f;
+#pragma unroll 1
+            for (int c = tc.ttid; c < nch; c += kTeamThreads) {
+                const uint4 wv = lds128(st + (uint32_t)(r * H * 2 + c * 16));
+                const uint32_t w[4] = {wv.x, wv.y, wv.z, wv.w};
+#pragma unroll
+                for (int s = 0; s < kMaxBatch; ++s) {
+                    if (s < B) {
+                        const uint4 xv = lds128(xbase + (uint32_t)((s * p.xs_stride + c * 8) * 2));
+                        const uint32_t x[4] = {xv.x, xv.y, xv.z, xv.w};
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            const float2 f = __half22float2(u32_as_h2(w[e])), xf = __half22float2(u32_as_h2(x[e]));
+                            a[s] = fmaf(f.x, xf.x, a[s]);
+                            a[s] = fmaf(f.y, xf.y, a[s]);
+                        }
+                    }
+                }
+            }
+#pragma unroll
+            for (int s = 0; s < kMaxBatch; ++s) {
+                if (s < B) {
+                    const float v = warp_sum(a[s]);
+                    if (tc.lane == 0) ps[(r * B + s) * kTeamWarps + tc.wt] = v;
+                }
+            }
+        }
+        cons_release(ring, tc.lane);
+        team_sync(tc.team);  // partials of this stage are visible; the other buffer is free again
+        if (tc.ttid < nrows * B) {
+            const int r = tc.ttid / B, s = tc.ttid - r * B;
+            float a = 0.f;
+#pragma unroll
+            for (int w = 0; w < kTeamWarps; ++w) a += ps[tc.ttid * kTeamWarps + w];
+            p.logits[(size_t)s * p.V + (size_t)u * R + r] = __float2half_rn(a);
+        }
+        buf ^= 1;
+    }
+}
+
+// greedy argmax of one row of logits written by other CTAs (lowest index wins ties); all consumer threads, thread 0 stores
+__device__ __forceinline__ void argmax_row(const __half* row, int V, int32_t* out) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    float best = -INFINITY;
+    int idx = 0x7fffffff;
+    for (int i = tid; i < V; i += kConsumers) {
+        const float v = __half2float(ld_cg_h(row + i));  // written by other CTAs
+        if (v > best || (v == best && i < idx)) {
+            best = v;
+            idx = i;
+        }
+    }
+    __shared__ float sv[kConsumerWarps];
+    __shared__ int si[kConsumerWarps];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+        if (ov > best || (ov == best && oi < idx)) {
+            best = ov;
+            idx = oi;
+        }
+    }
+    if (lane == 0) {
+        sv[warp] = best;
+        si[warp] = idx;
+    }
+    cta_sync();
+    if (tid == 0) {
+        for (int w = 1; w < kConsumerWarps; ++w)
+            if (sv[w] > best || (sv[w] == best && si[w] < idx)) {
+                best = sv[w];
+                idx = si[w];
+            }
+        out[0] = idx;
+    }
+}
+
+template <bool ACT, bool BATCH>
 __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __grid_constant__ MegaParams p) {
     extern __shared__ __align__(16) uint8_t smem_dyn[];
     uint8_t* smem_raw = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);  // TMA swizzle atoms: 1 KB aligned stages (1 KB of slack is allocated)
@@ -1122,10 +1403,12 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
     __shared__ __align__(8) unsigned long long bars_s[kTeams][2 * kMaxStages];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // smem (1 KB aligned): [team 0 ring][team 1 ring][xs: H halves][xsum: H/32 floats][tmp / team scratch]
+    // (BATCH: xs = batch rows of xs_stride halves, xsum = batch rows of H/32 floats)
     const uint32_t ring_bytes = (uint32_t)p.n_stages * kStageBytes;
+    const int nbat = BATCH ? p.batch : 1;
     __half* xs = reinterpret_cast<__half*>(smem_raw + kTeams * ring_bytes);
-    float* xsum = reinterpret_cast<float*>(xs + p.H);
-    uint8_t* tmp_raw = reinterpret_cast<uint8_t*>(xsum + p.H / 32);
+    float* xsum = reinterpret_cast<float*>(xs + (BATCH ? nbat * p.xs_stride : p.H));
+    uint8_t* tmp_raw = reinterpret_cast<uint8_t*>(xsum + nbat * (p.H / 32));
     tmp_raw += (16 - (reinterpret_cast<uintptr_t>(tmp_raw) & 15)) & 15;
     __half* tmp = reinterpret_cast<__half*>(tmp_raw);
 
@@ -1153,7 +1436,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
 #ifdef GPTQ_TRACE
             r.blocked = 0;
 #endif
-            producer_loop(p, r, blockIdx.x * kTeams + tm, nb);
+            producer_loop<BATCH>(p, r, blockIdx.x * kTeams + tm, nb);
         }
         return;
     }
@@ -1204,7 +1487,14 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
     };
 
     // this step's RoPE angles (quant/fused_attn.py:43,91): freq_i = exp(i * inv_base) * pos
-    if (blockIdx.x == 0 && tid < 64) {
+    if constexpr (BATCH) {  // one row of angles per sequence
+        if (blockIdx.x == 0 && tid < 64 * nbat) {
+            const int s = tid >> 6, i = tid & 63;
+            const float f = expf((float)i * p.inv_base) * (float)step_pos(p, s);
+            p.rope_cs[s * kHD + i] = cosf(f);
+            p.rope_cs[s * kHD + 64 + i] = sinf(f);
+        }
+    } else if (blockIdx.x == 0 && tid < 64) {
         const float f = expf((float)tid * p.inv_base) * (float)step_pos(p);
         p.rope_cs[tid] = cosf(f);
         p.rope_cs[64 + tid] = sinf(f);
@@ -1215,61 +1505,87 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
     const __half* resid_src = p.embed + (size_t)token * p.H;
     const float* resid_acc = nullptr;
     int cur = 1;
+    // BATCH: stage_norm for every sequence in turn (its tmp row and red_s are reused); sequence s reads row s of src / acc (or its own
+    // embedding row before the first layer) and writes row s of resid_out, xs and xsum
+    auto stage_norms = [&](bool plain, const __half* src, const float* acc, const __half* norm_w, __half* resid_out, const int32_t* perm) {
+#pragma unroll 1
+        for (int s = 0; s < nbat; ++s) {
+            const __half* src_s = acc != nullptr ? src + (size_t)s * p.H : p.embed + (size_t)min(max(p.tokens[s], 0), p.V - 1) * p.H;
+            const float* acc_s = acc != nullptr ? acc + (size_t)s * p.H : nullptr;
+            __half* out_s = resid_out != nullptr ? resid_out + (size_t)s * p.H : nullptr;
+            if (plain)
+                stage_norm<false, true>(p, src_s, acc_s, norm_w, out_s, xs + (size_t)s * p.xs_stride, xsum + s * (p.H / 32), tmp, red_s, nullptr);
+            else
+                stage_norm<ACT, false>(p, src_s, acc_s, norm_w, out_s, xs + (size_t)s * p.xs_stride, xsum + s * (p.H / 32), tmp, red_s, perm);
+        }
+    };
 #pragma unroll 1
     for (int l = 0; l < p.n_layers; ++l) {
         const LayerDesc& L = p.layers[l];
         // ---- Q ----
         MTRACE(l * 12 + 0);
-        stage_norm<ACT, false>(p, resid_src, resid_acc, L.input_norm, p.resid[cur ^ 1], xs, xsum, tmp, red_s, L.qkv_perm);
+        if constexpr (BATCH)
+            stage_norms(false, resid_src, resid_acc, L.input_norm, p.resid[cur ^ 1], L.qkv_perm);
+        else
+            stage_norm<ACT, false>(p, resid_src, resid_acc, L.input_norm, p.resid[cur ^ 1], xs, xsum, tmp, red_s, L.qkv_perm);
         MTRACE(l * 12 + 1);
         cur ^= 1;
-        zero_slice(p.acc_g, p.I);  // last read by the previous layer's D
-        zero_slice(p.acc_u, p.I);
+        zero_slice(p.acc_g, nbat * p.I);  // last read by the previous layer's D
+        zero_slice(p.acc_u, nbat * p.I);
         {
             OPTRACE_BEGIN(ring);
-            run_matvec<1, X_FULL>(p, ring, tc, L.qkv.gs_steps, p.H, 3 * p.Hq, p.acc_qkv, nullptr, xs, xsum);
+            run_matvec<1, X_FULL, false, BATCH>(p, ring, tc, L.qkv.gs_steps, p.H, 3 * p.Hq, p.acc_qkv, nullptr, xs, xsum);
             OPTRACE_END(ring, l, 0);
         }
         MTRACE(l * 12 + 2);
         grid_barrier(p.bar, gen);
         MTRACE(l * 12 + 3);
         // ---- A ----
-        zero_slice(p.acc_d, p.H);  // last read by this layer's Q
+        zero_slice(p.acc_d, nbat * p.H);  // last read by this layer's Q
         {
             OPTRACE_BEGIN(ring);
-            run_attention(p, ring, tc, l);
+            run_attention<BATCH>(p, ring, tc, l);
             OPTRACE_END(ring, l, 1);
         }
         MTRACE(l * 12 + 4);
         grid_barrier(p.bar, gen);
         MTRACE(l * 12 + 5);
         // ---- O ----
-        zero_slice(p.acc_qkv, 3 * p.Hq);
+        zero_slice(p.acc_qkv, nbat * 3 * p.Hq);
         {
             OPTRACE_BEGIN(ring);
-            run_matvec<1, X_ATTN, ACT>(p, ring, tc, L.o.gs_steps, p.Hq, p.H, p.tp_exchange ? p.acc_o_loc : p.acc_o, nullptr, xs, xsum, L.o_perm, (p.tp_size > 1 && !p.tp_exchange) ? p.acc_o_peer : nullptr);
+            if constexpr (BATCH)
+                run_matvec<1, X_ATTN, ACT, true>(p, ring, tc, L.o.gs_steps, p.Hq, p.H, p.acc_o, nullptr, xs, xsum, L.o_perm);
+            else
+                run_matvec<1, X_ATTN, ACT>(p, ring, tc, L.o.gs_steps, p.Hq, p.H, p.tp_exchange ? p.acc_o_loc : p.acc_o, nullptr, xs, xsum, L.o_perm, (p.tp_size > 1 && !p.tp_exchange) ? p.acc_o_peer : nullptr);
             OPTRACE_END(ring, l, 2);
         }
         MTRACE(l * 12 + 6);
         sync_all_ranks(p.acc_o_loc, p.acc_o_peer);
         MTRACE(l * 12 + 7);
         // ---- G ----
-        stage_norm<ACT, false>(p, p.resid[cur], p.acc_o, L.post_norm, p.resid[cur ^ 1], xs, xsum, tmp, red_s, L.mlp_perm);
+        if constexpr (BATCH)
+            stage_norms(false, p.resid[cur], p.acc_o, L.post_norm, p.resid[cur ^ 1], L.mlp_perm);
+        else
+            stage_norm<ACT, false>(p, p.resid[cur], p.acc_o, L.post_norm, p.resid[cur ^ 1], xs, xsum, tmp, red_s, L.mlp_perm);
         cur ^= 1;
         MTRACE(l * 12 + 8);
         {
             OPTRACE_BEGIN(ring);
-            run_matvec<2, X_FULL>(p, ring, tc, L.gate.gs_steps, p.H, p.I, p.acc_g, p.acc_u, xs, xsum);
+            run_matvec<2, X_FULL, false, BATCH>(p, ring, tc, L.gate.gs_steps, p.H, p.I, p.acc_g, p.acc_u, xs, xsum);
             OPTRACE_END(ring, l, 3);
         }
         MTRACE(l * 12 + 9);
         grid_barrier(p.bar, gen);
         // ---- D ----
-        zero_slice(p.acc_o, p.H);
+        zero_slice(p.acc_o, nbat * p.H);
         MTRACE(l * 12 + 10);
         {
             OPTRACE_BEGIN(ring);
-            run_matvec<1, X_SWIGLU>(p, ring, tc, L.down.gs_steps, p.I, p.H, p.tp_exchange ? p.acc_d_loc : p.acc_d, nullptr, xs, xsum, nullptr, (p.tp_size > 1 && !p.tp_exchange) ? p.acc_d_peer : nullptr);
+            if constexpr (BATCH)
+                run_matvec<1, X_SWIGLU, false, true>(p, ring, tc, L.down.gs_steps, p.I, p.H, p.acc_d, nullptr, xs, xsum);
+            else
+                run_matvec<1, X_SWIGLU>(p, ring, tc, L.down.gs_steps, p.I, p.H, p.tp_exchange ? p.acc_d_loc : p.acc_d, nullptr, xs, xsum, nullptr, (p.tp_size > 1 && !p.tp_exchange) ? p.acc_d_peer : nullptr);
             OPTRACE_END(ring, l, 4);
         }
         MTRACE(l * 12 + 11);
@@ -1278,13 +1594,22 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         resid_acc = p.acc_d;
     }
     // ---- L: final norm + lm_head ----
-    stage_norm<false, true>(p, resid_src, resid_acc, p.final_norm, nullptr, xs, xsum, tmp, red_s, nullptr);
-    zero_slice(p.acc_g, p.I);
-    zero_slice(p.acc_u, p.I);
-    run_lm_head(p, ring, tc, xs);
+    if constexpr (BATCH)
+        stage_norms(true, resid_src, resid_acc, p.final_norm, nullptr, nullptr);
+    else
+        stage_norm<false, true>(p, resid_src, resid_acc, p.final_norm, nullptr, xs, xsum, tmp, red_s, nullptr);
+    zero_slice(p.acc_g, nbat * p.I);
+    zero_slice(p.acc_u, nbat * p.I);
+    if constexpr (BATCH)
+        run_lm_head_batch(p, ring, tc, xs);
+    else
+        run_lm_head(p, ring, tc, xs);
     sync_all_ranks(nullptr, nullptr);
-    zero_slice(p.acc_d, p.H);
-    if (blockIdx.x == 0) {
+    zero_slice(p.acc_d, nbat * p.H);
+    if constexpr (BATCH) {
+        if (blockIdx.x == 0 && tid == 0) p.bar[1] = gen;  // see below
+        if ((int)blockIdx.x < nbat && p.next_token != nullptr) argmax_row(p.logits + (size_t)blockIdx.x * p.V, p.V, p.next_token + blockIdx.x);  // CTA s: sequence s
+    } else if (blockIdx.x == 0) {
         if (tid == 0) {  // every CTA has arrived at the last barrier: the counters rest at these values until the next launch
             p.bar[1] = gen;
             if (p.tp_size > 1) p.xbar_peer[p.tp_rank][32 * kMaxTP] = xgen;
@@ -1351,11 +1676,17 @@ struct MegaPlan {
     size_t smem;
 };
 
-// Shared-memory plan for this model on a device with `sms` SMs and `smem_max` bytes of opt-in shared memory per block;
-// returns false if the shape does not fit the kernel's staging buffers.
-bool mega_plan(const gptq_llama_model& m, int sms, size_t smem_max, size_t smem_static, MegaPlan& pl) {
+// halves between the sequences' rows of the staged x at batch > 1 (see MegaParams::xs_stride)
+inline int xs_stride(int H) { return H + 32; }
+
+// Shared-memory plan for this model at `batch` sequences on a device with `sms` SMs and `smem_max` bytes of opt-in shared memory per block;
+// returns false if the shape does not fit the kernel's staging buffers.  At batch B > 1 the staged x is B rows of xs_stride halves and its
+// step sums B rows of H/32 floats, which leaves fewer ring stages; the attention needs B * n_heads <= teams (one team per (sequence, head)
+// pair at least) and the lm_head partials of 2 * lm_rows * B rows x 8 warps must fit the team scratch.
+bool mega_plan(const gptq_llama_model& m, int batch, int sms, size_t smem_max, size_t smem_static, MegaPlan& pl) {
     const int H = m.hidden, I = m.intermediate;
-    const size_t fixed = (size_t)H * 2 + (size_t)(H / 32) * 4 + 16 + max((size_t)H * 2, (size_t)kTeams * kTeamScratch);
+    const size_t xs_bytes = batch > 1 ? (size_t)batch * xs_stride(H) * 2 : (size_t)H * 2;
+    const size_t fixed = xs_bytes + (size_t)batch * (H / 32) * 4 + 16 + max((size_t)H * 2, (size_t)kTeams * kTeamScratch);
     const size_t other = fixed + smem_static + 1024;  // + the kernel's static shared memory + 1 KB alignment slack of the rings
     if (smem_max < other) return false;
     int st = (int)((smem_max - other) / ((size_t)kTeams * kStageBytes));
@@ -1365,8 +1696,9 @@ bool mega_plan(const gptq_llama_model& m, int sms, size_t smem_max, size_t smem_
     pl.n_stages = st;
     pl.smem = fixed + 1024 + (size_t)kTeams * st * kStageBytes;
     pl.lm_rows = max(1, kLmStageBytes / (H * 2));
+    if (batch > 1) pl.lm_rows = max(1, min(pl.lm_rows, kTeamScratch / (2 * batch * kTeamWarps * 4)));
     if ((size_t)pl.lm_rows * H * 2 > (size_t)kStageBytes) return false;
-    if ((size_t)2 * pl.lm_rows * kTeamWarps * 4 > (size_t)kTeamScratch) return false;
+    if ((size_t)2 * pl.lm_rows * batch * kTeamWarps * 4 > (size_t)kTeamScratch) return false;
     // per-team k-segments of o_proj / down_proj are staged in half of the xs buffer, their step sums in half of xsum
     const long long nteams = (long long)sms * kTeams;
     const int Hq = m.n_heads * m.head_dim;  // attention width of this rank (= H on a single GPU)
@@ -1374,7 +1706,7 @@ bool mega_plan(const gptq_llama_model& m, int sms, size_t smem_max, size_t smem_
     const long long seg_d = ((long long)(H / kSlabCols) * (I / 32) + nteams - 1) / nteams + 1;
     const long long seg = max(seg_o, seg_d);
     if (seg * 32 > H / 2 || seg > H / 64) return false;
-    if (m.n_heads > nteams) return false;  // a team's attention range must meet at most two heads
+    if ((long long)batch * m.n_heads > nteams) return false;  // a team's attention range must meet at most two heads (one (sequence, head) pair at batch > 1)
     // 32-bit range arithmetic of team_range: (T + 1) * U must stay below 2^32 for every operation's unit count U
     const long long umax = max(max((long long)2 * (I / kSlabCols) * (H / 32), (long long)(H / kSlabCols) * (I / 32)),
                                max((long long)m.vocab, (long long)m.n_heads * 4096));
@@ -1386,7 +1718,8 @@ bool mega_plan(const gptq_llama_model& m, int sms, size_t smem_max, size_t smem_
 
 // ---------------------------------------------------------------------------------------------------
 bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st) {
-    if (st.batch != 1 || m.n_layers > kMaxLayers || m.head_dim != kHD) return false;
+    if (st.batch < 1 || st.batch > kMaxBatch || m.n_layers > kMaxLayers || m.head_dim != kHD) return false;
+    if (st.batch > 1 && st.tp != nullptr) return false;  // tensor parallelism: batch 1 only
     if (m.hidden % kSlabCols || m.intermediate % kSlabCols || m.hidden > 8192 || m.intermediate > 32768 || m.hidden % 64) return false;
     if ((3 * m.n_heads * m.head_dim) % kSlabCols) return false;  // the (local) fused qkv width is dealt in 256-column slabs
     if (st.tp != nullptr) {
@@ -1409,14 +1742,25 @@ bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st) {
         if (ly.gate.groupsize != ly.up.groupsize) return false;
     }
     if ((reinterpret_cast<uintptr_t>(m.lm_head) & 15) || (reinterpret_cast<uintptr_t>(st.k_cache) & 15) || (reinterpret_cast<uintptr_t>(st.v_cache) & 15)) return false;
+    // the staging buffers of this batch must fit the current device (mega_plan; every instantiation has the same static shared memory),
+    // so that gptq_llama_decode_launches reports the kernel chain wherever the launch would fall back to it
+    int dev = 0, sms = 0, smem_optin = 0;
+    cudaFuncAttributes fa;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
+        cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) == cudaSuccess &&
+        cudaFuncGetAttributes(&fa, llama_decode_mega_kernel<false, false>) == cudaSuccess) {
+        MegaPlan pl;
+        if (sms * kTeams > 1024 || !mega_plan(m, st.batch, sms, (size_t)smem_optin, fa.sharedSizeBytes, pl)) return false;
+    }
     return true;
 }
 
-size_t mega_scratch_bytes(const gptq_llama_model& m, int max_seq) {
+size_t mega_scratch_bytes(const gptq_llama_model& m, int batch, int max_seq) {
     (void)max_seq;
     const size_t max_teams = 1024;  // >= kTeams * SM count of any device this library runs on
-    return al256((size_t)m.hidden * 2) * 2 + al256((size_t)3 * m.hidden * 4) + al256((size_t)m.hidden * 4) * 2 + al256((size_t)m.intermediate * 4) * 2 +
-           al256(max_teams * kRec * 4) + al256(128 * 4) + 256 + (kMaxTP + 1) * 256 + al256((size_t)m.hidden * 4) * 2;
+    const size_t B = (size_t)batch;
+    return al256(B * m.hidden * 2) * 2 + al256(B * 3 * m.hidden * 4) + al256(B * m.hidden * 4) * 2 + al256(B * m.intermediate * 4) * 2 +
+           al256(max_teams * kRec * 4) + al256(B * 128 * 4) + 256 + (kMaxTP + 1) * 256 + al256((size_t)m.hidden * 4) * 2;
 }
 
 cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state& st, uint8_t* scratch, cudaStream_t stream) {
@@ -1427,11 +1771,13 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
         return cudaErrorInvalidDevice;
     bool any_perm = false;
     for (int l = 0; l < m.n_layers; ++l) any_perm = any_perm || m.layers[l].qkv_perm != nullptr || m.layers[l].o_perm != nullptr || m.layers[l].mlp_perm != nullptr;
-    auto kernel = any_perm ? llama_decode_mega_kernel<true> : llama_decode_mega_kernel<false>;
+    const int B = st.batch;
+    auto kernel = B > 1 ? (any_perm ? llama_decode_mega_kernel<true, true> : llama_decode_mega_kernel<false, true>)
+                        : (any_perm ? llama_decode_mega_kernel<true, false> : llama_decode_mega_kernel<false, false>);
     cudaFuncAttributes fa;
     if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess) return cudaErrorInvalidDeviceFunction;
     MegaPlan pl;
-    if (sms * kTeams > 1024 || !mega_plan(m, sms, (size_t)smem_optin, fa.sharedSizeBytes, pl)) return cudaErrorInvalidConfiguration;
+    if (sms * kTeams > 1024 || !mega_plan(m, B, sms, (size_t)smem_optin, fa.sharedSizeBytes, pl)) return cudaErrorInvalidConfiguration;
 
     MegaParams p{};
     p.n_layers = m.n_layers; p.H = m.hidden; p.Hq = m.n_heads * m.head_dim; p.I = m.intermediate; p.V = m.vocab; p.n_heads = m.n_heads;
@@ -1450,9 +1796,11 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     p.positions = st.positions;
     p.k_cache = reinterpret_cast<__half*>(st.k_cache);
     p.v_cache = reinterpret_cast<__half*>(st.v_cache);
-    p.layer_stride = (size_t)m.n_heads * st.max_seq * m.head_dim;
+    p.layer_stride = (size_t)B * m.n_heads * st.max_seq * m.head_dim;
     p.logits = reinterpret_cast<__half*>(st.logits);
     p.next_token = st.next_tokens;
+    p.batch = B;
+    p.xs_stride = xs_stride(m.hidden);
     size_t off = 0;
     auto take = [&](size_t bytes) {
         uint8_t* q = scratch + off;
@@ -1460,11 +1808,11 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
         return q;
     };
     // the head of the region has the same layout on every tensor-parallel rank (it depends on the hidden size only): peers address
-    // acc_o / acc_d / xbar of this rank through its scratch base
-    p.resid[0] = reinterpret_cast<__half*>(take((size_t)m.hidden * 2));
-    p.resid[1] = reinterpret_cast<__half*>(take((size_t)m.hidden * 2));
-    p.acc_o = reinterpret_cast<float*>(take((size_t)m.hidden * 4));
-    p.acc_d = reinterpret_cast<float*>(take((size_t)m.hidden * 4));
+    // acc_o / acc_d / xbar of this rank through its scratch base.  Every per-sequence buffer is [B][n] (gptq_b200.h).
+    p.resid[0] = reinterpret_cast<__half*>(take((size_t)B * m.hidden * 2));
+    p.resid[1] = reinterpret_cast<__half*>(take((size_t)B * m.hidden * 2));
+    p.acc_o = reinterpret_cast<float*>(take((size_t)B * m.hidden * 4));
+    p.acc_d = reinterpret_cast<float*>(take((size_t)B * m.hidden * 4));
     unsigned long long* xbar = reinterpret_cast<unsigned long long*>(take((kMaxTP + 1) * 256));
     const gptq_llama_tp* tp = st.tp;
     p.tp_size = tp != nullptr ? tp->size : 1;
@@ -1480,11 +1828,11 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     }
     p.acc_o_loc = reinterpret_cast<float*>(take((size_t)m.hidden * 4));
     p.acc_d_loc = reinterpret_cast<float*>(take((size_t)m.hidden * 4));
-    p.acc_qkv = reinterpret_cast<float*>(take((size_t)3 * p.Hq * 4));
-    p.acc_g = reinterpret_cast<float*>(take((size_t)m.intermediate * 4));
-    p.acc_u = reinterpret_cast<float*>(take((size_t)m.intermediate * 4));
+    p.acc_qkv = reinterpret_cast<float*>(take((size_t)B * 3 * p.Hq * 4));
+    p.acc_g = reinterpret_cast<float*>(take((size_t)B * m.intermediate * 4));
+    p.acc_u = reinterpret_cast<float*>(take((size_t)B * m.intermediate * 4));
     p.part = reinterpret_cast<float*>(take((size_t)1024 * kRec * 4));
-    p.rope_cs = reinterpret_cast<float*>(take(128 * 4));
+    p.rope_cs = reinterpret_cast<float*>(take((size_t)B * 128 * 4));
     p.bar = reinterpret_cast<unsigned long long*>(take(256));
     // One tensor map per row stride serves every layer: class 0 = qkv (N = 3H), 1 = o and down (N = H), 2 = gate and up (N = I).
     // Its base is the lowest qweight address of the class; a matrix is addressed through the chunk coordinate (128-byte units).

@@ -44,9 +44,9 @@ cudaError_t launch_qlinear_skinny(const QLinearArgs& a, bool pdl);
 bool gemm_tc_supported(const QLinearArgs& a);
 cudaError_t launch_qlinear_gemm_tc(const QLinearArgs& a);
 
-// decode_mega.cu -- persistent single-kernel decode step (batch 1, int4 kernel-form layers)
+// decode_mega.cu -- persistent single-kernel decode step (batch 1 to 8, int4 kernel-form layers)
 bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st);
-size_t mega_scratch_bytes(const gptq_llama_model& m, int max_seq);
+size_t mega_scratch_bytes(const gptq_llama_model& m, int batch, int max_seq);
 cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state& st, uint8_t* scratch, cudaStream_t stream);
 
 // elementwise.cu

@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('GPTQ_B200_LIB') or os.path.join(os.path.dirname(_HERE), 'libgptq_b200.so')  # env override: A/B builds during development
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 c_void_p, c_int, c_int64, c_size_t, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t, ctypes.c_float
 

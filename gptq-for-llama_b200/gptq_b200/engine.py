@@ -137,7 +137,7 @@ class LlamaDecoder:
         self.batch, self.max_seq = batch, max_seq
         with torch.cuda.device(self.dev):
             # kernel-side view of the weights: nibble-widened 2/3-bit fields, regrouped act-order rows (+ input gathers)
-            prepared = kernel_layers(layers, allow_perm=(batch == 1))
+            prepared = kernel_layers(layers)
             if prepared is None:
                 prepared = kernel_layers(layers, allow_perm=False)
             self.klayers, self.perms = prepared
@@ -265,69 +265,111 @@ class LlamaDecoder:
     def reset(self):
         self.positions.zero_()
 
-    def set_input(self, tokens, position):
-        """Token ids (int or sequence of `batch` ints) and the cache position of this step; validated on the host: the kernels
-        only clamp (a position beyond the cache or a token outside the vocabulary must never reach them)."""
+    def set_input(self, tokens, positions):
+        """Token ids (int or sequence of `batch` ints) and the cache position of this step (int: every sequence, or sequence of `batch` ints: one
+        per sequence); validated on the host: the kernels only clamp (a position beyond the cache or a token outside the vocabulary must never
+        reach them)."""
         toks = [int(tokens)] * self.batch if isinstance(tokens, int) else [int(t) for t in tokens]
         if len(toks) != self.batch:
             raise ValueError(f'expected {self.batch} token ids, got {len(toks)}')
-        if not 0 <= int(position) < self.max_seq:
-            raise ValueError(f'position {position} outside the KV cache (max_seq = {self.max_seq})')
+        pos = [int(positions)] * self.batch if isinstance(positions, int) else [int(p) for p in positions]
+        if len(pos) != self.batch:
+            raise ValueError(f'expected {self.batch} positions, got {len(pos)}')
+        if any(not 0 <= p < self.max_seq for p in pos):
+            raise ValueError(f'position {positions} outside the KV cache (max_seq = {self.max_seq})')
         if any(t < 0 or t >= self.vocab for t in toks):
             raise ValueError(f'token id outside the vocabulary (0..{self.vocab - 1})')
         self.tokens.copy_(torch.tensor(toks, dtype=torch.int32))
-        self.positions.fill_(int(position))
+        self.positions.copy_(torch.tensor(pos, dtype=torch.int32))
 
     @torch.no_grad()
     def prefill(self, prompt_ids):
-        """Batched pass over the first len(prompt) - 1 prompt tokens that fills the static KV cache (batch 1): per layer the quantized linears on
-        the wgmma GEMM path (gptq_qlinear_fwd / gptq_fused_mlp_fwd with M = tokens), the RoPE and RMSNorm kernels, torch SDPA for the causal
-        attention (as the reference's QuantLlamaAttention does, quant/fused_attn.py:154-155); keys are cached after RoPE.  The LAST prompt token then
-        goes through the decode step like every generated one (it produces the first logits).  Returns the number of cached positions."""
-        assert self.batch == 1 and self.tp is None
-        n = len(prompt_ids) - 1
-        if n <= 0:
-            return 0
+        """prefill_batch of one prompt (batch 1).  Returns the number of cached positions."""
+        assert self.batch == 1
+        return self.prefill_batch([prompt_ids])[0]
+
+    @torch.no_grad()
+    def prefill_batch(self, prompts):
+        """Ragged pass over the first len(prompt) - 1 tokens of each of the `batch` prompts that fills sequence b's slot of the static KV cache:
+        the rows of every prompt are concatenated into one M-row pass (M = the sum of their lengths) through the quantized linears on the wgmma
+        GEMM path (gptq_qlinear_fwd / gptq_fused_mlp_fwd), the RMSNorm kernel and the RoPE kernel (per-token positions); the causal attention
+        runs per prompt in torch SDPA (as the reference's QuantLlamaAttention does, quant/fused_attn.py:154-155); keys are cached after RoPE.
+        The LAST token of each prompt then goes through the decode step like every generated one (it produces the first logits).  Returns the
+        number of cached positions per prompt (0 for a prompt of length 1)."""
+        assert self.tp is None
+        if len(prompts) != self.batch:
+            raise ValueError(f'expected {self.batch} prompts, got {len(prompts)}')
+        ns = [max(len(p) - 1, 0) for p in prompts]
+        if any(n > self.max_seq for n in ns):
+            raise ValueError(f'prompt does not fit the KV cache (max_seq = {self.max_seq})')
+        total = sum(ns)
+        if total == 0:
+            return ns
         H, nh, hd = self.hidden, self.n_heads, self.head_dim
         w4 = lambda w: (w.qweight, w.scales, w.qzeros, w.g_idx)
-        x = self.embed[torch.tensor(list(prompt_ids[:n]), device=self.dev)]  # [n, H]
-        pos = torch.arange(n, device=self.dev, dtype=torch.int64)[None, :]
+        ids = [int(t) for p, n in zip(prompts, ns) for t in p[:n]]
+        x = self.embed[torch.tensor(ids, device=self.dev)]  # [total, H]
+        pos = torch.cat([torch.arange(n, dtype=torch.int64) for n in ns]).to(self.dev)[None, :]
+        spans = [(b, sum(ns[:b]), n) for b, n in enumerate(ns) if n > 0]  # (sequence, first row, rows)
         for li, ly in enumerate(self.layers):
-            qkv = ops.matmul248(ops.rmsnorm(x, ly['input_norm'], self.model.rms_eps), *w4(ly['qkv']), ly['qkv'].bits, groupsize=ly['qkv'].hint).view(1, n, 3, nh, hd)
+            qkv = ops.matmul248(ops.rmsnorm(x, ly['input_norm'], self.model.rms_eps), *w4(ly['qkv']), ly['qkv'].bits, groupsize=ly['qkv'].hint).view(1, total, 3, nh, hd)
             ops.rotate_half_(qkv[:, :, :2], pos, base=self.model.rope_base)
-            q, k, v = (qkv[0, :, i].transpose(0, 1) for i in range(3))  # [nh, n, hd]
-            self.k_cache[li, 0, :, :n] = k
-            self.v_cache[li, 0, :, :n] = v
-            att = torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None], is_causal=True)[0].transpose(0, 1).reshape(n, H)
+            atts = []
+            for b, r0, n in spans:
+                q, k, v = (qkv[0, r0:r0 + n, i].transpose(0, 1) for i in range(3))  # [nh, n, hd]
+                self.k_cache[li, b, :, :n] = k
+                self.v_cache[li, b, :, :n] = v
+                atts.append(torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None], is_causal=True)[0].transpose(0, 1).reshape(n, H))
+            att = atts[0] if len(atts) == 1 else torch.cat(atts)
             x = x + ops.matmul248(att, *w4(ly['o']), ly['o'].bits, groupsize=ly['o'].hint)
             h = ops.fused_mlp(ops.rmsnorm(x, ly['post_norm'], self.model.rms_eps), w4(ly['gate']), w4(ly['up']), ly['gate'].bits, ly['gate'].hint)
             x = x + ops.matmul248(h, *w4(ly['down']), ly['down'].bits, groupsize=ly['down'].hint)
-        return n
+        return ns
+
+    def _check_prompts(self, prompts, max_new_tokens):
+        if len(prompts) != self.batch:
+            raise ValueError(f'expected {self.batch} prompts, got {len(prompts)}')
+        for p in prompts:
+            if len(p) < 1 or len(p) + max_new_tokens > self.max_seq + 1:
+                raise ValueError(f'prompt ({len(p)}) + max_new_tokens ({max_new_tokens}) does not fit the KV cache (max_seq = {self.max_seq})')
+            if any(int(t) < 0 or int(t) >= self.vocab for t in p):
+                raise ValueError(f'prompt token id outside the vocabulary (0..{self.vocab - 1})')
+
+    def _decode(self, prompts, max_new_tokens, starts):
+        """Greedy lock-step decode: sequence b is stepped from position starts[b] (its cache holds the positions before it) until it has
+        max_new_tokens new tokens; the prompts' remaining tokens are fed first.  Every sequence takes the same number of steps."""
+        out = [[int(t) for t in p] for p in prompts]
+        steps = len(prompts[0]) + max_new_tokens - 1 - starts[0]
+        assert all(len(p) + max_new_tokens - 1 - s == steps for p, s in zip(prompts, starts))
+        for k in range(steps):
+            pos = [s + k for s in starts]
+            self.set_input([p[i] if i < len(p) else o[-1] for p, o, i in zip(prompts, out, pos)], pos)
+            self.step()
+            nxt = self.next_tokens.tolist()
+            for b, (p, i) in enumerate(zip(prompts, pos)):
+                if i >= len(p) - 1:
+                    out[b].append(nxt[b])
+        return out
 
     @torch.no_grad()
     def generate(self, prompt_ids, max_new_tokens, prefill=True):
         """Greedy decode (batch 1).  One engine, two phases: the prompt is prefilled in one batched pass (wgmma GEMM path) into the static KV
         cache, then the persistent decode kernel takes over token by token; prefill=False feeds the prompt through the decode step instead."""
         assert self.batch == 1
-        if len(prompt_ids) < 1 or len(prompt_ids) + max_new_tokens > self.max_seq + 1:
-            raise ValueError(f'prompt ({len(prompt_ids)}) + max_new_tokens ({max_new_tokens}) does not fit the KV cache (max_seq = {self.max_seq})')
-        if any(int(t) < 0 or int(t) >= self.vocab for t in prompt_ids):
-            raise ValueError(f'prompt token id outside the vocabulary (0..{self.vocab - 1})')
-        out = list(prompt_ids)
+        self._check_prompts([prompt_ids], max_new_tokens)
         self.reset()
         start = self.prefill(prompt_ids) if (prefill and self.tp is None) else 0
-        tok = torch.empty(1, dtype=torch.int32, device=self.dev)
-        for i in range(start, len(prompt_ids) + max_new_tokens - 1):
-            if i < len(prompt_ids):
-                self.tokens.copy_(torch.tensor([prompt_ids[i]], dtype=torch.int32), non_blocking=False)
-            else:
-                self.tokens.copy_(tok)
-            self.positions.fill_(i)
-            self.step()
-            tok.copy_(self.next_tokens)
-            if i >= len(prompt_ids) - 1:
-                out.append(int(tok.item()))
-        return out
+        return self._decode([prompt_ids], max_new_tokens, [start])[0]
+
+    @torch.no_grad()
+    def generate_batch(self, prompts, max_new_tokens):
+        """Greedy decode of `batch` prompts of different lengths: one ragged prefill (prefill_batch), then every sequence is stepped in
+        lock-step at its own position by the decode step (the persistent kernel decodes them all in one launch).  Returns one token list per
+        prompt: the prompt followed by its max_new_tokens generated tokens."""
+        self._check_prompts(prompts, max_new_tokens)
+        self.reset()
+        starts = self.prefill_batch(prompts)
+        return self._decode(prompts, max_new_tokens, starts)
 
 
 def synthetic_llama(size='7b', bits=4, groupsize=128, act_order=False, vocab=32000, device='cuda:0', seed=0, n_layers=None, **kw):

@@ -37,7 +37,8 @@
 extern "C" {
 #endif
 
-#define GPTQ_B200_ABI_VERSION 4 /* 2: act-order input gathers; 3: gptq_llama_persistent_scratch_offset; 4: tensor parallelism (gptq_llama_tp, gptq_ipc_*) */
+#define GPTQ_B200_ABI_VERSION 5 /* 2: act-order input gathers; 3: gptq_llama_persistent_scratch_offset; 4: tensor parallelism (gptq_llama_tp, gptq_ipc_*);
+                                   5: persistent path at batch 2..8 ([batch][hidden] residual rows in the persistent region) */
 
 typedef void* gptq_stream_t; /* cudaStream_t */
 
@@ -183,11 +184,13 @@ typedef struct gptq_llama_state {
 size_t gptq_llama_scratch_bytes(const gptq_llama_model* model, int batch, int max_seq);
 int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_llama_state* state, gptq_stream_t stream);
 /* Number of kernels one gptq_llama_decode_step launches for this model/state: 1 when the persistent single-kernel
- * path applies (batch 1, every layer int4 without act-order), else the per-operation kernel chain. */
+ * path applies (batch 1 to 8, every layer int4 in kernel form -- act-order layers with input gathers included -- and a shape
+ * whose staging buffers fit the device's shared memory at this batch; tensor parallelism at batch 1 only), else the
+ * per-operation kernel chain.  Each sequence b is stepped at its own positions[b]. */
 int gptq_llama_decode_launches(const gptq_llama_model* model, const gptq_llama_state* state);
 /* Diagnostics / tests: byte offset, inside the scratch area, of the persistent kernel's region.  It begins with the residual
- * stream ping-pong: two fp16 [hidden] vectors, each padded to 256 bytes (after a step: [0] = the residual entering the last
- * layer, [1] = the residual after the last layer's attention block). */
+ * stream ping-pong: two fp16 [batch, hidden] arrays (row b = sequence b), each padded to 256 bytes (after a step: [0] = the
+ * residual entering the last layer, [1] = the residual after the last layer's attention block). */
 size_t gptq_llama_persistent_scratch_offset(const gptq_llama_model* model, int batch, int max_seq);
 
 /* Device memory that other processes of the node can map (CUDA IPC), for the tensor-parallel scratch / logits buffers:
