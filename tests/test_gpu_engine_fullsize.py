@@ -19,6 +19,7 @@ import torch
 
 from oracle import cref
 from oracle import gptq_oracle as O
+from attn_probe import resid_buffers
 from gpu_util import assert_rel_close
 
 pytestmark = pytest.mark.gpu
@@ -102,13 +103,8 @@ def oracle_head(dec, x):
 
 
 def _resid_buffers(dec):
-    """The kernel's residual ping-pong (fp16 [H] x 2 at the head of its scratch area, gptq_llama_persistent_scratch_offset):
-    after a step [0] = x entering the last layer, [1] = x after the last layer's attention block."""
-    H = dec.hidden
-    step = (H * 2 + 255) // 256 * 256
-    base = dec.mega_scratch_offset()
-    raw = dec.scratch[base:base + 2 * step]
-    return [raw[i * step:i * step + H * 2].view(torch.float16).cpu().clone() for i in range(2)]
+    """Row 0 of the kernel's residual ping-pong (attn_probe.resid_buffers): [0] = x entering the last layer, [1] = x after its attention."""
+    return [r[0].cpu() for r in resid_buffers(dec)]
 
 
 def _check_last_layer_blocks(dec, layers, n_layers, tok, pos, kc, vc, what):
