@@ -347,40 +347,63 @@ ScratchLayout scratch_layout(const gptq_llama_model& m, int batch, int max_seq) 
     ws = max(ws, skinny_workspace_bytes(batch, m.intermediate, m.hidden, false));
     L.ws_bytes = ws;
     L.ws = take(ws);
-    L.mega = take(mega_scratch_bytes(m, batch, max_seq));
+    L.mega = take(mega_scratch_bytes(m, batch));
     L.total = off;
     return L;
 }
 
-// One (optionally norm-prologue / residual-epilogue fused) quantized linear of the layer stack.
-cudaError_t engine_linear(const gptq_qweight& w, const gptq_qweight* w2, const void* x, int64_t ldx, const void* norm_w, float eps, const void* residual, void* out,
-                          int64_t ldo, int M, uint8_t* scratch, const ScratchLayout& L, cudaStream_t stream) {
-    QLinearArgs a{};
-    a.x = x; a.ldx = ldx; a.w = w; a.dual = (w2 != nullptr);
-    if (w2) a.w2 = *w2;
-    a.norm_w = norm_w; a.eps = eps; a.residual = residual; a.ldr = ldo; a.out = out; a.ldo = ldo; a.M = M;
-    a.workspace = scratch + L.ws; a.ws_bytes = L.ws_bytes; a.stream = stream;
-    if (skinny_supported(a)) return launch_qlinear_skinny(a, true);
-    // general path (act-order, other bit widths): separate norm / generic product / residual add
+// One quantized linear of the kernel chain with its fused RMSNorm prologue (norm_w) or residual epilogue (residual), and whether the
+// tuned int4 matvec serves it whole; otherwise the norm, the generic product and the residual add run as separate kernels.
+struct ChainLinear {
+    QLinearArgs a;
+    bool skinny;
+    int launches() const { return skinny ? 1 : 1 + (a.norm_w != nullptr) + (a.residual != nullptr); }
+};
+
+// The four quantized linears of layer ly in launch order: qkv (input norm), o_proj (x +=), gate|up (post norm), down_proj (x +=).
+void chain_linears(const gptq_llama_model& m, const gptq_llama_layer& ly, const gptq_llama_state& st, const ScratchLayout& L, cudaStream_t stream,
+                   ChainLinear (&out)[4]) {
+    uint8_t* sc = reinterpret_cast<uint8_t*>(st.scratch);
+    uint8_t* x = sc + L.x;
+    const int H = m.hidden, I = m.intermediate;
+    auto make = [&](const gptq_qweight& w, const gptq_qweight* w2, const void* in, int64_t ldx, const void* norm_w, const void* residual, void* o, int64_t ldo) {
+        ChainLinear c{};
+        QLinearArgs& a = c.a;
+        a.x = in; a.ldx = ldx; a.w = w; a.dual = (w2 != nullptr);
+        if (w2) a.w2 = *w2;
+        a.norm_w = norm_w; a.eps = norm_w != nullptr ? m.rms_eps : 0.f; a.residual = residual; a.ldr = ldo; a.out = o; a.ldo = ldo; a.M = st.batch;
+        a.workspace = sc + L.ws; a.ws_bytes = L.ws_bytes; a.stream = stream;
+        c.skinny = skinny_supported(a);
+        return c;
+    };
+    out[0] = make(ly.qkv, nullptr, x, H, ly.input_norm, nullptr, sc + L.qkv, 3 * H);
+    out[1] = make(ly.o, nullptr, sc + L.attn, H, nullptr, x, x, H);
+    out[2] = make(ly.gate, &ly.up, x, H, ly.post_norm, nullptr, sc + L.h, I);
+    out[3] = make(ly.down, nullptr, sc + L.h, I, nullptr, x, x, H);
+}
+
+cudaError_t engine_linear(const ChainLinear& c, uint8_t* scratch, const ScratchLayout& L) {
+    const QLinearArgs& a = c.a;
+    if (c.skinny) return launch_qlinear_skinny(a, true);
     QLinearArgs g = a;
     g.norm_w = nullptr;
     g.residual = nullptr;
-    if (norm_w != nullptr) {
-        cudaError_t e = launch_rmsnorm(x, ldx, norm_w, scratch + L.xn, w.K, M, w.K, eps, stream);
+    if (a.norm_w != nullptr) {
+        cudaError_t e = launch_rmsnorm(a.x, a.ldx, a.norm_w, scratch + L.xn, a.w.K, a.M, a.w.K, a.eps, a.stream);
         if (e != cudaSuccess) return e;
         g.x = scratch + L.xn;
-        g.ldx = w.K;
+        g.ldx = a.w.K;
     }
-    if (residual != nullptr) {
+    if (a.residual != nullptr) {
         g.out = scratch + L.tmp;
-        g.ldo = w.N;
+        g.ldo = a.w.N;
     }
     cudaError_t e = launch_qlinear_generic(g);
     if (e != cudaSuccess) return e;
-    if (residual != nullptr) {
+    if (a.residual != nullptr) {
         // residual and out are the same buffer in the engine (in-place x += f(x))
-        const int n = M * w.N;
-        return launch_pdl(residual_add_kernel, dim3(ceil_div(n, 256)), dim3(256), 0, stream, reinterpret_cast<__half*>(out),
+        const int n = a.M * a.w.N;
+        return launch_pdl(residual_add_kernel, dim3(ceil_div(n, 256)), dim3(256), 0, a.stream, reinterpret_cast<__half*>(a.out),
                           reinterpret_cast<const __half*>(scratch + L.tmp), n);
     }
     return cudaSuccess;
@@ -401,26 +424,17 @@ extern "C" size_t gptq_llama_persistent_scratch_offset(const gptq_llama_model* m
     return scratch_layout(*model, batch, max_seq).mega;  // (0 for a tensor-parallel state)
 }
 
-static bool has_input_perm(const gptq_llama_model& m) {
-    for (int l = 0; l < m.n_layers; ++l)
-        if (m.layers[l].qkv_perm != nullptr || m.layers[l].o_perm != nullptr || m.layers[l].mlp_perm != nullptr) return true;
-    return false;
-}
-
 extern "C" int gptq_llama_decode_launches(const gptq_llama_model* model, const gptq_llama_state* st) {
     if (model == nullptr || st == nullptr || model->layers == nullptr) return GPTQ_ERR_NULL;
     if (mega_supported(*model, *st)) return 1;
     if (has_input_perm(*model)) return GPTQ_ERR_UNSUPPORTED;  // regrouped act-order layers need the persistent kernel's gathers
+    const ScratchLayout L = scratch_layout(*model, st->batch, st->max_seq);
     int n = 1 + 1 + (st->next_tokens != nullptr ? 1 : 0);  // embed + lm_head (+ argmax)
     for (int l = 0; l < model->n_layers; ++l) {
-        const gptq_llama_layer& ly = model->layers[l];
-        const gptq_qweight* ws[4] = {&ly.qkv, &ly.o, &ly.gate, &ly.down};
-        const int extra_norm[4] = {1, 0, 1, 0}, extra_res[4] = {0, 1, 0, 1};
+        ChainLinear c[4];
+        chain_linears(*model, model->layers[l], *st, L, nullptr, c);
         n += 2;  // attention + combine
-        for (int i = 0; i < 4; ++i) {
-            const bool fast = ws[i]->bits == 4 && ws[i]->groupsize > 0 && ws[i]->groupsize % 32 == 0 && st->batch <= 8;
-            n += 1 + (fast ? 0 : extra_norm[i] + extra_res[i]);
-        }
+        for (const ChainLinear& lin : c) n += lin.launches();
     }
     return n;
 }
@@ -448,18 +462,15 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
 
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     uint8_t* sc = reinterpret_cast<uint8_t*>(st->scratch);
-    if (mega_supported(m, *st)) {
-        // tensor-parallel ranks keep the persistent kernel's region at the START of the scratch area (peers address it by offset)
-        const cudaError_t e = launch_decode_mega(m, *st, st->tp != nullptr ? sc : sc + L.mega, stream);
-        if (e == cudaSuccess) return GPTQ_OK;
-        if (e != cudaErrorCooperativeLaunchTooLarge && e != cudaErrorInvalidConfiguration) return GPTQ_ERR_CUDA;
-        // the device cannot co-schedule the persistent grid (or the shape does not fit its staging buffers): per-op kernel chain below
-    }
+    // tensor-parallel ranks keep the persistent kernel's region at the START of the scratch area (peers address it by offset)
+    const cudaError_t mega = launch_decode_mega(m, *st, st->tp != nullptr ? sc : sc + L.mega, stream);
+    if (mega == cudaSuccess) return GPTQ_OK;
+    if (mega != cudaErrorCooperativeLaunchTooLarge && mega != cudaErrorInvalidConfiguration) return GPTQ_ERR_CUDA;
+    // the step does not fit the persistent kernel, or the device cannot co-schedule its grid: per-op kernel chain below
     if (has_input_perm(m) || st->tp != nullptr) return GPTQ_ERR_UNSUPPORTED;  // only the persistent kernel implements these
     __half* x = reinterpret_cast<__half*>(sc + L.x);
     __half* qkv = reinterpret_cast<__half*>(sc + L.qkv);
     __half* attn = reinterpret_cast<__half*>(sc + L.attn);
-    __half* h = reinterpret_cast<__half*>(sc + L.h);
     float* part = reinterpret_cast<float*>(sc + L.part);
     const int B = st->batch, H = m.hidden;
     const float inv_base = (float)(-2.0 * log((double)m.rope_base) / (double)m.head_dim);
@@ -473,15 +484,14 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
 
     GPTQ_TRY(launch_pdl(embed_kernel, dim3(B), dim3(256), 0, stream, reinterpret_cast<const __half*>(m.embed), st->tokens, x, H, m.vocab));
     for (int l = 0; l < m.n_layers; ++l) {
-        const gptq_llama_layer& ly = m.layers[l];
-        GPTQ_TRY(engine_linear(ly.qkv, nullptr, x, H, ly.input_norm, m.rms_eps, nullptr, qkv, 3 * H, B, sc, L, stream));
+        ChainLinear c[4];
+        chain_linears(m, m.layers[l], *st, L, stream, c);
+        GPTQ_TRY(engine_linear(c[0], sc, L));
         GPTQ_TRY(launch_pdl(attn_decode_kernel, dim3(m.n_heads, L.nsplit, B), dim3(kAttnThreads), 0, stream, qkv, H,
                             reinterpret_cast<__half*>(st->k_cache) + l * layer_stride, reinterpret_cast<__half*>(st->v_cache) + l * layer_stride, st->positions,
                             m.n_heads, st->max_seq, B, inv_base, scale, part, L.nsplit));
         GPTQ_TRY(launch_pdl(attn_combine_kernel, dim3(m.n_heads, B), dim3(kHeadDim), 0, stream, part, st->positions, attn, H, m.n_heads, L.nsplit));
-        GPTQ_TRY(engine_linear(ly.o, nullptr, attn, H, nullptr, 0.f, x, x, H, B, sc, L, stream));
-        GPTQ_TRY(engine_linear(ly.gate, &ly.up, x, H, ly.post_norm, m.rms_eps, nullptr, h, m.intermediate, B, sc, L, stream));
-        GPTQ_TRY(engine_linear(ly.down, nullptr, h, m.intermediate, nullptr, 0.f, x, x, H, B, sc, L, stream));
+        for (int i = 1; i < 4; ++i) GPTQ_TRY(engine_linear(c[i], sc, L));
     }
     {
         const size_t smem = (size_t)B * H * sizeof(__half);

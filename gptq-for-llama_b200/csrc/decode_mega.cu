@@ -25,8 +25,7 @@
 // exact, and scale / zero are applied ONCE per group on the fp32 accumulator together with the group's sum of
 // x (computed when x is staged).  5 integer instructions + 1 HMMA per packed word; the result differs from the
 // reference only by NOT rounding every dequantised weight to fp16 (it is closer to the exact product); the
-// 1e-3 tests in tests/ hold it to the oracle.  -DGPTQ_DQ_EXACT_INT selects the variant that converts nibbles to
-// exact fp16 integers (magic-number trick, 4 more fp16 instructions per word) and leaves x unscaled.
+// 1e-3 tests in tests/ hold it to the oracle.
 //
 // Split-K partial sums are accumulated with red.global.add.f32 into fp32 vectors that the NEXT operation
 // rounds to fp16 exactly where the reference rounds (a QuantLinear output is fp16); each vector is re-zeroed
@@ -37,7 +36,7 @@
 // reads sequence min(g, B - 1)), so one weight stream, one dequantisation and one HMMA per packed word serve the whole batch.  Every
 // per-sequence vector (residual stream, accumulators, staged x and its step sums, RoPE angles, logits) gets a [B] dimension; the
 // attention teams are dealt to (sequence, head) pairs in proportion to each sequence's context (seq_teams).  Batch 1 is the
-// !BATCH instantiation, whose code is the single-sequence kernel unchanged.
+// !BATCH instantiation: its loops over the sequences have the compile-time count 1.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
@@ -71,12 +70,7 @@ constexpr int kMaxStages = 8;
 constexpr int kTeamScratch = 4224;     // per-team scratch (attention merge buffers / lm_head partials)
 constexpr int kLmStageBytes = 16384;   // lm_head bytes per stage (whole rows)
 constexpr int kMaxBatch = 8;           // sequences of one step (the columns of the mma B operand)
-
-#ifdef GPTQ_DQ_EXACT_INT
-constexpr bool kSubnormal = false;
-#else
-constexpr bool kSubnormal = true;
-#endif
+constexpr int kMaxTeams = 1024;        // >= kTeams * SM count of any device this library runs on (attention records in the scratch region)
 
 #ifdef GPTQ_TRACE
 }  // namespace
@@ -219,8 +213,7 @@ __device__ __forceinline__ void attn_range(unsigned T, int n_heads, unsigned nb,
 // k-steps of the stage that starts `gpos` steps into its quantisation group, in a segment with `left` steps to go
 __device__ __forceinline__ int stage_steps(int gpos, int gs_steps, int left) { return min(min(kStageSteps, gs_steps - gpos), left); }
 
-// position of this step, clamped to the cache (the host rejects pos >= max_seq; the kernel must not write outside)
-__device__ __forceinline__ int step_pos(const MegaParams& p) { return min(max(p.positions[0], 0), p.max_seq - 1); }
+// position of sequence s in this step, clamped to the cache (the host rejects pos >= max_seq; the kernel must not write outside)
 __device__ __forceinline__ int step_pos(const MegaParams& p, int s) { return min(max(p.positions[s], 0), p.max_seq - 1); }
 
 // Batched attention: sequence s is served by teams [first, first + count): n_heads teams plus a share of the other nb - batch * n_heads
@@ -255,12 +248,8 @@ template <bool BATCH>
 __device__ __forceinline__ int attn_work(const MegaParams& p, unsigned T, unsigned nb, int& pos, int& Tlen, int& head, int& b0, int& b1) {
     int s = 0;
     HeadTeams st{0, (int)nb};
-    if constexpr (BATCH) {
-        s = team_seq(p, T, nb, st);
-        pos = step_pos(p, s);
-    } else {
-        pos = step_pos(p);
-    }
+    if constexpr (BATCH) s = team_seq(p, T, nb, st);
+    pos = step_pos(p, s);
     Tlen = pos + 1;
     const int upb = (Tlen + kKeysPerUnit - 1) / kKeysPerUnit;
     attn_range(T - st.first, p.n_heads, st.count, upb, head, b0, b1);
@@ -459,9 +448,6 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* bar, unsigned l
         do {
             asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(bar) : "memory");
         } while (v < target);
-#ifdef GPTQ_BARRIER_FENCE
-        fence_acq_rel_gpu();
-#endif
     }
     cta_sync();
 }
@@ -521,29 +507,24 @@ __device__ __forceinline__ float block_sum(float v, float* red_s) {
 // ---- x staging ----------------------------------------------------------------------------------------------------------
 // Matvec input layout: 8 consecutive k (natural order, 4 half2 words w0..w3) are stored k-permuted as
 // (k0,k4)(k1,k5)(k2,k6)(k3,k7): the B fragments of the two MMAs of a packed word; the pairs that meet the ODD
-// nibbles (k1,k5 / k3,k7; mask 0x00f000f0 = 16 n) are pre-scaled by 1/16 (kSubnormal only).
+// nibbles (k1,k5 / k3,k7; mask 0x00f000f0 = 16 n) are pre-scaled by 1/16.
 __device__ __forceinline__ uint4 perm8(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3) {
+    const __half2 sixteenth = __float2half2_rn(0.0625f);
     uint4 o;
     o.x = __byte_perm(w0, w2, 0x5410);
-    o.y = __byte_perm(w0, w2, 0x7632);
+    o.y = h2_as_u32(__hmul2(u32_as_h2(__byte_perm(w0, w2, 0x7632)), sixteenth));
     o.z = __byte_perm(w1, w3, 0x5410);
-    o.w = __byte_perm(w1, w3, 0x7632);
-    if (kSubnormal) {
-        const __half2 sixteenth = __float2half2_rn(0.0625f);
-        o.y = h2_as_u32(__hmul2(u32_as_h2(o.y), sixteenth));
-        o.w = h2_as_u32(__hmul2(u32_as_h2(o.w), sixteenth));
-    }
+    o.w = h2_as_u32(__hmul2(u32_as_h2(__byte_perm(w1, w3, 0x7632)), sixteenth));
     return o;
 }
-// position of natural index j (0..7) inside the permuted run of 8, and whether it is pre-scaled
+// position of natural index j (0..7) inside the permuted run of 8; the odd j are pre-scaled
 __device__ __forceinline__ int perm_pos(int j) { return ((j & 3) << 1) + (j >> 2); }
-__device__ __forceinline__ bool perm_scaled(int j) { return kSubnormal && (j & 1); }
 
 // sum of the EFFECTIVE x of one staged run of 8 (what the tensor pipe will multiply the nibbles with)
 __device__ __forceinline__ float run_sum(uint4 v) {
     const float2 a = __half22float2(u32_as_h2(v.x)), b = __half22float2(u32_as_h2(v.y)), c = __half22float2(u32_as_h2(v.z)), d = __half22float2(u32_as_h2(v.w));
     const float even = (a.x + a.y) + (c.x + c.y), odd = (b.x + b.y) + (d.x + d.y);
-    return kSubnormal ? fmaf(odd, 16.0f, even) : even + odd;
+    return fmaf(odd, 16.0f, even);
 }
 // xsum[s] = sum over the 32 k of step s of the staged x (4 runs of 8), for s < nsteps; `nthreads` threads (a multiple of 32) cooperate
 __device__ __forceinline__ void compute_xsum(const __half* xs, int nsteps, float* xsum, int tid, int nthreads) {
@@ -653,21 +634,13 @@ __device__ __forceinline__ void mma_16816_z(float (&d)[4], uint32_t a0, uint32_t
                  : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1), "f"(0.f));
 }
 
-// the four A registers (k-pairs (0,4), (1,5), (2,6), (3,7)) of one packed word
+// the four A registers (k-pairs (0,4), (1,5), (2,6), (3,7)) of one packed word, masked in place: fp16 subnormals n * 2^-24 and 16 n * 2^-24
 __device__ __forceinline__ void nibble_regs(uint32_t q, uint32_t (&a)[4]) {
     const uint32_t q8 = q >> 8;  // (as IMAD.HI on the FMA pipe it is far slower: tools/ubench/loop.cu, 1102 vs 817 cycles per stage)
-    if (kSubnormal) {  // masked in place: fp16 subnormals n * 2^-24 and 16 n * 2^-24
-        a[0] = q & 0x000f000fu;
-        a[1] = q & 0x00f000f0u;
-        a[2] = q8 & 0x000f000fu;
-        a[3] = q8 & 0x00f000f0u;
-    } else {  // exact fp16 integers: (1024 + n) - 1024 and (1024 + 16 n) / 16 - 64
-        const __half2 c1024 = __float2half2_rn(1024.0f), sixteenth = __float2half2_rn(0.0625f), m64 = __float2half2_rn(-64.0f);
-        a[0] = h2_as_u32(__hsub2(nibbles_to_h2<0x000f000fu>(q), c1024));
-        a[1] = h2_as_u32(__hfma2(nibbles_to_h2<0x00f000f0u>(q), sixteenth, m64));
-        a[2] = h2_as_u32(__hsub2(nibbles_to_h2<0x000f000fu>(q8), c1024));
-        a[3] = h2_as_u32(__hfma2(nibbles_to_h2<0x00f000f0u>(q8), sixteenth, m64));
-    }
+    a[0] = q & 0x000f000fu;
+    a[1] = q & 0x00f000f0u;
+    a[2] = q8 & 0x000f000fu;
+    a[3] = q8 & 0x00f000f0u;
 }
 
 // one k-step (4 packed words of this lane = columns 4g..4g+3 x 8 k) into the two accumulators
@@ -732,14 +705,14 @@ __device__ __forceinline__ float merge_records(const MegaParams& p, const HeadTe
     return O / Ls;
 }
 
-
 // Input of o_proj (XMODE == X_ATTN) / down_proj (X_SWIGLU) for the team's WHOLE unit range [u0, u1) (units = k-steps of 32, numbered
 // slab-major; the range wraps at most once from the end of one slab's k-range to the start of the next): staged once, in unit order,
 // into the team's half of the xs buffer with its per-step sums.  One L2 round trip for the common shapes.
-template <int XMODE, bool ACT>
+// BATCH: sequence s of the range goes to xseg + s * xs_stride, its step sums to xsum_seg + s * H / 32.
+template <int XMODE, bool ACT, bool BATCH>
 __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int u0, int u1, const int32_t* perm) {
-    const int lane = tc.lane;
     const int nun = u1 - u0, nfeat = nun * 32;
+    const int nbat = BATCH ? p.batch : 1;
     const int ksb = u0 % nk;  // k-step of the first unit
     auto k_of = [&](int e) {  // feature e of the range -> input index k
         int ks = ksb + (e >> 5);
@@ -748,143 +721,15 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
     };
     team_sync(tc.team);  // previous readers of xseg are done
     if constexpr (XMODE == X_SWIGLU) {  // h = fp16(silu(acc_gate) * acc_up)  (quant/fused_mlp.py:163-165)
-        for (int c = tc.ttid; c < nun * 4; c += kTeamThreads) {
-            const int k = k_of(c * 8);
-            const float4 g0 = ld_cg4(p.acc_g + k), g1 = ld_cg4(p.acc_g + k + 4);
-            const float4 a0 = ld_cg4(p.acc_u + k), a1 = ld_cg4(p.acc_u + k + 4);
-            const uint32_t o0 = h2_as_u32(__floats2half2_rn(swiglu(g0.x, a0.x), swiglu(g0.y, a0.y)));
-            const uint32_t o1 = h2_as_u32(__floats2half2_rn(swiglu(g0.z, a0.z), swiglu(g0.w, a0.w)));
-            const uint32_t o2 = h2_as_u32(__floats2half2_rn(swiglu(g1.x, a1.x), swiglu(g1.y, a1.y)));
-            const uint32_t o3 = h2_as_u32(__floats2half2_rn(swiglu(g1.z, a1.z), swiglu(g1.w, a1.w)));
-            *reinterpret_cast<uint4*>(tc.xseg + c * 8) = perm8(o0, o1, o2, o3);
-        }
-    } else {
-        // attention output: softmax-merge of the partial records (m, l, o[128]) of the head's teams (head_teams: contiguous, one
-        // record each).
-        constexpr int kBatch = 12;  // records fetched per round trip (a 7B head has 9 or 10 teams)
-        auto put = [&](int e, float v) {
-            __half hv = __float2half_rn(v);
-            const int j8 = e & 7;
-            if (perm_scaled(j8)) hv = __hmul(hv, __float2half_rn(0.0625f));
-            tc.xseg[(e & ~7) + perm_pos(j8)] = hv;
-        };
-        // heads of the range: [hA0, hA1] before the wrap, [0, hB1] after it
-        const int nA = min(nun, nk - ksb);
-        const int hA0 = (ksb * 32) / kHD, hA1 = ((ksb + nA) * 32 - 1) / kHD;
-        const int nslotA = hA1 - hA0 + 1, nslotB = (nun > nA) ? ((nun - nA) * 32 - 1) / kHD + 1 : 0;
-        bool fast = (nslotA + nslotB <= kTeamWarps) && (nun <= nk) && ((int)tc.nb / p.n_heads + 1 <= kBatch);
-        if constexpr (ACT) fast = fast && (perm == nullptr);
-        if (fast) {
-            // ONE round trip (per 256 features): every thread fetches the o values of its feature from all records of its head while
-            // warp w fetches (m, l) of the w-th head of the range and turns them into merge weights exp(m - M) / L.
-            float* wts = reinterpret_cast<float*>(tc.scratch);  // [kTeamWarps][kBatch]
-            float ov[kBatch];
-            int slot = 0;
-            auto fetch = [&](int e) {
-                const bool active = e < nfeat;
-                const int k = k_of(active ? e : 0);
-                const int head = k / kHD, d = k - head * kHD;
-                slot = ((e >> 5) < nA) ? head - hA0 : nslotA + head;
-                const HeadTeams ht = head_teams(head, p.n_heads, tc.nb);
-#pragma unroll
-                for (int i = 0; i < kBatch; ++i) ov[i] = (active && i < ht.count) ? ld_cg(p.part + (size_t)(ht.first + i) * kRec + 4 + d) : 0.f;
-            };
-            auto emit = [&](int e) {
-                if (e < nfeat) {
-                    float O = 0.f;
-#pragma unroll
-                    for (int i = 0; i < kBatch; ++i) O = fmaf(wts[slot * kBatch + i], ov[i], O);
-                    put(e, O);
-                }
-            };
-            fetch(tc.ttid);
-            if (tc.wt < nslotA + nslotB) {
-                const int head = tc.wt < nslotA ? hA0 + tc.wt : tc.wt - nslotA;
-                const HeadTeams ht = head_teams(head, p.n_heads, tc.nb);
-                float m = -INFINITY, l = 0.f;
-                if (lane < ht.count) {
-                    m = ld_cg(p.part + (size_t)(ht.first + lane) * kRec);
-                    l = ld_cg(p.part + (size_t)(ht.first + lane) * kRec + 1);
-                }
-                float M = m;
-#pragma unroll
-                for (int o = 8; o > 0; o >>= 1) M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, o));  // lanes 0..15 hold the batch
-                M = __shfl_sync(0xffffffffu, M, 0);
-                const float w = (m == -INFINITY) ? 0.f : expf(m - M);
-                float L = l * w;
-#pragma unroll
-                for (int o = 8; o > 0; o >>= 1) L += __shfl_xor_sync(0xffffffffu, L, o);
-                L = __shfl_sync(0xffffffffu, L, 0);
-                if (lane < kBatch) wts[tc.wt * kBatch + lane] = w / L;
+        for (int c = tc.ttid; c < nun * 4 * nbat; c += kTeamThreads) {
+            int s = 0, cs = c;  // sequence, 8-feature chunk of the range
+            if constexpr (BATCH) {
+                s = c / (nun * 4);
+                cs = c - s * (nun * 4);
             }
-            team_sync(tc.team);
-            emit(tc.ttid);
-            for (int e = tc.ttid + kTeamThreads; e - tc.ttid < nfeat; e += kTeamThreads) {  // wider ranges (13B, 65B): further round trips
-                fetch(e);
-                emit(e);
-            }
-        } else {
-            for (int e = tc.ttid; e < nfeat; e += kTeamThreads) {
-                int k = k_of(e);
-                if constexpr (ACT) {
-                    if (perm != nullptr) k = perm[k];  // regrouped rows: position k' of the matvec input is attention feature perm[k']
-                }
-                const int head = k / kHD, d = k - head * kHD;
-                const HeadTeams ht = head_teams(head, p.n_heads, tc.nb);
-                float M = -INFINITY, Ls = 0.f, O = 0.f;  // (merge_records, written out: this is the code batch 1 has always compiled to)
-#pragma unroll 1
-                for (int ib = 0; ib < ht.count; ib += kBatch) {
-                    float mv[kBatch], lv[kBatch], ov[kBatch];
-#pragma unroll
-                    for (int i = 0; i < kBatch; ++i) {  // all loads of the batch are in flight together
-                        const bool on = ib + i < ht.count;
-                        const float* rc = p.part + (size_t)(ht.first + (on ? ib + i : 0)) * kRec;
-                        const float m = ld_cg(rc), l = ld_cg(rc + 1), o = ld_cg(rc + 4 + d);
-                        mv[i] = on ? m : -INFINITY;
-                        lv[i] = on ? l : 0.f;
-                        ov[i] = on ? o : 0.f;
-                    }
-                    float Mb = M;
-#pragma unroll
-                    for (int i = 0; i < kBatch; ++i) Mb = fmaxf(Mb, mv[i]);
-                    const float w0 = (M == -INFINITY) ? 0.f : expf(M - Mb);
-                    Ls *= w0;
-                    O *= w0;
-#pragma unroll
-                    for (int i = 0; i < kBatch; ++i) {
-                        const float w = (mv[i] == -INFINITY) ? 0.f : expf(mv[i] - Mb);
-                        Ls = fmaf(lv[i], w, Ls);
-                        O = fmaf(ov[i], w, O);
-                    }
-                    M = Mb;
-                }
-                put(e, O / Ls);
-            }
-        }
-    }
-    team_sync(tc.team);
-    compute_xsum(tc.xseg, nun, tc.xsum_seg, tc.ttid, kTeamThreads);
-    team_sync(tc.team);
-}
-
-// The same staging for a batch: sequence s of the team's range goes to xseg + s * xs_stride, its step sums to xsum_seg + s * H / 32.
-template <int XMODE, bool ACT>
-__device__ void stage_range_batch(const MegaParams& p, const TeamCtx& tc, int nk, int u0, int u1, const int32_t* perm) {
-    const int nun = u1 - u0, nfeat = nun * 32, B = p.batch;
-    const int ksb = u0 % nk;
-    auto k_of = [&](int e) {
-        int ks = ksb + (e >> 5);
-        if (ks >= nk) ks -= nk;
-        return ks * 32 + (e & 31);
-    };
-    team_sync(tc.team);
-    if constexpr (XMODE == X_SWIGLU) {
-        const int N = p.I;
-        for (int c = tc.ttid; c < nun * 4 * B; c += kTeamThreads) {
-            const int s = c / (nun * 4), cs = c - s * (nun * 4);
             const int k = k_of(cs * 8);
-            const float* ag = p.acc_g + (size_t)s * N + k;
-            const float* au = p.acc_u + (size_t)s * N + k;
+            const float* ag = p.acc_g + (size_t)s * p.I + k;
+            const float* au = p.acc_u + (size_t)s * p.I + k;
             const float4 g0 = ld_cg4(ag), g1 = ld_cg4(ag + 4);
             const float4 a0 = ld_cg4(au), a1 = ld_cg4(au + 4);
             const uint32_t o0 = h2_as_u32(__floats2half2_rn(swiglu(g0.x, a0.x), swiglu(g0.y, a0.y)));
@@ -894,29 +739,94 @@ __device__ void stage_range_batch(const MegaParams& p, const TeamCtx& tc, int nk
             *reinterpret_cast<uint4*>(tc.xseg + (size_t)s * p.xs_stride + cs * 8) = perm8(o0, o1, o2, o3);
         }
     } else {
-        // attention output of sequence s: the records of (s, head) are those of the head's teams inside the sequence's teams
-#pragma unroll 1
-        for (int s = 0; s < B; ++s) {
-            const HeadTeams st = seq_teams(p, s, tc.nb);
-            __half* xseg = tc.xseg + (size_t)s * p.xs_stride;
-            for (int e = tc.ttid; e < nfeat; e += kTeamThreads) {
-                int k = k_of(e);
-                if constexpr (ACT) {
-                    if (perm != nullptr) k = perm[k];
+        // attention output: softmax-merge of the partial records (m, l, o[128]) of the head's teams (head_teams: contiguous, one
+        // record each; BATCH: the head's teams inside the sequence's teams, seq_teams).
+        constexpr int kBatch = 12;  // records fetched per round trip (a 7B head has 9 or 10 teams)
+        auto put = [&](__half* xseg, int e, float v) {
+            __half hv = __float2half_rn(v);
+            const int j8 = e & 7;
+            if (j8 & 1) hv = __hmul(hv, __float2half_rn(0.0625f));
+            xseg[(e & ~7) + perm_pos(j8)] = hv;
+        };
+        bool fast = false;
+        if constexpr (!BATCH) {
+            // heads of the range: [hA0, hA1] before the wrap, [0, hB1] after it
+            const int nA = min(nun, nk - ksb);
+            const int hA0 = (ksb * 32) / kHD, hA1 = ((ksb + nA) * 32 - 1) / kHD;
+            const int nslotA = hA1 - hA0 + 1, nslotB = (nun > nA) ? ((nun - nA) * 32 - 1) / kHD + 1 : 0;
+            fast = (nslotA + nslotB <= kTeamWarps) && (nun <= nk) && ((int)tc.nb / p.n_heads + 1 <= kBatch);
+            if constexpr (ACT) fast = fast && (perm == nullptr);
+            if (fast) {
+                // ONE round trip (per 256 features): every thread fetches the o values of its feature from all records of its head while
+                // warp w fetches (m, l) of the w-th head of the range and turns them into merge weights exp(m - M) / L.
+                float* wts = reinterpret_cast<float*>(tc.scratch);  // [kTeamWarps][kBatch]
+                float ov[kBatch];
+                int slot = 0;
+                auto fetch = [&](int e) {
+                    const bool active = e < nfeat;
+                    const int k = k_of(active ? e : 0);
+                    const int head = k / kHD, d = k - head * kHD;
+                    slot = ((e >> 5) < nA) ? head - hA0 : nslotA + head;
+                    const HeadTeams ht = head_teams(head, p.n_heads, tc.nb);
+#pragma unroll
+                    for (int i = 0; i < kBatch; ++i) ov[i] = (active && i < ht.count) ? ld_cg(p.part + (size_t)(ht.first + i) * kRec + 4 + d) : 0.f;
+                };
+                auto emit = [&](int e) {
+                    if (e < nfeat) {
+                        float O = 0.f;
+#pragma unroll
+                        for (int i = 0; i < kBatch; ++i) O = fmaf(wts[slot * kBatch + i], ov[i], O);
+                        put(tc.xseg, e, O);
+                    }
+                };
+                fetch(tc.ttid);
+                if (tc.wt < nslotA + nslotB) {
+                    const int lane = tc.lane;
+                    const int head = tc.wt < nslotA ? hA0 + tc.wt : tc.wt - nslotA;
+                    const HeadTeams ht = head_teams(head, p.n_heads, tc.nb);
+                    float m = -INFINITY, l = 0.f;
+                    if (lane < ht.count) {
+                        m = ld_cg(p.part + (size_t)(ht.first + lane) * kRec);
+                        l = ld_cg(p.part + (size_t)(ht.first + lane) * kRec + 1);
+                    }
+                    float M = m;
+#pragma unroll
+                    for (int o = 8; o > 0; o >>= 1) M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, o));  // lanes 0..15 hold the batch
+                    M = __shfl_sync(0xffffffffu, M, 0);
+                    const float w = (m == -INFINITY) ? 0.f : expf(m - M);
+                    float L = l * w;
+#pragma unroll
+                    for (int o = 8; o > 0; o >>= 1) L += __shfl_xor_sync(0xffffffffu, L, o);
+                    L = __shfl_sync(0xffffffffu, L, 0);
+                    if (lane < kBatch) wts[tc.wt * kBatch + lane] = w / L;
                 }
-                const int head = k / kHD, d = k - head * kHD;
-                HeadTeams ht = head_teams(head, p.n_heads, st.count);
-                ht.first += st.first;
-                __half hv = __float2half_rn(merge_records<12>(p, ht, d));
-                const int j8 = e & 7;
-                if (perm_scaled(j8)) hv = __hmul(hv, __float2half_rn(0.0625f));
-                xseg[(e & ~7) + perm_pos(j8)] = hv;
+                team_sync(tc.team);
+                emit(tc.ttid);
+                for (int e = tc.ttid + kTeamThreads; e - tc.ttid < nfeat; e += kTeamThreads) {  // wider ranges (13B, 65B): further round trips
+                    fetch(e);
+                    emit(e);
+                }
+            }
+        }
+        if (!fast) {
+            for (int s = 0; s < nbat; ++s) {
+                HeadTeams st{0, (int)tc.nb};
+                if constexpr (BATCH) st = seq_teams(p, s, tc.nb);
+                for (int e = tc.ttid; e < nfeat; e += kTeamThreads) {
+                    int k = k_of(e);
+                    if constexpr (ACT) {
+                        if (perm != nullptr) k = perm[k];  // regrouped rows: position k' of the matvec input is attention feature perm[k']
+                    }
+                    const int head = k / kHD, d = k - head * kHD;
+                    HeadTeams ht = head_teams(head, p.n_heads, st.count);
+                    ht.first += st.first;
+                    put(tc.xseg + (size_t)s * p.xs_stride, e, merge_records<kBatch>(p, ht, d));
+                }
             }
         }
     }
     team_sync(tc.team);
-#pragma unroll 1
-    for (int s = 0; s < B; ++s) compute_xsum(tc.xseg + (size_t)s * p.xs_stride, nun, tc.xsum_seg + s * (p.H / 32), tc.ttid, kTeamThreads);
+    for (int s = 0; s < nbat; ++s) compute_xsum(tc.xseg + (size_t)s * p.xs_stride, nun, tc.xsum_seg + s * (p.H / 32), tc.ttid, kTeamThreads);
     team_sync(tc.team);
 }
 
@@ -943,7 +853,7 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
     const uint32_t lane_s = (uint32_t)(kScaleOff + (tc.wt * 32 + col_l) * 2);      // scale of its column
     const uint32_t lane_z = (uint32_t)(kZeroOff + (tc.wt * 4 + (cg >> 1)) * 4);    // the qzeros word holding its zero
     const int zshift = (cg & 1) * 16 + t * 4;
-    const float unit = kSubnormal ? 16777216.0f : 1.0f;  // the accumulators are in units of 2^-24
+    const float unit = 16777216.0f;  // the accumulators are in units of 2^-24
     // BATCH: lane group g feeds sequence min(g, B - 1) to the tensor pipe and the lane finishes sequences 2t and 2t + 1 (clamped: lanes
     // past the batch read sequence B - 1 and drop their results); xsum_hi = offset of the step sums of sequence 2t + 1 from those of 2t
     const int B = p.batch;
@@ -954,10 +864,7 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
 #ifdef GPTQ_TRACE
             const long long stg0 = clock64();
 #endif
-            if constexpr (BATCH)
-                stage_range_batch<XMODE, ACT>(p, tc, nk, u, u_end, perm);
-            else
-                stage_range<XMODE, ACT>(p, tc, nk, u, u_end, perm);
+            stage_range<XMODE, ACT, BATCH>(p, tc, nk, u, u_end, perm);
 #ifdef GPTQ_TRACE
             if (g_mega_trace != nullptr && threadIdx.x == 0) g_mega_trace[blockIdx.x * 64 + 36 + XMODE] += (unsigned long long)(clock64() - stg0);
 #endif
@@ -1486,27 +1393,20 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         }
     };
 
-    // this step's RoPE angles (quant/fused_attn.py:43,91): freq_i = exp(i * inv_base) * pos
-    if constexpr (BATCH) {  // one row of angles per sequence
-        if (blockIdx.x == 0 && tid < 64 * nbat) {
-            const int s = tid >> 6, i = tid & 63;
-            const float f = expf((float)i * p.inv_base) * (float)step_pos(p, s);
-            p.rope_cs[s * kHD + i] = cosf(f);
-            p.rope_cs[s * kHD + 64 + i] = sinf(f);
-        }
-    } else if (blockIdx.x == 0 && tid < 64) {
-        const float f = expf((float)tid * p.inv_base) * (float)step_pos(p);
-        p.rope_cs[tid] = cosf(f);
-        p.rope_cs[64 + tid] = sinf(f);
+    // this step's RoPE angles, one row per sequence (quant/fused_attn.py:43,91): freq_i = exp(i * inv_base) * pos
+    if (blockIdx.x == 0 && tid < 64 * nbat) {
+        const int s = tid >> 6, i = tid & 63;
+        const float f = expf((float)i * p.inv_base) * (float)step_pos(p, s);
+        p.rope_cs[s * kHD + i] = cosf(f);
+        p.rope_cs[s * kHD + 64 + i] = sinf(f);
     }
 
-    // residual stream: every stage_norm reads buffer `cur` (or the embedding row) and writes the other one
-    const int token = min(max(p.tokens[0], 0), p.V - 1);
-    const __half* resid_src = p.embed + (size_t)token * p.H;
+    // residual stream: every stage_norm reads buffer `cur` (or, before the first layer, the embedding rows) and writes the other one
+    const __half* resid_src = nullptr;
     const float* resid_acc = nullptr;
     int cur = 1;
-    // BATCH: stage_norm for every sequence in turn (its tmp row and red_s are reused); sequence s reads row s of src / acc (or its own
-    // embedding row before the first layer) and writes row s of resid_out, xs and xsum
+    // stage_norm for every sequence in turn (its tmp row and red_s are reused); sequence s reads row s of src / acc (or its own
+    // embedding row while acc is nullptr) and writes row s of resid_out, xs and xsum
     auto stage_norms = [&](bool plain, const __half* src, const float* acc, const __half* norm_w, __half* resid_out, const int32_t* perm) {
 #pragma unroll 1
         for (int s = 0; s < nbat; ++s) {
@@ -1524,10 +1424,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         const LayerDesc& L = p.layers[l];
         // ---- Q ----
         MTRACE(l * 12 + 0);
-        if constexpr (BATCH)
-            stage_norms(false, resid_src, resid_acc, L.input_norm, p.resid[cur ^ 1], L.qkv_perm);
-        else
-            stage_norm<ACT, false>(p, resid_src, resid_acc, L.input_norm, p.resid[cur ^ 1], xs, xsum, tmp, red_s, L.qkv_perm);
+        stage_norms(false, resid_src, resid_acc, L.input_norm, p.resid[cur ^ 1], L.qkv_perm);
         MTRACE(l * 12 + 1);
         cur ^= 1;
         zero_slice(p.acc_g, nbat * p.I);  // last read by the previous layer's D
@@ -1564,10 +1461,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         sync_all_ranks(p.acc_o_loc, p.acc_o_peer);
         MTRACE(l * 12 + 7);
         // ---- G ----
-        if constexpr (BATCH)
-            stage_norms(false, p.resid[cur], p.acc_o, L.post_norm, p.resid[cur ^ 1], L.mlp_perm);
-        else
-            stage_norm<ACT, false>(p, p.resid[cur], p.acc_o, L.post_norm, p.resid[cur ^ 1], xs, xsum, tmp, red_s, L.mlp_perm);
+        stage_norms(false, p.resid[cur], p.acc_o, L.post_norm, p.resid[cur ^ 1], L.mlp_perm);
         cur ^= 1;
         MTRACE(l * 12 + 8);
         {
@@ -1594,10 +1488,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         resid_acc = p.acc_d;
     }
     // ---- L: final norm + lm_head ----
-    if constexpr (BATCH)
-        stage_norms(true, resid_src, resid_acc, p.final_norm, nullptr, nullptr);
-    else
-        stage_norm<false, true>(p, resid_src, resid_acc, p.final_norm, nullptr, xs, xsum, tmp, red_s, nullptr);
+    stage_norms(true, resid_src, resid_acc, p.final_norm, nullptr, nullptr);
     zero_slice(p.acc_g, nbat * p.I);
     zero_slice(p.acc_u, nbat * p.I);
     if constexpr (BATCH)
@@ -1606,50 +1497,11 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         run_lm_head(p, ring, tc, xs);
     sync_all_ranks(nullptr, nullptr);
     zero_slice(p.acc_d, nbat * p.H);
-    if constexpr (BATCH) {
-        if (blockIdx.x == 0 && tid == 0) p.bar[1] = gen;  // see below
-        if ((int)blockIdx.x < nbat && p.next_token != nullptr) argmax_row(p.logits + (size_t)blockIdx.x * p.V, p.V, p.next_token + blockIdx.x);  // CTA s: sequence s
-    } else if (blockIdx.x == 0) {
-        if (tid == 0) {  // every CTA has arrived at the last barrier: the counters rest at these values until the next launch
-            p.bar[1] = gen;
-            if (p.tp_size > 1) p.xbar_peer[p.tp_rank][32 * kMaxTP] = xgen;
-        }
-        if (p.next_token != nullptr) {  // greedy argmax (lowest index wins ties)
-            float best = -INFINITY;
-            int idx = 0x7fffffff;
-            for (int i = tid; i < p.V; i += kConsumers) {
-                const float v = __half2float(ld_cg_h(p.logits + i));  // written by other CTAs
-                if (v > best || (v == best && i < idx)) {
-                    best = v;
-                    idx = i;
-                }
-            }
-            __shared__ float sv[kConsumerWarps];
-            __shared__ int si[kConsumerWarps];
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-                if (ov > best || (ov == best && oi < idx)) {
-                    best = ov;
-                    idx = oi;
-                }
-            }
-            if (lane == 0) {
-                sv[warp] = best;
-                si[warp] = idx;
-            }
-            cta_sync();
-            if (tid == 0) {
-                for (int w = 1; w < kConsumerWarps; ++w)
-                    if (sv[w] > best || (sv[w] == best && si[w] < idx)) {
-                        best = sv[w];
-                        idx = si[w];
-                    }
-                p.next_token[0] = idx;
-            }
-        }
+    if (blockIdx.x == 0 && tid == 0) {  // every CTA has arrived at the last barrier: the counters rest at these values until the next launch
+        p.bar[1] = gen;
+        if (p.tp_size > 1) p.xbar_peer[p.tp_rank][32 * kMaxTP] = xgen;
     }
+    if ((int)blockIdx.x < nbat && p.next_token != nullptr) argmax_row(p.logits + (size_t)blockIdx.x * p.V, p.V, p.next_token + blockIdx.x);  // CTA s: sequence s
 }
 
 inline size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
@@ -1714,70 +1566,101 @@ bool mega_plan(const gptq_llama_model& m, int batch, int sms, size_t smem_max, s
     return true;
 }
 
-}  // namespace
 
-// ---------------------------------------------------------------------------------------------------
-bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st) {
-    if (st.batch < 1 || st.batch > kMaxBatch || m.n_layers > kMaxLayers || m.head_dim != kHD) return false;
-    if (st.batch > 1 && st.tp != nullptr) return false;  // tensor parallelism: batch 1 only
-    if (m.hidden % kSlabCols || m.intermediate % kSlabCols || m.hidden > 8192 || m.intermediate > 32768 || m.hidden % 64) return false;
-    if ((3 * m.n_heads * m.head_dim) % kSlabCols) return false;  // the (local) fused qkv width is dealt in 256-column slabs
+// Byte offsets of the persistent kernel's buffers in its scratch region.  The head (resid, acc_o, acc_d, xbar) depends on the hidden size
+// and the batch only, so it has the same layout on every tensor-parallel rank: peers address acc_o / acc_d / xbar of this rank through its
+// scratch base.  Every per-sequence buffer is [B][n] (gptq_b200.h); acc_qkv has room for 3 H (a tensor-parallel rank uses 3 Hq of it).
+struct MegaScratch {
+    size_t resid[2], acc_o, acc_d, xbar, acc_o_loc, acc_d_loc, acc_qkv, acc_g, acc_u, part, rope_cs, bar, total;
+};
+MegaScratch mega_scratch(const gptq_llama_model& m, int batch) {
+    const size_t B = (size_t)batch, H = (size_t)m.hidden, I = (size_t)m.intermediate;
+    MegaScratch s{};
+    auto take = [&](size_t bytes) {
+        const size_t o = s.total;
+        s.total += al256(bytes);
+        return o;
+    };
+    s.resid[0] = take(B * H * 2);
+    s.resid[1] = take(B * H * 2);
+    s.acc_o = take(B * H * 4);
+    s.acc_d = take(B * H * 4);
+    s.xbar = take((kMaxTP + 1) * 256);
+    s.acc_o_loc = take(H * 4);
+    s.acc_d_loc = take(H * 4);
+    s.acc_qkv = take(B * 3 * H * 4);
+    s.acc_g = take(B * I * 4);
+    s.acc_u = take(B * I * 4);
+    s.part = take((size_t)kMaxTeams * kRec * 4);
+    s.rope_cs = take(B * 128 * 4);
+    s.bar = take(256);
+    return s;
+}
+
+// the instantiation for this model and batch: ACT if any layer carries an input gather, BATCH at batch > 1
+using MegaKernel = void (*)(MegaParams);
+MegaKernel mega_kernel(const gptq_llama_model& m, int batch) {
+    const bool act = has_input_perm(m);
+    return batch > 1 ? (act ? llama_decode_mega_kernel<true, true> : llama_decode_mega_kernel<false, true>)
+                     : (act ? llama_decode_mega_kernel<true, false> : llama_decode_mega_kernel<false, false>);
+}
+
+// Launch plan of the persistent kernel for this step.  cudaErrorInvalidConfiguration: the step does not fit the kernel (the kernel chain
+// runs it).  Any other error: the device could not be queried, and only the shapes were checked.
+cudaError_t mega_step_plan(const gptq_llama_model& m, const gptq_llama_state& st, MegaPlan& pl) {
+    constexpr cudaError_t kNo = cudaErrorInvalidConfiguration;
+    if (st.batch < 1 || st.batch > kMaxBatch || m.n_layers > kMaxLayers || m.head_dim != kHD) return kNo;
+    if (st.batch > 1 && st.tp != nullptr) return kNo;  // tensor parallelism: batch 1 only
+    if (m.hidden % kSlabCols || m.intermediate % kSlabCols || m.hidden > 8192 || m.intermediate > 32768 || m.hidden % 64) return kNo;
+    if ((3 * m.n_heads * m.head_dim) % kSlabCols) return kNo;  // the (local) fused qkv width is dealt in 256-column slabs
     if (st.tp != nullptr) {
         const gptq_llama_tp& tp = *st.tp;
-        if (tp.size < 1 || tp.size > kMaxTP || tp.rank < 0 || tp.rank >= tp.size) return false;
-        if (tp.vocab_begin < 0 || tp.vocab_end > m.vocab || tp.vocab_begin >= tp.vocab_end) return false;
+        if (tp.size < 1 || tp.size > kMaxTP || tp.rank < 0 || tp.rank >= tp.size) return kNo;
+        if (tp.vocab_begin < 0 || tp.vocab_end > m.vocab || tp.vocab_begin >= tp.vocab_end) return kNo;
         for (int q = 0; q < tp.size; ++q)
-            if (q != tp.rank && (tp.peer_scratch[q] == nullptr || tp.peer_logits[q] == nullptr)) return false;
+            if (q != tp.rank && (tp.peer_scratch[q] == nullptr || tp.peer_logits[q] == nullptr)) return kNo;
     } else if (m.n_heads * m.head_dim != m.hidden) {
-        return false;
+        return kNo;
     }
     for (int l = 0; l < m.n_layers; ++l) {
         const gptq_llama_layer& ly = m.layers[l];
         const gptq_qweight* ws[5] = {&ly.qkv, &ly.o, &ly.gate, &ly.up, &ly.down};
         for (const gptq_qweight* w : ws) {
-            if (w->bits != 4 || w->groupsize <= 0 || w->groupsize % 32) return false;
+            if (w->bits != 4 || w->groupsize <= 0 || w->groupsize % 32) return kNo;
             if ((reinterpret_cast<uintptr_t>(w->qweight) & 15) || (reinterpret_cast<uintptr_t>(w->scales) & 15) || (reinterpret_cast<uintptr_t>(w->qzeros) & 15))
-                return false;
+                return kNo;
         }
-        if (ly.gate.groupsize != ly.up.groupsize) return false;
+        if (ly.gate.groupsize != ly.up.groupsize) return kNo;
     }
-    if ((reinterpret_cast<uintptr_t>(m.lm_head) & 15) || (reinterpret_cast<uintptr_t>(st.k_cache) & 15) || (reinterpret_cast<uintptr_t>(st.v_cache) & 15)) return false;
-    // the staging buffers of this batch must fit the current device (mega_plan; every instantiation has the same static shared memory),
-    // so that gptq_llama_decode_launches reports the kernel chain wherever the launch would fall back to it
-    int dev = 0, sms = 0, smem_optin = 0;
-    cudaFuncAttributes fa;
-    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
-        cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) == cudaSuccess &&
-        cudaFuncGetAttributes(&fa, llama_decode_mega_kernel<false, false>) == cudaSuccess) {
-        MegaPlan pl;
-        if (sms * kTeams > 1024 || !mega_plan(m, st.batch, sms, (size_t)smem_optin, fa.sharedSizeBytes, pl)) return false;
-    }
-    return true;
-}
-
-size_t mega_scratch_bytes(const gptq_llama_model& m, int batch, int max_seq) {
-    (void)max_seq;
-    const size_t max_teams = 1024;  // >= kTeams * SM count of any device this library runs on
-    const size_t B = (size_t)batch;
-    return al256(B * m.hidden * 2) * 2 + al256(B * 3 * m.hidden * 4) + al256(B * m.hidden * 4) * 2 + al256(B * m.intermediate * 4) * 2 +
-           al256(max_teams * kRec * 4) + al256(B * 128 * 4) + 256 + (kMaxTP + 1) * 256 + al256((size_t)m.hidden * 4) * 2;
-}
-
-cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state& st, uint8_t* scratch, cudaStream_t stream) {
-    static_assert(sizeof(MegaParams) < 32000, "kernel parameter space");
+    if ((reinterpret_cast<uintptr_t>(m.lm_head) & 15) || (reinterpret_cast<uintptr_t>(st.k_cache) & 15) || (reinterpret_cast<uintptr_t>(st.v_cache) & 15)) return kNo;
+    // the staging buffers of this batch must fit the current device
     int dev = 0, sms = 0, smem_optin = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess)
         return cudaErrorInvalidDevice;
-    bool any_perm = false;
-    for (int l = 0; l < m.n_layers; ++l) any_perm = any_perm || m.layers[l].qkv_perm != nullptr || m.layers[l].o_perm != nullptr || m.layers[l].mlp_perm != nullptr;
-    const int B = st.batch;
-    auto kernel = B > 1 ? (any_perm ? llama_decode_mega_kernel<true, true> : llama_decode_mega_kernel<false, true>)
-                        : (any_perm ? llama_decode_mega_kernel<true, false> : llama_decode_mega_kernel<false, false>);
     cudaFuncAttributes fa;
-    if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess) return cudaErrorInvalidDeviceFunction;
+    if (cudaFuncGetAttributes(&fa, mega_kernel(m, st.batch)) != cudaSuccess) return cudaErrorInvalidDeviceFunction;
+    if (sms * kTeams > kMaxTeams || !mega_plan(m, st.batch, sms, (size_t)smem_optin, fa.sharedSizeBytes, pl)) return kNo;
+    return cudaSuccess;
+}
+
+}  // namespace
+
+// ---------------------------------------------------------------------------------------------------
+bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st) {
     MegaPlan pl;
-    if (sms * kTeams > 1024 || !mega_plan(m, B, sms, (size_t)smem_optin, fa.sharedSizeBytes, pl)) return cudaErrorInvalidConfiguration;
+    return mega_step_plan(m, st, pl) != cudaErrorInvalidConfiguration;
+}
+
+size_t mega_scratch_bytes(const gptq_llama_model& m, int batch) { return mega_scratch(m, batch).total; }
+
+cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state& st, uint8_t* scratch, cudaStream_t stream) {
+    static_assert(sizeof(MegaParams) < 32000, "kernel parameter space");
+    MegaPlan pl;
+    cudaError_t e = mega_step_plan(m, st, pl);
+    if (e != cudaSuccess) return e;
+    const int B = st.batch;
+    const MegaKernel kernel = mega_kernel(m, B);
 
     MegaParams p{};
     p.n_layers = m.n_layers; p.H = m.hidden; p.Hq = m.n_heads * m.head_dim; p.I = m.intermediate; p.V = m.vocab; p.n_heads = m.n_heads;
@@ -1801,19 +1684,11 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     p.next_token = st.next_tokens;
     p.batch = B;
     p.xs_stride = xs_stride(m.hidden);
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        uint8_t* q = scratch + off;
-        off += al256(bytes);
-        return q;
-    };
-    // the head of the region has the same layout on every tensor-parallel rank (it depends on the hidden size only): peers address
-    // acc_o / acc_d / xbar of this rank through its scratch base.  Every per-sequence buffer is [B][n] (gptq_b200.h).
-    p.resid[0] = reinterpret_cast<__half*>(take((size_t)B * m.hidden * 2));
-    p.resid[1] = reinterpret_cast<__half*>(take((size_t)B * m.hidden * 2));
-    p.acc_o = reinterpret_cast<float*>(take((size_t)B * m.hidden * 4));
-    p.acc_d = reinterpret_cast<float*>(take((size_t)B * m.hidden * 4));
-    unsigned long long* xbar = reinterpret_cast<unsigned long long*>(take((kMaxTP + 1) * 256));
+    const MegaScratch ms = mega_scratch(m, B);
+    p.resid[0] = reinterpret_cast<__half*>(scratch + ms.resid[0]);
+    p.resid[1] = reinterpret_cast<__half*>(scratch + ms.resid[1]);
+    p.acc_o = reinterpret_cast<float*>(scratch + ms.acc_o);
+    p.acc_d = reinterpret_cast<float*>(scratch + ms.acc_d);
     const gptq_llama_tp* tp = st.tp;
     p.tp_size = tp != nullptr ? tp->size : 1;
     p.tp_rank = tp != nullptr ? tp->rank : 0;
@@ -1821,19 +1696,19 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     p.tp_exchange = (tp != nullptr && tp->size > 1) ? (tp->reduce_mode == 0 ? (tp->size > 4) : (tp->reduce_mode == 2)) : 0;
     for (int q = 0; q < p.tp_size; ++q) {
         uint8_t* base = (tp != nullptr && q != tp->rank) ? reinterpret_cast<uint8_t*>(tp->peer_scratch[q]) : scratch;
-        p.acc_o_peer[q] = reinterpret_cast<float*>(base + (reinterpret_cast<uint8_t*>(p.acc_o) - scratch));
-        p.acc_d_peer[q] = reinterpret_cast<float*>(base + (reinterpret_cast<uint8_t*>(p.acc_d) - scratch));
-        p.xbar_peer[q] = reinterpret_cast<unsigned long long*>(base + (reinterpret_cast<uint8_t*>(xbar) - scratch));
+        p.acc_o_peer[q] = reinterpret_cast<float*>(base + ms.acc_o);
+        p.acc_d_peer[q] = reinterpret_cast<float*>(base + ms.acc_d);
+        p.xbar_peer[q] = reinterpret_cast<unsigned long long*>(base + ms.xbar);
         p.logits_peer[q] = reinterpret_cast<__half*>((tp != nullptr && q != tp->rank) ? tp->peer_logits[q] : st.logits);
     }
-    p.acc_o_loc = reinterpret_cast<float*>(take((size_t)m.hidden * 4));
-    p.acc_d_loc = reinterpret_cast<float*>(take((size_t)m.hidden * 4));
-    p.acc_qkv = reinterpret_cast<float*>(take((size_t)B * 3 * p.Hq * 4));
-    p.acc_g = reinterpret_cast<float*>(take((size_t)B * m.intermediate * 4));
-    p.acc_u = reinterpret_cast<float*>(take((size_t)B * m.intermediate * 4));
-    p.part = reinterpret_cast<float*>(take((size_t)1024 * kRec * 4));
-    p.rope_cs = reinterpret_cast<float*>(take((size_t)B * 128 * 4));
-    p.bar = reinterpret_cast<unsigned long long*>(take(256));
+    p.acc_o_loc = reinterpret_cast<float*>(scratch + ms.acc_o_loc);
+    p.acc_d_loc = reinterpret_cast<float*>(scratch + ms.acc_d_loc);
+    p.acc_qkv = reinterpret_cast<float*>(scratch + ms.acc_qkv);
+    p.acc_g = reinterpret_cast<float*>(scratch + ms.acc_g);
+    p.acc_u = reinterpret_cast<float*>(scratch + ms.acc_u);
+    p.part = reinterpret_cast<float*>(scratch + ms.part);
+    p.rope_cs = reinterpret_cast<float*>(scratch + ms.rope_cs);
+    p.bar = reinterpret_cast<unsigned long long*>(scratch + ms.bar);
     // One tensor map per row stride serves every layer: class 0 = qkv (N = 3H), 1 = o and down (N = H), 2 = gate and up (N = I).
     // Its base is the lowest qweight address of the class; a matrix is addressed through the chunk coordinate (128-byte units).
     const int classN[3] = {3 * m.n_heads * m.head_dim, m.hidden, m.intermediate};
@@ -1857,7 +1732,6 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
             if (!encode_weight_map(&p.tmaps[3 * v + c], reinterpret_cast<const void*>(base[c]), rows_max[c], chunks, classN[c], v == 0 ? 4 * kStageSteps : 4))
                 return cudaErrorNotSupported;
     }
-    bool act = false;  // any act-order gather: the ACT instantiation (the plain one carries no trace of the feature)
     for (int l = 0; l < m.n_layers; ++l) {
         const gptq_llama_layer& ly = m.layers[l];
         bool aligned = true;
@@ -1883,10 +1757,8 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
         p.layers[l].qkv_perm = ly.qkv_perm;
         p.layers[l].o_perm = ly.o_perm;
         p.layers[l].mlp_perm = ly.mlp_perm;
-        act = act || ly.qkv_perm != nullptr || ly.o_perm != nullptr || ly.mlp_perm != nullptr;
     }
-    (void)act;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
     if (e != cudaSuccess) return e;
     int occ = 0;
     // cooperative launch: every CTA must be co-resident (one per SM); if the device cannot host them, the caller falls back to

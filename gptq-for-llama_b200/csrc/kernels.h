@@ -6,6 +6,13 @@
 
 namespace gptq {
 
+// Does any layer carry an act-order input gather (gptq_llama_layer)?  Only the persistent kernel implements them.
+inline bool has_input_perm(const gptq_llama_model& m) {
+    for (int l = 0; l < m.n_layers; ++l)
+        if (m.layers[l].qkv_perm != nullptr || m.layers[l].o_perm != nullptr || m.layers[l].mlp_perm != nullptr) return true;
+    return false;
+}
+
 struct QLinearArgs {
     const void* x;
     int64_t ldx;
@@ -46,7 +53,7 @@ cudaError_t launch_qlinear_gemm_tc(const QLinearArgs& a);
 
 // decode_mega.cu -- persistent single-kernel decode step (batch 1 to 8, int4 kernel-form layers)
 bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st);
-size_t mega_scratch_bytes(const gptq_llama_model& m, int batch, int max_seq);
+size_t mega_scratch_bytes(const gptq_llama_model& m, int batch);
 cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state& st, uint8_t* scratch, cudaStream_t stream);
 
 // elementwise.cu
