@@ -12,7 +12,8 @@ import math
 import torch
 
 from . import ops
-from ._lib import LlamaLayer, LlamaModel, LlamaState, LlamaTP, QWeight, check, lib
+from ._lib import LlamaLayer, LlamaModel, LlamaState, LlamaTP, check, lib
+from .ops import QLayerWeights
 
 c_void_p, c_int, c_float, c_size_t = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_size_t
 
@@ -26,51 +27,6 @@ LLAMA_SHAPES = {  # hidden, intermediate, layers, heads (SURVEY.md section 8)
     'tiny256': (256, 768, 2, 2),  # eligible for the persistent single-kernel path
     'tiny512': (512, 1024, 2, 4),  # shardable over 2 tensor-parallel ranks (2 heads and 2 slabs of 256 MLP columns each)
 }
-
-
-class QLayerWeights:
-    """Packed tensors of one QuantLinear (kept alive by the engine) + the act-order probe result."""
-
-    def __init__(self, qweight, scales, qzeros, g_idx, bits, groupsize):
-        self.qweight, self.scales, self.qzeros, self.g_idx, self.bits = qweight.contiguous(), scales.contiguous(), qzeros.contiguous(), g_idx.contiguous(), bits
-        K = qweight.shape[0] * 32 // bits
-        self.g_idx = self.g_idx[:K].contiguous()
-        self.groupsize = groupsize
-        self.hint = groupsize if ops.is_trivial_g_idx(self.g_idx, groupsize) else 0
-
-    def kernel_form(self, allow_perm=True):
-        """(layer in the layout the tuned int4 kernels take, input gather or None); see ops.kernel_form."""
-        plan = ops.kernel_form(self.qweight, self.scales, self.qzeros, self.g_idx, self.bits, self.groupsize, allow_perm=allow_perm)
-        if plan is None:
-            return self, None
-        return QLayerWeights(plan['qweight'], self.scales, plan['qzeros'], plan['g_idx'], plan['bits'], self.groupsize), plan['perm']
-
-    def permute_columns(self, perm):
-        """The same layer with output columns reordered: out'[:, j] = out[:, perm[j]] (used to fold the NEXT layer's input gather)."""
-        zeros = ops.unpack_qzeros(self.qzeros, self.bits).index_select(1, perm)
-        return QLayerWeights(self.qweight.index_select(1, perm), self.scales.index_select(1, perm), ops.pack_qzeros(zeros, self.bits), self.g_idx, self.bits,
-                             self.groupsize)
-
-    def column_slice(self, cols):
-        """The layer restricted to output columns `cols` (a LongTensor of whole groups of 8 consecutive columns): out[:, j] = full[:, cols[j]]."""
-        ipb = 32 // self.bits
-        assert cols.numel() % ipb == 0 and bool((cols.view(-1, ipb)[:, 0] % ipb == 0).all()), 'column shards must keep the packed zero words whole'
-        zcols = (cols.view(-1, ipb)[:, 0] // ipb).contiguous()
-        return QLayerWeights(self.qweight.index_select(1, cols), self.scales.index_select(1, cols), self.qzeros.index_select(1, zcols), self.g_idx, self.bits, self.groupsize)
-
-    def row_slice(self, k0, k1):
-        """The layer restricted to input features [k0, k1) (whole quantisation groups, no act-order): a K-shard whose partial outputs add up."""
-        assert self.hint == self.groupsize and k0 % self.groupsize == 0 and k1 % self.groupsize == 0 and self.bits in (2, 4, 8)
-        ipb, gs = 32 // self.bits, self.groupsize
-        g = (torch.arange(k1 - k0, device=self.qweight.device) // gs).to(torch.int32)
-        return QLayerWeights(self.qweight[k0 // ipb:k1 // ipb], self.scales[k0 // gs:k1 // gs], self.qzeros[k0 // gs:k1 // gs], g, self.bits, gs)
-
-    @classmethod
-    def from_module(cls, m):
-        return cls(m.qweight, m.scales, m.qzeros, m.g_idx, m.bits, m.groupsize)
-
-    def struct(self) -> QWeight:
-        return ops.make_qweight(self.qweight, self.scales, self.qzeros, self.g_idx, self.bits, self.hint)
 
 
 def random_qlayer(K, N, bits, groupsize, device, gen, act_order=False):
@@ -96,17 +52,17 @@ def random_qlayer(K, N, bits, groupsize, device, gen, act_order=False):
 
 def kernel_layers(layers, allow_perm=True):
     """Load-time preparation of a layer stack for the decode kernels (the stored tensors stay as they are):
-    2/3-bit fields widened to nibbles and act-order rows regrouped (ops.kernel_form).  The input gathers this needs are
+    2/3-bit fields widened to nibbles and act-order rows regrouped (QLayerWeights.kernel_form).  The input gathers this needs are
     returned per layer for the kernel (qkv, o, gate|up); down_proj's gather costs nothing at run time: it is folded into
     the column order of gate|up, whose SwiGLU output then comes out in down_proj's regrouped order.
     Returns (prepared layers, perms) or None when gate and up do not share their act-order map."""
     out, perms = [], []
     for ly in layers:
-        k, pm = {}, {}
-        for name in ('qkv', 'o', 'gate', 'up', 'down'):
-            k[name], pm[name] = ly[name].kernel_form(allow_perm)
-        if (pm['gate'] is None) != (pm['up'] is None) or (pm['gate'] is not None and not torch.equal(pm['gate'], pm['up'])):
+        mlp = ops.mlp_kernel_form(ly['gate'], ly['up'], allow_perm)
+        if mlp is None:
             return None
+        k = dict(zip(('gate', 'up'), mlp), **{name: ly[name].kernel_form(allow_perm) for name in ('qkv', 'o', 'down')})
+        pm = {name: k[name].perm for name in ('qkv', 'o', 'gate', 'down')}
         if pm['down'] is not None:
             k['gate'], k['up'] = k['gate'].permute_columns(pm['down']), k['up'].permute_columns(pm['down'])
         # per-input-feature vectors of a regrouped matvec are handed over in regrouped order
@@ -136,13 +92,7 @@ class LlamaDecoder:
         self.intermediate = layers[0]['gate'].qweight.shape[1]
         self.batch, self.max_seq = batch, max_seq
         with torch.cuda.device(self.dev):
-            # kernel-side view of the weights: nibble-widened 2/3-bit fields, regrouped act-order rows (+ input gathers)
-            prepared = kernel_layers(layers)
-            if prepared is None:
-                prepared = kernel_layers(layers, allow_perm=False)
-            self.klayers, self.perms = prepared
-            self._layer_arr = (LlamaLayer * len(layers))()
-            self._fill_layer_structs()
+            self._layer_arr = (LlamaLayer * len(layers))()  # filled below, once the kernel form of the layers is chosen
             m = LlamaModel()
             m.n_layers, m.hidden, m.n_heads, m.head_dim = len(layers), self.hidden, n_heads, self.head_dim
             m.intermediate, m.vocab, m.rms_eps, m.rope_base = self.intermediate, self.vocab, rms_eps, rope_base
@@ -173,10 +123,16 @@ class LlamaDecoder:
             if self._tp_struct is not None:
                 st.tp = ctypes.pointer(self._tp_struct)
             self.state = st
-            if any(p is not None for pm in self.perms for p in pm.values()) and self.launches_per_step() != 1:
-                # the input gathers exist only in the persistent kernel: act-order layers go back to their stored form
-                self.klayers, self.perms = kernel_layers(layers, allow_perm=False)
-                self._fill_layer_structs()
+            # kernel-side view of the weights: nibble-widened 2/3-bit fields, regrouped act-order rows (+ input gathers).  The gathers exist
+            # only in the persistent kernel: when gate and up cannot share one, or the step would not take that kernel, act-order layers
+            # keep their stored form.
+            for allow_perm in (True, False):
+                prepared = kernel_layers(layers, allow_perm)
+                if prepared is not None:
+                    self.klayers, self.perms = prepared
+                    self._fill_layer_structs()
+                    if all(p is None for pm in self.perms for p in pm.values()) or self.launches_per_step() == 1:
+                        break
         self.n_launches = None
         self.graph = None
         self._stream = torch.cuda.Stream(self.dev)
@@ -306,13 +262,12 @@ class LlamaDecoder:
         if total == 0:
             return ns
         H, nh, hd = self.hidden, self.n_heads, self.head_dim
-        w4 = lambda w: (w.qweight, w.scales, w.qzeros, w.g_idx)
         ids = [int(t) for p, n in zip(prompts, ns) for t in p[:n]]
         x = self.embed[torch.tensor(ids, device=self.dev)]  # [total, H]
         pos = torch.cat([torch.arange(n, dtype=torch.int64) for n in ns]).to(self.dev)[None, :]
         spans = [(b, sum(ns[:b]), n) for b, n in enumerate(ns) if n > 0]  # (sequence, first row, rows)
         for li, ly in enumerate(self.layers):
-            qkv = ops.matmul248(ops.rmsnorm(x, ly['input_norm'], self.model.rms_eps), *w4(ly['qkv']), ly['qkv'].bits, groupsize=ly['qkv'].hint).view(1, total, 3, nh, hd)
+            qkv = ops.matmul248(ops.rmsnorm(x, ly['input_norm'], self.model.rms_eps), *ly['qkv'].parts(), ly['qkv'].bits, groupsize=ly['qkv'].hint).view(1, total, 3, nh, hd)
             ops.rotate_half_(qkv[:, :, :2], pos, base=self.model.rope_base)
             atts = []
             for b, r0, n in spans:
@@ -321,9 +276,9 @@ class LlamaDecoder:
                 self.v_cache[li, b, :, :n] = v
                 atts.append(torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None], is_causal=True)[0].transpose(0, 1).reshape(n, H))
             att = atts[0] if len(atts) == 1 else torch.cat(atts)
-            x = x + ops.matmul248(att, *w4(ly['o']), ly['o'].bits, groupsize=ly['o'].hint)
-            h = ops.fused_mlp(ops.rmsnorm(x, ly['post_norm'], self.model.rms_eps), w4(ly['gate']), w4(ly['up']), ly['gate'].bits, ly['gate'].hint)
-            x = x + ops.matmul248(h, *w4(ly['down']), ly['down'].bits, groupsize=ly['down'].hint)
+            x = x + ops.matmul248(att, *ly['o'].parts(), ly['o'].bits, groupsize=ly['o'].hint)
+            h = ops.fused_mlp(ops.rmsnorm(x, ly['post_norm'], self.model.rms_eps), ly['gate'].parts(), ly['up'].parts(), ly['gate'].bits, ly['gate'].hint)
+            x = x + ops.matmul248(h, *ly['down'].parts(), ly['down'].bits, groupsize=ly['down'].hint)
         return ns
 
     def _check_prompts(self, prompts, max_new_tokens):
@@ -457,13 +412,9 @@ def from_hf_quant_model(model, batch=1, max_seq=2048, **kw):
         attn, mlp = layer.self_attn, layer.mlp
         if not isinstance(attn, quant.QuantLlamaAttention):
             raise ValueError('call quant.make_quant_attn(model) first')
-        if isinstance(mlp, quant.QuantLlamaMLP):
-            gate = QLayerWeights(mlp.gate_proj_qweight, mlp.gate_proj_scales, mlp.gate_proj_qzeros, mlp.gate_proj_g_idx, mlp.bits, mlp.groupsize)
-            up = QLayerWeights(mlp.up_proj_qweight, mlp.up_proj_scales, mlp.up_proj_qzeros, mlp.up_proj_g_idx, mlp.bits, mlp.groupsize)
-        else:
-            gate, up = QLayerWeights.from_module(mlp.gate_proj), QLayerWeights.from_module(mlp.up_proj)
+        gate, up = mlp.weights() if isinstance(mlp, quant.QuantLlamaMLP) else (mlp.gate_proj.weights(), mlp.up_proj.weights())
         L.append(
-            dict(qkv=QLayerWeights.from_module(attn.qkv_proj), o=QLayerWeights.from_module(attn.o_proj), gate=gate, up=up, down=QLayerWeights.from_module(mlp.down_proj),
+            dict(qkv=attn.qkv_proj.weights(), o=attn.o_proj.weights(), gate=gate, up=up, down=mlp.down_proj.weights(),
                  input_norm=layer.input_layernorm.weight.data.half().contiguous(), post_norm=layer.post_attention_layernorm.weight.data.half().contiguous()))
     cfg = model.config
     return LlamaDecoder(L, model.model.embed_tokens.weight.data.half(), model.model.norm.weight.data.half().contiguous(), model.lm_head.weight.data.half(),

@@ -8,6 +8,7 @@ rmsnorm                          <- TritonLlamaRMSNorm.forward, quant/triton_nor
 torch is plumbing here (device memory, current stream); all arithmetic happens in libgptq_b200.so.
 """
 import ctypes
+import functools
 
 import torch
 
@@ -223,37 +224,105 @@ def unpack_qzeros(qzeros, bits):
     return out
 
 
+class QLayerWeights:
+    """One packed GPTQ layer: (qweight, scales, qzeros, g_idx) with its bit width and groupsize, and `perm`, the input gather
+    x'[k'] = x[perm[k']] it expects (None for a stored layer; set on a kernel form with regrouped rows).  The one host object that
+    knows the packed layout: the groupsize hint, the kernel form of act-order and 2/3-bit layers, and column / row slices."""
+
+    def __init__(self, qweight, scales, qzeros, g_idx, bits, groupsize, perm=None):
+        K = qweight.shape[0] * 32 // bits
+        self.qweight, self.scales, self.qzeros = qweight.contiguous(), scales.contiguous(), qzeros.contiguous()
+        self.g_idx = g_idx[:K].contiguous()  # the fused qkv g_idx of the reference is 3K long; only the first K entries are read
+        self.bits, self.groupsize, self.perm = bits, groupsize, perm
+
+    def __getitem__(self, name):
+        """Field access by key (plan['qweight'], plan['perm'], ...), as callers of kernel_form and QuantLinear.kernel_plan read their result."""
+        return getattr(self, name)
+
+    @functools.cached_property
+    def hint(self) -> int:
+        """groupsize when g_idx is the trivial k // groupsize map (the kernels then skip the gather), else 0.  One device->host sync, once."""
+        return self.groupsize if is_trivial_g_idx(self.g_idx, self.groupsize) else 0
+
+    def parts(self):
+        """(qweight, scales, qzeros, g_idx): the layer as matmul248 and fused_mlp take it."""
+        return self.qweight, self.scales, self.qzeros, self.g_idx
+
+    def struct(self) -> QWeight:
+        return make_qweight(*self.parts(), self.bits, self.hint)
+
+    def kernel_form(self, allow_perm=True):
+        """The layer in the layout the tuned int4 kernels (matvec, wgmma GEMM, persistent decode kernel) take, derived at load time for a
+        layer they would otherwise leave to the generic kernel.  The stored tensors are not touched.
+
+        * act-order (arbitrary g_idx, gptq.py:210-216) with equal-sized groups, if allow_perm: the packed rows are regrouped so that every
+          group is contiguous (k' = rank of k in a stable sort by group); the caller feeds x'[k'] = x[perm[k']] (`.perm`, int64).  Every
+          weight keeps its own scale/zero, so the products are the same numbers; only the fp32 summation order changes.
+        * bits 2 or 3: every field is widened to a nibble (same integers, same stored-minus-one zeros), i.e. the layer is
+          re-expressed in the int4 layout.  This trades 33 % (int3) / 100 % (int2) more weight bytes for the tuned kernels;
+          a native 3-bit streaming kernel is the follow-up.
+
+        Returns self when neither applies."""
+        _require_cuda(self.qweight)
+        K, G, gs = self.g_idx.numel(), self.scales.shape[0], self.groupsize
+        perm, rows = None, None
+        if not self.hint:
+            g = self.g_idx.long()
+            if not allow_perm or K % gs or G * gs != K or not bool((torch.bincount(g, minlength=G) == gs).all()):
+                return self
+            perm = torch.argsort(g, stable=True)
+            rows = unpack_qweight(self.qweight, self.bits).index_select(0, perm)
+        widen = self.bits in (2, 3)
+        if perm is None and not widen:
+            return self
+        if rows is None:
+            rows = unpack_qweight(self.qweight, self.bits)
+        bits = 4 if widen else self.bits
+        qzeros = pack_qzeros(unpack_qzeros(self.qzeros, self.bits), 4) if widen else self.qzeros
+        g_triv = (torch.arange(K, device=self.qweight.device) // gs).to(torch.int32)
+        out = QLayerWeights(pack_qweight(rows, bits), self.scales, qzeros, g_triv, bits, gs, perm)
+        out.hint = gs  # trivial by construction: no probe
+        return out
+
+    def permute_columns(self, perm):
+        """The same layer with output columns reordered: out'[:, j] = out[:, perm[j]] (folds the NEXT layer's input gather)."""
+        zeros = unpack_qzeros(self.qzeros, self.bits).index_select(1, perm)
+        return QLayerWeights(self.qweight.index_select(1, perm), self.scales.index_select(1, perm), pack_qzeros(zeros, self.bits), self.g_idx, self.bits,
+                             self.groupsize, self.perm)
+
+    def column_slice(self, cols):
+        """The layer restricted to output columns `cols`: out[:, j] = full[:, cols[j]].  `cols` (a LongTensor) is made of whole runs of 32
+        consecutive columns starting at multiples of 32, so that every packed zero word is kept whole (bits of them per run)."""
+        runs = cols.view(-1, 32) if cols.numel() % 32 == 0 else None
+        if runs is None or not bool(((runs[:, :1] % 32 == 0) & (runs - runs[:, :1] == torch.arange(32, device=cols.device))).all()):
+            raise ValueError('column shards must be whole runs of 32 columns starting at multiples of 32')
+        zcols = (runs[:, :1] // 32 * self.bits + torch.arange(self.bits, device=cols.device)).reshape(-1)
+        return QLayerWeights(self.qweight.index_select(1, cols), self.scales.index_select(1, cols), self.qzeros.index_select(1, zcols), self.g_idx, self.bits,
+                             self.groupsize, self.perm)
+
+    def row_slice(self, k0, k1):
+        """The layer restricted to input features [k0, k1): a K-shard whose partial outputs add up.  Needs the trivial g_idx and
+        boundaries on whole quantisation groups and whole packed words."""
+        gs, bits = self.groupsize, self.bits
+        if not self.hint:
+            raise ValueError('row sharding of act-order layers is not supported (scales/zeros would have to be replicated)')
+        if k0 % gs or k1 % gs or k0 * bits % 32 or k1 * bits % 32:
+            raise ValueError(f'row shard [{k0}, {k1}) does not keep whole groups of {gs} and whole packed words')
+        g = (torch.arange(k1 - k0, device=self.g_idx.device) // gs).to(torch.int32)
+        return QLayerWeights(self.qweight[k0 * bits // 32:k1 * bits // 32], self.scales[k0 // gs:k1 // gs], self.qzeros[k0 // gs:k1 // gs], g, bits, gs)
+
+
 def kernel_form(qweight, scales, qzeros, g_idx, bits, groupsize, allow_perm=True):
-    """Load-time derived buffers that let the tuned int4 kernels (matvec, wgmma GEMM, persistent decode kernel)
-    serve a layer they would otherwise leave to the generic kernel.  The stored tensors are not touched.
+    """QLayerWeights.kernel_form of a stored layer, or None when the layer is already in that form or does not qualify."""
+    stored = QLayerWeights(qweight, scales, qzeros, g_idx, bits, groupsize)
+    kf = stored.kernel_form(allow_perm)
+    return None if kf is stored else kf
 
-    * act-order (arbitrary g_idx, gptq.py:210-216) with equal-sized groups: the packed rows are regrouped so that every
-      group is contiguous (k' = rank of k in a stable sort by group); the caller feeds x'[k'] = x[perm[k']].  Every
-      weight keeps its own scale/zero, so the products are the same numbers; only the fp32 summation order changes.
-    * bits 2 or 3: every field is widened to a nibble (same integers, same stored-minus-one zeros), i.e. the layer is
-      re-expressed in the int4 layout.  This trades 33 % (int3) / 100 % (int2) more weight bytes for the tuned kernels;
-      a native 3-bit streaming kernel is the follow-up.
 
-    Returns None when nothing applies, else a dict(qweight, qzeros, g_idx, bits, perm) -- perm is an int64 tensor or None.
-    """
-    _require_cuda(qweight)
-    K, N = qweight.shape[0] * 32 // bits, qweight.shape[1]
-    trivial = is_trivial_g_idx(g_idx, groupsize)
-    perm, rows = None, None
-    if not trivial:
-        g = g_idx[:K].long()
-        G = scales.shape[0]
-        if not allow_perm or K % groupsize or G * groupsize != K or not bool((torch.bincount(g, minlength=G) == groupsize).all()):
-            return None
-        perm = torch.argsort(g, stable=True)
-        rows = unpack_qweight(qweight, bits).index_select(0, perm)
-    widen = bits in (2, 3)
-    if perm is None and not widen:
+def mlp_kernel_form(gate, up, allow_perm=True):
+    """Kernel forms (gate', up') of gate_proj and up_proj (QLayerWeights.kernel_form).  The two see the same input, so they must share
+    one input gather: None when their act-order maps differ."""
+    kg, ku = gate.kernel_form(allow_perm), up.kernel_form(allow_perm)
+    if (kg.perm is None) != (ku.perm is None) or (kg.perm is not None and not torch.equal(kg.perm, ku.perm)):
         return None
-    new_bits = 4 if widen else bits
-    if rows is None:
-        rows = unpack_qweight(qweight, bits)
-    new_qweight = pack_qweight(rows, new_bits)
-    new_qzeros = pack_qzeros(unpack_qzeros(qzeros, bits), 4) if widen else qzeros
-    g_triv = (torch.arange(K, device=qweight.device) // groupsize).to(torch.int32)
-    return dict(qweight=new_qweight, qzeros=new_qzeros, g_idx=g_triv, bits=new_bits, perm=perm)
+    return kg, ku

@@ -21,6 +21,8 @@ import torch
 import torch.distributed as dist
 import torch.nn as nn
 
+from .ops import QLayerWeights
+
 
 def column_partition(N: int, world: int, align: int = 32):
     """Boundaries [n_0 .. n_world] splitting N into `world` contiguous shards of multiples of `align` columns."""
@@ -42,26 +44,20 @@ def row_partition(K: int, groupsize: int, world: int):
 
 def shard_columns(qweight, scales, qzeros, g_idx, bits: int, rank: int, world: int, bias=None):
     """This rank's column shard of a packed layer: (qweight, scales, qzeros, g_idx, bias)."""
-    N = qweight.shape[1]
-    b = column_partition(N, world)
+    b = column_partition(qweight.shape[1], world)
     n0, n1 = b[rank], b[rank + 1]
-    z0, z1 = n0 * bits // 32, n1 * bits // 32
-    return (qweight[:, n0:n1].contiguous(), scales[:, n0:n1].contiguous(), qzeros[:, z0:z1].contiguous(), g_idx.clone(),
-            bias[n0:n1].contiguous() if bias is not None else None)
+    # a column slice does not depend on the groupsize (0: no hint is ever asked of this layer)
+    w = QLayerWeights(qweight, scales, qzeros, g_idx, bits, 0).column_slice(torch.arange(n0, n1, device=qweight.device))
+    return w.qweight, w.scales, w.qzeros, w.g_idx.clone(), bias[n0:n1].contiguous() if bias is not None else None
 
 
 def shard_rows(qweight, scales, qzeros, g_idx, bits: int, groupsize: int, rank: int, world: int):
     """This rank's row (K) shard: (qweight, scales, qzeros, g_idx_local, (k0, k1)).  Requires the trivial g_idx."""
-    K = qweight.shape[0] * 32 // bits
-    ref = torch.arange(K, device=g_idx.device) // groupsize
-    if not torch.equal(g_idx[:K].long(), ref):
-        raise ValueError('row sharding of act-order layers is not supported (scales/zeros would have to be replicated)')
-    b = row_partition(K, groupsize, world)
+    w = QLayerWeights(qweight, scales, qzeros, g_idx, bits, groupsize)
+    b = row_partition(w.g_idx.numel(), groupsize, world)
     k0, k1 = b[rank], b[rank + 1]
-    r0, r1 = k0 * bits // 32, k1 * bits // 32
-    g0, g1 = k0 // groupsize, k1 // groupsize
-    g_local = (torch.arange(k1 - k0, device=g_idx.device) // groupsize).to(torch.int32)
-    return qweight[r0:r1].contiguous(), scales[g0:g1].contiguous(), qzeros[g0:g1].contiguous(), g_local, (k0, k1)
+    w = w.row_slice(k0, k1)
+    return w.qweight, w.scales, w.qzeros, w.g_idx, (k0, k1)
 
 
 class TPQuantLinear(nn.Module):

@@ -4,7 +4,6 @@ Mirrors quant/fused_mlp.py of the reference (QuantLlamaMLP :177-238, make_fused_
 autotune_warmup_fused :256-288); the gate/up contraction + SwiGLU epilogue is one CUDA kernel
 (gptq_fused_mlp_fwd) instead of ``fusedmatmul_248_kernel`` (:84-168).
 """
-import torch
 import torch.nn as nn
 
 from gptq_b200 import ops
@@ -35,47 +34,46 @@ class QuantLlamaMLP(nn.Module):
         self.maxq = gate_proj.maxq
         self.groupsize = gate_proj.groupsize
         self.down_proj = down_proj
-        self._g_key = None
-        self._g_trivial = False
-        self._plan = None  # (cache key, derived gate/up buffers for the tuned kernels or None)
+        self._view = None  # {'key', 'weights': (gate, up) as ops.QLayerWeights, 'plan': their kernel form once asked for}
+
+    def _cached_view(self):
+        # like QuantLinear's: keyed on the buffers, which fused2cuda / fused2cpu and .cuda() replace
+        bufs = [getattr(self, f'{proj}_{part}') for proj in ('gate_proj', 'up_proj') for part in _PARTS]
+        key = [(t.device, t.data_ptr(), t._version) for t in bufs]
+        if self._view is None or self._view['key'] != key:
+            self._view = dict(key=key, weights=(ops.QLayerWeights(*bufs[:4], self.bits, self.groupsize), ops.QLayerWeights(*bufs[4:], self.bits, self.groupsize)))
+        return self._view
+
+    def weights(self):
+        """(gate, up) as gptq_b200.ops.QLayerWeights (cached until a buffer is replaced or modified)."""
+        return self._cached_view()['weights']
 
     def kernel_plan(self):
-        """gate/up in the layout of the tuned int4 kernels (ops.kernel_form: act-order rows regrouped, 2/3-bit fields widened) when
-        both qualify and share their input gather (same input, hence the same act-order map); None otherwise."""
-        key = tuple((t.data_ptr(), t._version) for t in (self.gate_proj_qweight, self.up_proj_qweight, self.gate_proj_g_idx, self.up_proj_g_idx))
-        if self._plan is None or self._plan[0] != key:
-            pg = ops.kernel_form(self.gate_proj_qweight, self.gate_proj_scales, self.gate_proj_qzeros, self.gate_proj_g_idx, self.bits, self.groupsize)
-            pu = ops.kernel_form(self.up_proj_qweight, self.up_proj_scales, self.up_proj_qzeros, self.up_proj_g_idx, self.bits, self.groupsize)
-            ok = pg is not None and pu is not None and ((pg['perm'] is None and pu['perm'] is None) or
-                                                        (pg['perm'] is not None and pu['perm'] is not None and torch.equal(pg['perm'], pu['perm'])))
-            self._plan = (key, (pg, pu) if ok else None)
-        return self._plan[1]
+        """(gate, up) in the layout of the tuned int4 kernels (ops.mlp_kernel_form: act-order rows regrouped, 2/3-bit fields widened;
+        their shared input gather in `perm`) when both need it and share their input gather; None otherwise."""
+        view = self._cached_view()
+        if 'plan' not in view:
+            gate, up = view['weights']
+            plan = ops.mlp_kernel_form(gate, up)
+            # the fused kernel takes one bit width: a pair with a layer left as stored runs as stored
+            view['plan'] = None if plan is None or plan[0] is gate or plan[1] is up else plan
+        return view['plan']
 
     def forward(self, x):
         return self.down_proj(self.triton_llama_mlp(x))
 
     def groupsize_hint(self):
-        g1, g2 = self.gate_proj_g_idx, self.up_proj_g_idx
-        key = (g1.data_ptr(), g1._version, g2.data_ptr(), g2._version, g1.device)
-        if key != self._g_key:
-            self._g_trivial = ops.is_trivial_g_idx(g1, self.groupsize) and ops.is_trivial_g_idx(g2, self.groupsize)
-            self._g_key = key
-        return self.groupsize if self._g_trivial else 0
+        gate, up = self.weights()
+        return min(gate.hint, up.hint)  # groupsize when both g_idx are trivial, else 0
 
     def triton_llama_mlp(self, x):
         """fp16 [..., intermediate] = silu(x.Wgate) * (x.Wup).  The name is the reference's (:206); no Triton is involved."""
         out_shape = x.shape[:-1] + (self.intermediate_size, )
-        plan = self.kernel_plan() if self.gate_proj_qweight.is_cuda else None
-        if plan is not None:
-            pg, pu = plan
-            x2 = x.reshape(-1, x.shape[-1])
-            if pg['perm'] is not None:
-                x2 = x2.index_select(1, pg['perm'])
-            c = ops.fused_mlp(x2, (pg['qweight'], self.gate_proj_scales, pg['qzeros'], pg['g_idx']), (pu['qweight'], self.up_proj_scales, pu['qzeros'], pu['g_idx']),
-                              pg['bits'], self.groupsize)
-            return c.reshape(out_shape)
-        c = ops.fused_mlp(x.reshape(-1, x.shape[-1]), tuple(getattr(self, f'gate_proj_{p}') for p in _PARTS),
-                          tuple(getattr(self, f'up_proj_{p}') for p in _PARTS), self.bits, self.groupsize_hint())
+        x2 = x.reshape(-1, x.shape[-1])
+        gate, up = self.kernel_plan() or self.weights()
+        if gate.perm is not None:  # regrouped rows: x is gathered to match
+            x2 = x2.index_select(1, gate.perm)
+        c = ops.fused_mlp(x2, gate.parts(), up.parts(), gate.bits, min(gate.hint, up.hint))
         return c.reshape(out_shape)
 
     fused_llama_mlp = triton_llama_mlp

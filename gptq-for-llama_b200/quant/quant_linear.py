@@ -70,9 +70,7 @@ class QuantLinear(nn.Module):
             self.register_buffer('bias', torch.zeros((outfeatures), dtype=torch.float16))
         else:
             self.bias = None
-        self._g_key = None  # cache key of the act-order probe
-        self._g_trivial = False
-        self._sorted = None  # (cache key, ops.kernel_form result), derived lazily
+        self._view = None  # {'key', 'weights': ops.QLayerWeights of the buffers, 'plan': its kernel form once asked for}
 
     # ------------------------------------------------------------------ packing (offline)
     def pack(self, linear, scales, zeros, g_idx=None):
@@ -102,41 +100,40 @@ class QuantLinear(nn.Module):
         self.scales = scales_h.to(home)
         if linear.bias is not None:
             self.bias = linear.bias.detach().clone().half().to(home)
-        self._g_key = None
-        self._sorted = None  # derived kernel-form buffers belong to the tensors that were just replaced
 
     # ------------------------------------------------------------------ forward
+    def _cached_view(self):
+        # pack(), load_state_dict and .cuda() replace or modify the buffers: the view, and what is derived from it, is rebuilt then
+        key = [(t.device, t.data_ptr(), t._version) for t in (self.qweight, self.scales, self.qzeros, self.g_idx)]
+        if self._view is None or self._view['key'] != key:
+            self._view = dict(key=key, weights=ops.QLayerWeights(self.qweight, self.scales, self.qzeros, self.g_idx, self.bits, self.groupsize))
+        return self._view
+
+    def weights(self):
+        """The buffers as one gptq_b200.ops.QLayerWeights (cached until a buffer is replaced or modified)."""
+        return self._cached_view()['weights']
+
     def groupsize_hint(self):
         """groupsize if g_idx is the trivial k // groupsize map (lets the kernels skip the gather), else 0.
-        The probe costs one device->host sync and is cached until g_idx is replaced."""
-        g = self.g_idx
-        key = (g.data_ptr(), g._version, g.device)
-        if key != self._g_key:
-            self._g_trivial = ops.is_trivial_g_idx(g[:self.infeatures], self.groupsize)
-            self._g_key = key
-        return self.groupsize if self._g_trivial else 0
+        The probe costs one device->host sync and is cached until a buffer is replaced."""
+        return self.weights().hint
 
     def kernel_plan(self):
-        """Derived buffers (gptq_b200.ops.kernel_form) that route an act-order and/or 2/3-bit layer to the tuned int4
-        kernels without touching the stored tensors; None when the layer needs none or does not qualify."""
-        key = (self.g_idx.data_ptr(), self.g_idx._version, self.qweight.data_ptr(), self.qweight._version, self.qzeros.data_ptr())
-        if self._sorted is None or self._sorted[0] != key:
-            self._sorted = (key, ops.kernel_form(self.qweight, self.scales, self.qzeros, self.g_idx, self.bits, self.groupsize))
-        return self._sorted[1]
-
-    act_order_plan = kernel_plan  # earlier name
+        """The derived layer (ops.QLayerWeights.kernel_form, with its input gather in `perm`) that routes an act-order and/or 2/3-bit layer to
+        the tuned int4 kernels without touching the stored tensors; None when the layer needs none or does not qualify."""
+        view = self._cached_view()
+        if 'plan' not in view:
+            form = view['weights'].kernel_form()
+            view['plan'] = None if form is view['weights'] else form
+        return view['plan']
 
     def forward(self, x):
         out_shape = x.shape[:-1] + (self.outfeatures, )
         x2 = x.reshape(-1, x.shape[-1])
-        plan = self.kernel_plan() if self.qweight.is_cuda else None
-        if plan is not None:  # regrouped rows (+ gathered x) and/or nibble-widened fields -> the tuned trivial-g_idx int4 kernels
-            if plan['perm'] is not None:
-                x2 = x2.index_select(1, plan['perm'])
-            out = QuantLinearFunction.apply(x2, plan['qweight'], self.scales, plan['qzeros'], plan['g_idx'], plan['bits'], 2**plan['bits'] - 1, self.bias,
-                                            self.groupsize)
-            return out.reshape(out_shape)
-        out = QuantLinearFunction.apply(x2, self.qweight, self.scales, self.qzeros, self.g_idx, self.bits, self.maxq, self.bias, self.groupsize_hint())
+        w = self.kernel_plan() or self.weights()
+        if w.perm is not None:  # regrouped rows: x is gathered to match
+            x2 = x2.index_select(1, w.perm)
+        out = QuantLinearFunction.apply(x2, *w.parts(), w.bits, 2**w.bits - 1, self.bias, w.hint)
         return out.reshape(out_shape)
 
 
@@ -157,12 +154,12 @@ make_quant = make_quant_linear  # older / cuda-branch entry-point name
 
 def autotune_warmup_linear(model, transpose=False):
     """Kept for API compatibility (quant_linear.py:393-423).  There is nothing to autotune: dispatch is
-    static.  The pass only primes each layer's act-order probe so that the first forward (possibly under
-    CUDA-graph capture) does no device->host sync."""
+    static.  The pass only primes each layer's act-order probe and kernel form (act-order rows regrouped, 2- and 3-bit
+    fields widened) so that the first forward (possibly under CUDA-graph capture) does no device->host sync."""
     n = 0
     for _, m in model.named_modules():
         if isinstance(m, QuantLinear) and m.qweight.is_cuda:
             m.groupsize_hint()
-            m.kernel_plan()  # regroup act-order rows / widen 2- and 3-bit fields once, at load time
+            m.kernel_plan()
             n += 1
     return n

@@ -36,12 +36,12 @@ def test_quantlinear_module_forward_and_backward(bits, act):
     assert_rel_close(xd.grad, gref, what='module bwd')
 
 
-def _tiny_quant_llama(bits=4, gs=32, act=False):
+def _tiny_quant_llama(bits=4, gs=32, act=False, hidden=128, intermediate=352, heads=4):
     import quant
     import utils
     from transformers import LlamaConfig, LlamaForCausalLM
-    cfg = LlamaConfig(hidden_size=128, intermediate_size=352, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=4, vocab_size=256,
-                      max_position_embeddings=128)
+    cfg = LlamaConfig(hidden_size=hidden, intermediate_size=intermediate, num_hidden_layers=2, num_attention_heads=heads, num_key_value_heads=heads,
+                      vocab_size=256, max_position_embeddings=128)
     torch.manual_seed(0)
     model = LlamaForCausalLM(cfg).half().eval()
     layers = utils.find_layers(model)
@@ -108,6 +108,32 @@ def test_load_quant_pipeline_on_tiny_llama(bits, act):
         assert_rel_close(out.logits[0], ref_logits[0, :8], rel=2e-2, what='prefill logits')
         step = model(ids[:, 8:9].cuda(), past_key_values=out.past_key_values, use_cache=True)
         assert_rel_close(step.logits[0, 0], ref_logits[0, 8], rel=2e-2, what='decode logits')
+
+
+@pytest.mark.parametrize('bits', [4, 3])
+def test_engine_and_modules_derive_the_same_kernel_form(bits):
+    """engine.from_hf_quant_model and the quant modules of one act-order model derive the kernel form of every layer through the same
+    owner (ops.QLayerWeights, ops.mlp_kernel_form): the decoder's layers and input gathers equal the modules' kernel_plan()s.  head_dim 128
+    so that the decoder takes the persistent kernel and keeps its gathers."""
+    import quant
+    from gptq_b200 import engine, ops
+    gs = 32
+    model = _tiny_quant_llama(bits=bits, gs=gs, act=True, hidden=256, intermediate=768, heads=2)
+    quant.make_quant_attn(model)
+    quant.make_quant_norm(model)
+    quant.make_fused_mlp(model)
+    model = model.cuda()
+    dec = engine.from_hf_quant_model(model, max_seq=16, use_graph=False)
+    assert dec.launches_per_step() == 1
+    for layer, kl, pm in zip(model.model.layers, dec.klayers, dec.perms):
+        plans = {'qkv': layer.self_attn.qkv_proj.kernel_plan(), 'o': layer.self_attn.o_proj.kernel_plan(), 'down': layer.mlp.down_proj.kernel_plan()}
+        for name, w in plans.items():
+            assert kl[name].bits == w.bits == 4 and all(torch.equal(a, b) for a, b in zip(kl[name].parts(), w.parts())), name
+            assert name == 'down' or torch.equal(pm[name], w.perm.int()), name
+        gate, up = layer.mlp.kernel_plan()
+        assert torch.equal(pm['gate'], gate.perm.int()) and torch.equal(gate.perm, up.perm)
+        for name, w in (('gate', gate), ('up', up)):  # the decoder folds down_proj's gather into the column order of gate|up
+            assert torch.equal(ops.dequant(*kl[name].parts(), 4, gs), ops.dequant(*w.parts(), 4, gs)[:, plans['down'].perm]), name
 
 
 # ----------------------------------------------------------------------------- full BASELINE sizes: size-independent properties

@@ -44,6 +44,32 @@ def test_shards_reassemble():
         tp.shard_rows(qw, s, qz, O.make_g_idx(K, gs, True, torch.Generator().manual_seed(0)), bits, gs, 0, 2)
 
 
+@pytest.mark.parametrize('bits', [3, 2])
+def test_narrow_bit_slices_reassemble(bits):
+    """column_slice / row_slice of 3- and 2-bit layers (whole 32-column runs, whole packed words) dequantise exactly to the corresponding
+    block: the tensor-parallel shards, scattered column runs like the decode engine's per-head qkv shards, and an uneven row shard."""
+    from gptq_b200 import ops, tp
+    K, N, gs = 512, 256, 128
+    qw, s, qz, g, _ = O.random_packed(K, N, bits, gs, seed=bits)
+    W = O.dequant(qw, s, qz, g, bits)
+    b = tp.column_partition(N, 4)
+    cols = [O.dequant(*tp.shard_columns(qw, s, qz, g, bits, r, 4)[:4], bits) for r in range(4)]
+    assert all(torch.equal(c, W[:, b[r]:b[r + 1]]) for r, c in enumerate(cols))
+    for r in range(4):
+        sqw, ss, sqz, sg, (k0, k1) = tp.shard_rows(qw, s, qz, g, bits, gs, r, 4)
+        assert torch.equal(O.dequant(sqw, ss, sqz, sg, bits), W[k0:k1])
+    w = ops.QLayerWeights(qw, s, qz, g, bits, gs)
+    c = torch.cat([torch.arange(32, 64), torch.arange(160, 256)])
+    assert torch.equal(O.dequant(*w.column_slice(c).parts(), bits), W[:, c])
+    rows = w.row_slice(128, 512)
+    assert torch.equal(O.dequant(*rows.parts(), bits), W[128:512]) and rows.hint == gs
+    for bad in (torch.arange(16, 48), torch.arange(0, 48)):
+        with pytest.raises(ValueError):
+            w.column_slice(bad)
+    with pytest.raises(ValueError):
+        w.row_slice(64, 256)
+
+
 def _worker(rank, world, port, q):
     os.environ.update(MASTER_ADDR='127.0.0.1', MASTER_PORT=str(port))
     dist.init_process_group('gloo', rank=rank, world_size=world)
