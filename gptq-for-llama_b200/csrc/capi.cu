@@ -149,6 +149,19 @@ int gptq_unpack_qzeros(const int32_t* qzeros, int32_t* zeros_m1, int G, int N, i
     return pack_common(qzeros, zeros_m1, N, G, bits, true, false, stream);
 }
 
+size_t gptq_lm_head_logprob_workspace_bytes(int M, int V) { return lm_head_logprob_workspace_bytes(M, V); }
+
+int gptq_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int K, int V, const int32_t* targets, float* logprob,
+                         void* workspace, size_t ws_bytes, gptq_stream_t stream) {
+    if (x == nullptr || w == nullptr || targets == nullptr || logprob == nullptr) return GPTQ_ERR_NULL;
+    if (K <= 0 || K % 64 != 0 || V <= 0 || M < 0 || ldx < K || ldw < K) return GPTQ_ERR_SHAPE;
+    if ((int64_t)ceil_div(M, 256) * ceil_div(V, 128) > 0x7fffffffLL) return GPTQ_ERR_SHAPE;  // one CTA per 256 x 128 tile, 1-D grid
+    if (!aligned(x, 16) || !aligned(w, 16) || ldx % 8 != 0 || ldw % 8 != 0) return GPTQ_ERR_ALIGN;  // TMA: 16-byte base and row pitch
+    if (M == 0) return GPTQ_OK;
+    if (workspace == nullptr || !aligned(workspace, 256) || ws_bytes < lm_head_logprob_workspace_bytes(M, V)) return GPTQ_ERR_WORKSPACE;
+    return cuda_status(launch_lm_head_logprob(x, ldx, w, ldw, M, K, V, targets, logprob, workspace, static_cast<cudaStream_t>(stream)));
+}
+
 int gptq_ipc_alloc(size_t bytes, void** ptr, unsigned char handle[64]) {
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "handle size");
     if (ptr == nullptr || handle == nullptr || bytes == 0) return GPTQ_ERR_NULL;

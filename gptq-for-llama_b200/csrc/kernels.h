@@ -51,6 +51,11 @@ cudaError_t launch_qlinear_skinny(const QLinearArgs& a, bool pdl);
 bool gemm_tc_supported(const QLinearArgs& a);
 cudaError_t launch_qlinear_gemm_tc(const QLinearArgs& a);
 
+// lm_head_logprob.cu -- per-row log-probability of a target through the fp16 lm_head (wgmma + fused log-softmax), and its combine pass
+size_t lm_head_logprob_workspace_bytes(int M, int V);
+cudaError_t launch_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int K, int V, const int32_t* targets, float* logprob,
+                                   void* workspace, cudaStream_t stream);
+
 // decode_mega.cu -- persistent single-kernel decode step (batch 1 to 8, int4 kernel-form layers)
 bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st);
 size_t mega_scratch_bytes(const gptq_llama_model& m, int batch);

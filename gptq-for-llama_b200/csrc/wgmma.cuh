@@ -1,0 +1,71 @@
+// Hopper tensor-core helpers shared by the wgmma kernels (qgemm_wgmma.cu, lm_head_logprob.cu): shared-memory matrix
+// descriptors, the wgmma fence / commit / wait protocol, the m64n128k16 f16 MMA, and the TMA tensor map of a K-major fp16 matrix.
+#pragma once
+#include <cuda.h>
+#include <cudaTypedefs.h>
+
+#include "common.cuh"
+
+namespace gptq {
+
+constexpr int kWgmmaBK = 64;  // K step of one SWIZZLE_128B atom row: 64 halves = 128 B
+
+// wgmma shared-memory matrix descriptor, K-major, SWIZZLE_128B: start >> 4, LBO unused (1), SBO = 1024 B between 8-row groups,
+// layout type 1 (128-byte swizzle) at bit 62.  Tiles are 1024 B aligned (base offset 0); +32 B (K = 16) inside the atom = +2.
+__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr) {
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// the accumulators must stay in place while a wgmma that writes them is in flight
+__device__ __forceinline__ void pin(float (&d)[64]) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 128] += A[64 x 16] . B[16 x 128], both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, "
+        "%30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, "
+        "%58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+          "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+          "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(1));
+}
+
+// TMA tensor map of an fp16 [rows, K] matrix with `ld` elements between rows (K-major, like the wgmma operands): box 64 (k) x 128 rows,
+// SWIZZLE_128B; rows past `rows` read as zeros.  cuTensorMapEncodeTiled is reached through the runtime's driver entry point (libcuda is
+// not linked: the library must load without a driver).
+inline bool make_kmajor_tensor_map(CUtensorMap* tm, const void* base, int rows, int K, int64_t ld) {
+    static PFN_cuTensorMapEncodeTiled encode = []() -> PFN_cuTensorMapEncodeTiled {
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) return nullptr;
+        return reinterpret_cast<PFN_cuTensorMapEncodeTiled>(fn);
+    }();
+    if (encode == nullptr) return false;
+    const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};  // innermost first
+    const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};            // bytes between rows
+    const cuuint32_t box[2] = {(cuuint32_t)kWgmmaBK, 128};         // 64 halves (128 B) x 128 rows
+    const cuuint32_t estr[2] = {1, 1};
+    return encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+}  // namespace gptq

@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('GPTQ_B200_LIB') or os.path.join(os.path.dirname(_HERE), 'libgptq_b200.so')  # env override: A/B builds during development
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 c_void_p, c_int, c_int64, c_size_t, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t, ctypes.c_float
 
@@ -80,6 +80,8 @@ SIGNATURES = {
     'gptq_llama_decode_step': (c_int, [ctypes.POINTER(LlamaModel), ctypes.POINTER(LlamaState), c_void_p]),
     'gptq_llama_decode_launches': (c_int, [ctypes.POINTER(LlamaModel), ctypes.POINTER(LlamaState)]),
     'gptq_llama_persistent_scratch_offset': (c_size_t, [ctypes.POINTER(LlamaModel), c_int, c_int]),
+    'gptq_lm_head_logprob_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'gptq_lm_head_logprob': (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'gptq_ipc_alloc': (c_int, [c_size_t, ctypes.POINTER(c_void_p), ctypes.c_char_p]),
     'gptq_ipc_open': (c_int, [ctypes.c_char_p, ctypes.POINTER(c_void_p)]),
     'gptq_ipc_close': (c_int, [c_void_p]),

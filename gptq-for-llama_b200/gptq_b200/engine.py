@@ -73,6 +73,9 @@ def kernel_layers(layers, allow_perm=True):
     return out, perms
 
 
+SCORE_ROWS = 16384  # rows per scoring pass (LlamaDecoder.score): bounds the activations (at LLaMA-7B the fp16 MLP intermediate of a pass is 361 MB)
+
+
 class LlamaDecoder:
     """Owns the weights, the KV cache and the captured graph; `step()` decodes one token per sequence."""
 
@@ -244,42 +247,100 @@ class LlamaDecoder:
         assert self.batch == 1
         return self.prefill_batch([prompt_ids])[0]
 
-    @torch.no_grad()
-    def prefill_batch(self, prompts):
-        """Ragged pass over the first len(prompt) - 1 tokens of each of the `batch` prompts that fills sequence b's slot of the static KV cache:
-        the rows of every prompt are concatenated into one M-row pass (M = the sum of their lengths) through the quantized linears on the wgmma
-        GEMM path (gptq_qlinear_fwd / gptq_fused_mlp_fwd), the RMSNorm kernel and the RoPE kernel (per-token positions); the causal attention
-        runs per prompt in torch SDPA (as the reference's QuantLlamaAttention does, quant/fused_attn.py:154-155); keys are cached after RoPE.
-        The LAST token of each prompt then goes through the decode step like every generated one (it produces the first logits).  Returns the
-        number of cached positions per prompt (0 for a prompt of length 1)."""
-        assert self.tp is None
-        if len(prompts) != self.batch:
-            raise ValueError(f'expected {self.batch} prompts, got {len(prompts)}')
-        ns = [max(len(p) - 1, 0) for p in prompts]
-        if any(n > self.max_seq for n in ns):
-            raise ValueError(f'prompt does not fit the KV cache (max_seq = {self.max_seq})')
+    def _forward_rows(self, seqs, cache=False):
+        """The ragged pass shared by prefill and scoring: the token lists `seqs` are concatenated into one M-row pass (M = the sum of their
+        lengths) through the quantized linears on the wgmma GEMM path (gptq_qlinear_fwd / gptq_fused_mlp_fwd), the RMSNorm kernel and the RoPE
+        kernel (per-token positions, every list from position 0); the causal attention runs per list in torch SDPA (as the reference's
+        QuantLlamaAttention does, quant/fused_attn.py:154-155).  With `cache`, every layer's keys (after RoPE) and values of list b are written
+        to rows 0..len - 1 of sequence b's KV cache; without, nothing but the returned tensor is written.
+        Returns the residual stream after the last layer, fp16 [M, hidden] (final norm not applied)."""
+        ns = [len(s) for s in seqs]
         total = sum(ns)
-        if total == 0:
-            return ns
         H, nh, hd = self.hidden, self.n_heads, self.head_dim
-        ids = [int(t) for p, n in zip(prompts, ns) for t in p[:n]]
+        ids = [int(t) for s in seqs for t in s]
         x = self.embed[torch.tensor(ids, device=self.dev)]  # [total, H]
         pos = torch.cat([torch.arange(n, dtype=torch.int64) for n in ns]).to(self.dev)[None, :]
-        spans = [(b, sum(ns[:b]), n) for b, n in enumerate(ns) if n > 0]  # (sequence, first row, rows)
+        spans = [(b, sum(ns[:b]), n) for b, n in enumerate(ns) if n > 0]  # (list, first row, rows)
         for li, ly in enumerate(self.layers):
             qkv = ops.matmul248(ops.rmsnorm(x, ly['input_norm'], self.model.rms_eps), *ly['qkv'].parts(), ly['qkv'].bits, groupsize=ly['qkv'].hint).view(1, total, 3, nh, hd)
             ops.rotate_half_(qkv[:, :, :2], pos, base=self.model.rope_base)
             atts = []
             for b, r0, n in spans:
                 q, k, v = (qkv[0, r0:r0 + n, i].transpose(0, 1) for i in range(3))  # [nh, n, hd]
-                self.k_cache[li, b, :, :n] = k
-                self.v_cache[li, b, :, :n] = v
+                if cache:
+                    self.k_cache[li, b, :, :n] = k
+                    self.v_cache[li, b, :, :n] = v
                 atts.append(torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None], is_causal=True)[0].transpose(0, 1).reshape(n, H))
             att = atts[0] if len(atts) == 1 else torch.cat(atts)
             x = x + ops.matmul248(att, *ly['o'].parts(), ly['o'].bits, groupsize=ly['o'].hint)
             h = ops.fused_mlp(ops.rmsnorm(x, ly['post_norm'], self.model.rms_eps), ly['gate'].parts(), ly['up'].parts(), ly['gate'].bits, ly['gate'].hint)
             x = x + ops.matmul248(h, *ly['down'].parts(), ly['down'].bits, groupsize=ly['down'].hint)
+        return x
+
+    @torch.no_grad()
+    def prefill_batch(self, prompts):
+        """Ragged pass (_forward_rows) over the first len(prompt) - 1 tokens of each of the `batch` prompts that fills sequence b's slot of the
+        static KV cache.  The LAST token of each prompt then goes through the decode step like every generated one (it produces the first
+        logits).  Returns the number of cached positions per prompt (0 for a prompt of length 1)."""
+        assert self.tp is None
+        if len(prompts) != self.batch:
+            raise ValueError(f'expected {self.batch} prompts, got {len(prompts)}')
+        ns = [max(len(p) - 1, 0) for p in prompts]
+        if any(n > self.max_seq for n in ns):
+            raise ValueError(f'prompt does not fit the KV cache (max_seq = {self.max_seq})')
+        if sum(ns) == 0:
+            return ns
+        self._forward_rows([p[:n] for p, n in zip(prompts, ns)], cache=True)
         return ns
+
+    @torch.no_grad()
+    def score(self, sequences):
+        """Per-token log-likelihood: for each token list t of length n >= 2, the n - 1 fp32 values log p(t_i | t_<i), i = 1..n-1 (one tensor per
+        list).  Each list is scored from position 0 by the ragged pass (_forward_rows, no KV cache), the final RMSNorm and the fused
+        lm_head + log-softmax kernel (gptq_lm_head_logprob).  Lists are grouped into passes of at most SCORE_ROWS rows (a longer list is scored
+        alone), so activation memory stays bounded.  Independent of `batch` and `max_seq`; the KV cache, the decode buffers and the captured
+        graph are not touched."""
+        if self.tp is not None:
+            raise ValueError('score() is not supported under tensor parallelism')
+        seqs = [s.reshape(-1).tolist() if isinstance(s, torch.Tensor) else [int(t) for t in s] for s in sequences]
+        for s in seqs:
+            if len(s) < 2:
+                raise ValueError('every scored sequence needs at least 2 tokens')
+            if any(t < 0 or t >= self.vocab for t in s):
+                raise ValueError(f'token id outside the vocabulary (0..{self.vocab - 1})')
+        out = []
+        i = 0
+        while i < len(seqs):
+            j, rows = i + 1, len(seqs[i])
+            while j < len(seqs) and rows + len(seqs[j]) <= SCORE_ROWS:
+                rows += len(seqs[j])
+                j += 1
+            group = seqs[i:j]
+            x = self._forward_rows(group)
+            # row r of a list predicts its token r + 1: every row but the list's last
+            keep, r0 = [], 0
+            for s in group:
+                keep.append(torch.arange(r0, r0 + len(s) - 1))
+                r0 += len(s)
+            xn = ops.rmsnorm(x.index_select(0, torch.cat(keep).to(self.dev)), self.final_norm, self.model.rms_eps)
+            targets = torch.tensor([t for s in group for t in s[1:]], dtype=torch.int32, device=self.dev)
+            out.extend(ops.lm_head_logprob(xn, self.lm_head, targets).split([len(s) - 1 for s in group]))
+            i = j
+        return out
+
+    @torch.no_grad()
+    def perplexity(self, token_ids, seqlen=2048):
+        """Perplexity of a token stream as the reference's llama_eval computes it (llama.py:174-259): nsamples = len // seqlen chunks (the tail is
+        dropped), each scored from position 0, ppl = exp(sum of the chunks' NLL / (nsamples * (seqlen - 1))), the NLL summed in fp64."""
+        ids = token_ids.reshape(-1).tolist() if isinstance(token_ids, torch.Tensor) else [int(t) for t in token_ids]
+        if seqlen < 2:
+            raise ValueError('seqlen must be at least 2')
+        nsamples = len(ids) // seqlen
+        if nsamples == 0:
+            raise ValueError(f'{len(ids)} tokens do not fill one chunk of seqlen {seqlen}')
+        lps = self.score([ids[i * seqlen:(i + 1) * seqlen] for i in range(nsamples)])
+        nll = -float(torch.cat(lps).double().sum())
+        return math.exp(nll / (nsamples * (seqlen - 1)))
 
     def _check_prompts(self, prompts, max_new_tokens):
         if len(prompts) != self.batch:

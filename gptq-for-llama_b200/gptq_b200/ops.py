@@ -4,6 +4,7 @@ matmul248 / transpose_matmul248  <- quant/quant_linear.py:263-279
 fused_mlp                        <- QuantLlamaMLP.triton_llama_mlp, quant/fused_mlp.py:206-218
 rotate_half_                     <- triton_rotate_half_, quant/fused_attn.py:61-93
 rmsnorm                          <- TritonLlamaRMSNorm.forward, quant/triton_norm.py:50-67
+lm_head_logprob                  <- lm_head + shifted CrossEntropyLoss of llama_eval, llama.py:246-256 (per-token, fp32)
 
 torch is plumbing here (device memory, current stream); all arithmetic happens in libgptq_b200.so.
 """
@@ -169,6 +170,37 @@ def rmsnorm(x, weight, eps: float):
         y = torch.empty((M, N), device=x.device, dtype=torch.float16)
         check(lib.gptq_rmsnorm_fwd(x_arg.data_ptr(), x_arg.stride(0) if M > 1 else N, weight.data_ptr(), y.data_ptr(), N, M, N, float(eps), _stream(x)))
     return y.reshape(x.shape)
+
+
+def lm_head_logprob(x, weight, targets):
+    """fp32 [M]: log-softmax of the fp16 logits fp16(x . weight^T) at column targets[m], for x fp16 [M, K] and the lm_head weight fp16 [V, K]
+    (as nn.Linear stores it); the [M, V] logits are never materialised.  Targets are checked against [0, V) here (one device->host sync)."""
+    _require_cuda(x, weight, targets)
+    if x.dim() != 2 or weight.dim() != 2 or x.shape[1] != weight.shape[1]:
+        raise ValueError(f'expected x [M, K] and weight [V, K], got {tuple(x.shape)} and {tuple(weight.shape)}')
+    if x.dtype != torch.float16 or weight.dtype != torch.float16:
+        raise ValueError('lm_head_logprob expects float16 activations and weight')
+    M, K = x.shape
+    V = weight.shape[0]
+    targets = targets.reshape(-1)
+    if targets.numel() != M:
+        raise ValueError(f'expected {M} targets, got {targets.numel()}')
+    if M == 0:
+        return torch.empty(0, device=x.device, dtype=torch.float32)
+    if int(targets.min()) < 0 or int(targets.max()) >= V:
+        raise ValueError(f'target id outside the vocabulary (0..{V - 1})')
+    targets = targets.to(torch.int32).contiguous()
+    if x.stride(1) != 1:
+        x = x.contiguous()
+    if weight.stride(1) != 1:
+        weight = weight.contiguous()
+    with torch.cuda.device(x.device):
+        out = torch.empty(M, device=x.device, dtype=torch.float32)
+        ws, ws_bytes = _workspace(x.device, lib.gptq_lm_head_logprob_workspace_bytes(M, V))
+        check(
+            lib.gptq_lm_head_logprob(x.data_ptr(), x.stride(0) if M > 1 else K, weight.data_ptr(), weight.stride(0) if V > 1 else K, M, K, V,
+                                     targets.data_ptr(), out.data_ptr(), ws.data_ptr(), ws_bytes, _stream(x)))
+    return out
 
 
 def dequant(qweight, scales, qzeros, g_idx, bits, groupsize: int = 0):

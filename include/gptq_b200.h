@@ -37,8 +37,9 @@
 extern "C" {
 #endif
 
-#define GPTQ_B200_ABI_VERSION 5 /* 2: act-order input gathers; 3: gptq_llama_persistent_scratch_offset; 4: tensor parallelism (gptq_llama_tp, gptq_ipc_*);
-                                   5: persistent path at batch 2..8 ([batch][hidden] residual rows in the persistent region) */
+#define GPTQ_B200_ABI_VERSION 6 /* 2: act-order input gathers; 3: gptq_llama_persistent_scratch_offset; 4: tensor parallelism (gptq_llama_tp, gptq_ipc_*);
+                                   5: persistent path at batch 2..8 ([batch][hidden] residual rows in the persistent region);
+                                   6: gptq_lm_head_logprob (scoring) */
 
 typedef void* gptq_stream_t; /* cudaStream_t */
 
@@ -192,6 +193,19 @@ int gptq_llama_decode_launches(const gptq_llama_model* model, const gptq_llama_s
  * stream ping-pong: two fp16 [batch, hidden] arrays (row b = sequence b), each padded to 256 bytes (after a step: [0] = the
  * residual entering the last layer, [1] = the residual after the last layer's attention block). */
 size_t gptq_llama_persistent_scratch_offset(const gptq_llama_model* model, int batch, int max_seq);
+
+/* ------------------------------------------------------------------------------------------------
+ * Scoring (the perplexity evaluation of llama.py:246-259): per-row log-likelihood of a target token through the fp16 lm_head,
+ *   logprob[m] = l[m, t_m] - logsumexp_v l[m, v],   l = fp16(x[m] . w[v]) (fp32 accumulation, one fp16 rounding),
+ * with the log-softmax in fp32 on the fp16 logits and the [M, V] logits never written to memory.
+ * x fp16 [M, K] (ldx elements between rows), w fp16 [V, K] as nn.Linear stores the lm_head (ldw), targets int32 [M] in [0, V)
+ * (the caller validates them; a row whose target is outside that range gets NaN), logprob fp32 [M] out.
+ * K must be a positive multiple of 64; x and w 16-byte aligned, ldx and ldw multiples of 8.  The workspace (256-byte aligned,
+ * gptq_lm_head_logprob_workspace_bytes) follows the workspace rule above.  A row's result is bit-for-bit the same whatever M
+ * is and whatever the other rows hold. */
+size_t gptq_lm_head_logprob_workspace_bytes(int M, int V);
+int gptq_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int K, int V, const int32_t* targets, float* logprob,
+                         void* workspace, size_t ws_bytes, gptq_stream_t stream);
 
 /* Device memory that other processes of the node can map (CUDA IPC), for the tensor-parallel scratch / logits buffers:
  * alloc returns a zero-filled device buffer and its 64-byte handle (to be sent to the peers, e.g. with torch.distributed);
