@@ -162,6 +162,28 @@ int gptq_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw,
     return cuda_status(launch_lm_head_logprob(x, ldx, w, ldw, M, K, V, targets, logprob, workspace, static_cast<cudaStream_t>(stream)));
 }
 
+int gptq_cached_attention(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int head_dim, int max_seq,
+                          int n_spans, const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
+                          gptq_stream_t stream) {
+    if (q == nullptr || k_cache == nullptr || v_cache == nullptr || out == nullptr) return GPTQ_ERR_NULL;
+    if (n_spans > 0 && (span_seq == nullptr || span_start == nullptr || span_rows == nullptr)) return GPTQ_ERR_NULL;
+    if (batch <= 0 || n_heads <= 0 || head_dim <= 0 || max_seq <= 0) return GPTQ_ERR_SHAPE;
+    if (head_dim != 128) return GPTQ_ERR_UNSUPPORTED;  // the head size of both decode engines
+    if (n_spans < 0 || n_spans > kCachedAttnMaxSpans) return GPTQ_ERR_SHAPE;
+    if ((int64_t)batch * n_heads * max_seq > 0x7fffffffLL) return GPTQ_ERR_SHAPE;  // TMA row coordinates are 32-bit
+    const int64_t width = (int64_t)n_heads * head_dim;
+    if (ldq < width || ldo < width || ldq % 8 != 0 || ldo % 8 != 0) return GPTQ_ERR_SHAPE;  // TMA: 16-byte row pitch
+    for (int i = 0; i < n_spans; ++i) {
+        if (span_seq[i] < 0 || span_seq[i] >= batch || span_start[i] < 0 || span_rows[i] < 0) return GPTQ_ERR_SHAPE;
+        if ((int64_t)span_start[i] + span_rows[i] > max_seq) return GPTQ_ERR_SHAPE;
+        for (int j = 0; j < i; ++j)
+            if (span_seq[j] == span_seq[i]) return GPTQ_ERR_SHAPE;
+    }
+    if (!aligned(q, 16) || !aligned(k_cache, 16) || !aligned(v_cache, 16) || !aligned(out, 16)) return GPTQ_ERR_ALIGN;
+    return cuda_status(launch_cached_attention(q, ldq, k_cache, v_cache, batch, n_heads, max_seq, n_spans, span_seq, span_start, span_rows, out, ldo,
+                                               static_cast<cudaStream_t>(stream)));
+}
+
 int gptq_ipc_alloc(size_t bytes, void** ptr, unsigned char handle[64]) {
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "handle size");
     if (ptr == nullptr || handle == nullptr || bytes == 0) return GPTQ_ERR_NULL;

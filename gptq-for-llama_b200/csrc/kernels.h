@@ -56,6 +56,12 @@ size_t lm_head_logprob_workspace_bytes(int M, int V);
 cudaError_t launch_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int K, int V, const int32_t* targets, float* logprob,
                                    void* workspace, cudaStream_t stream);
 
+// cached_attention.cu -- causal attention of new rows over a sequence's cached prefix (wgmma, read in place from the KV cache), head_dim 128
+constexpr int kCachedAttnMaxSpans = 64;
+cudaError_t launch_cached_attention(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int max_seq, int n_spans,
+                                    const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
+                                    cudaStream_t stream);
+
 // decode_mega.cu -- persistent single-kernel decode step (batch 1 to 8, int4 kernel-form layers)
 bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st);
 size_t mega_scratch_bytes(const gptq_llama_model& m, int batch);

@@ -44,12 +44,6 @@ struct LogprobParams {
     int M, K, V, ntiles, mtiles;
 };
 
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, int k, int row, uint32_t bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst), "l"(tm), "r"(k),
-                 "r"(row), "r"(bar)
-                 : "memory");
-}
-
 __global__ void __launch_bounds__(kThreads, 1) lm_head_logprob_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
                                                                       const LogprobParams p) {
     extern __shared__ __align__(16) uint8_t smem_raw[];

@@ -1,5 +1,6 @@
-// Hopper tensor-core helpers shared by the wgmma kernels (qgemm_wgmma.cu, lm_head_logprob.cu): shared-memory matrix
-// descriptors, the wgmma fence / commit / wait protocol, the m64n128k16 f16 MMA, and the TMA tensor map of a K-major fp16 matrix.
+// Hopper tensor-core helpers shared by the wgmma kernels (qgemm_wgmma.cu, lm_head_logprob.cu, cached_attention.cu): shared-memory matrix
+// descriptors, the wgmma fence / commit / wait protocol, the m64n128k16 f16 MMAs (both operands in shared memory; A in registers with a
+// transposed B), and the TMA tensor map of a K-major fp16 matrix with its box load.
 #pragma once
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -47,6 +48,41 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, ui
           "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
           "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(da), "l"(db), "r"(1));
+}
+
+// wgmma shared-memory matrix descriptor of an MN-major B operand (N contiguous), SWIZZLE_128B: atoms of 8 K-rows x 64 N-halves (1024 B);
+// `lbo` bytes between atoms adjacent in N, SBO = 1024 B between atoms adjacent in K (8-row groups).  Used with the transpose-B immediate.
+__device__ __forceinline__ uint64_t smem_desc_mn(uint32_t saddr, uint32_t lbo) {
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+
+// D[64 x 128] += A[64 x 16] . B[16 x 128], A from registers (four f16x2 per thread, the layout of an m64nNk16 accumulator fragment:
+// a[0] = row r cols c, c+1; a[1] = row r+8; a[2] = cols c+8, c+9; a[3] = row r+8, cols c+8, c+9), B MN-major in shared memory (transposed)
+__device__ __forceinline__ void wgmma_m64n128k16_rs_tn(float (&d)[64], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %69, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, "
+        "%30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, "
+        "%58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+          "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+          "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
+}
+
+// one TMA box (box 64 (k) x 128 rows of a make_kmajor_tensor_map map) global -> shared at (k, row); completion on the mbarrier `bar`
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, int k, int row, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst), "l"(tm), "r"(k),
+                 "r"(row), "r"(bar)
+                 : "memory");
 }
 
 // TMA tensor map of an fp16 [rows, K] matrix with `ld` elements between rows (K-major, like the wgmma operands): box 64 (k) x 128 rows,

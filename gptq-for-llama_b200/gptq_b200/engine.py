@@ -136,6 +136,10 @@ class LlamaDecoder:
                     self._fill_layer_structs()
                     if all(p is None for pm in self.perms for p in pm.values()) or self.launches_per_step() == 1:
                         break
+        # host-side record of the KV cache: lengths[b] positions of sequence b are cached, cached_tokens[b] are the token ids of its first
+        # positions as far as they are known (reset, prefill_batch, set_input and extend keep both; raw writes to self.positions do not)
+        self.lengths = [0] * batch
+        self.cached_tokens = [[] for _ in range(batch)]
         self.n_launches = None
         self.graph = None
         self._stream = torch.cuda.Stream(self.dev)
@@ -223,11 +227,21 @@ class LlamaDecoder:
 
     def reset(self):
         self.positions.zero_()
+        self.lengths = [0] * self.batch
+        self.cached_tokens = [[] for _ in range(self.batch)]
+
+    def _record(self, b, pos, toks):
+        """Sequence b's cache rows pos .. pos + len(toks) - 1 now hold `toks` and nothing past them is cached.  The known token prefix grows only
+        when it reaches pos (otherwise the rows in between are of unknown origin and the prefix stays as it was)."""
+        self.lengths[b] = pos + len(toks)
+        known = self.cached_tokens[b]
+        self.cached_tokens[b] = known[:pos] + list(toks) if len(known) >= pos else known
 
     def set_input(self, tokens, positions):
         """Token ids (int or sequence of `batch` ints) and the cache position of this step (int: every sequence, or sequence of `batch` ints: one
         per sequence); validated on the host: the kernels only clamp (a position beyond the cache or a token outside the vocabulary must never
-        reach them)."""
+        reach them).  The step that follows caches row p of each sequence, so `lengths` becomes p + 1 (writing self.positions directly bypasses
+        this record, and generate(..., reuse_cache=True) then reuses less or nothing)."""
         toks = [int(tokens)] * self.batch if isinstance(tokens, int) else [int(t) for t in tokens]
         if len(toks) != self.batch:
             raise ValueError(f'expected {self.batch} token ids, got {len(toks)}')
@@ -240,6 +254,8 @@ class LlamaDecoder:
             raise ValueError(f'token id outside the vocabulary (0..{self.vocab - 1})')
         self.tokens.copy_(torch.tensor(toks, dtype=torch.int32))
         self.positions.copy_(torch.tensor(pos, dtype=torch.int32))
+        for b, (t, p) in enumerate(zip(toks, pos)):
+            self._record(b, p, [t])
 
     @torch.no_grad()
     def prefill(self, prompt_ids):
@@ -247,31 +263,46 @@ class LlamaDecoder:
         assert self.batch == 1
         return self.prefill_batch([prompt_ids])[0]
 
-    def _forward_rows(self, seqs, cache=False):
-        """The ragged pass shared by prefill and scoring: the token lists `seqs` are concatenated into one M-row pass (M = the sum of their
-        lengths) through the quantized linears on the wgmma GEMM path (gptq_qlinear_fwd / gptq_fused_mlp_fwd), the RMSNorm kernel and the RoPE
-        kernel (per-token positions, every list from position 0); the causal attention runs per list in torch SDPA (as the reference's
-        QuantLlamaAttention does, quant/fused_attn.py:154-155).  With `cache`, every layer's keys (after RoPE) and values of list b are written
-        to rows 0..len - 1 of sequence b's KV cache; without, nothing but the returned tensor is written.
+    def _forward_rows(self, seqs, cache=False, starts=None):
+        """The ragged pass shared by prefill, scoring and extend: the token lists `seqs` are concatenated into one M-row pass (M = the sum of
+        their lengths) through the quantized linears on the wgmma GEMM path (gptq_qlinear_fwd / gptq_fused_mlp_fwd), the RMSNorm kernel and the
+        RoPE kernel (per-token positions).
+        starts=None: every list from position 0; the causal attention runs per list in torch SDPA (as the reference's QuantLlamaAttention does,
+        quant/fused_attn.py:154-155).  With `cache`, every layer's keys (after RoPE) and values of list b are written to rows 0..len - 1 of
+        sequence b's KV cache; without, nothing but the returned tensor is written.
+        starts[b] = p: list b continues sequence b from position p (its cache holds positions 0..p - 1; requires `cache`): its keys and values
+        are written to rows p..p + len - 1, and the attention of all lists runs in one gptq_cached_attention call per layer, over each
+        sequence's cached prefix and its new rows, read in place from the cache.
         Returns the residual stream after the last layer, fp16 [M, hidden] (final norm not applied)."""
         ns = [len(s) for s in seqs]
         total = sum(ns)
         H, nh, hd = self.hidden, self.n_heads, self.head_dim
         ids = [int(t) for s in seqs for t in s]
         x = self.embed[torch.tensor(ids, device=self.dev)]  # [total, H]
-        pos = torch.cat([torch.arange(n, dtype=torch.int64) for n in ns]).to(self.dev)[None, :]
+        if starts is None:
+            pos = torch.cat([torch.arange(n, dtype=torch.int64) for n in ns]).to(self.dev)[None, :]
+        else:
+            assert cache
+            pos = torch.cat([torch.arange(p, p + n, dtype=torch.int64) for p, n in zip(starts, ns)]).to(self.dev)[None, :]
         spans = [(b, sum(ns[:b]), n) for b, n in enumerate(ns) if n > 0]  # (list, first row, rows)
         for li, ly in enumerate(self.layers):
             qkv = ops.matmul248(ops.rmsnorm(x, ly['input_norm'], self.model.rms_eps), *ly['qkv'].parts(), ly['qkv'].bits, groupsize=ly['qkv'].hint).view(1, total, 3, nh, hd)
             ops.rotate_half_(qkv[:, :, :2], pos, base=self.model.rope_base)
-            atts = []
-            for b, r0, n in spans:
-                q, k, v = (qkv[0, r0:r0 + n, i].transpose(0, 1) for i in range(3))  # [nh, n, hd]
-                if cache:
-                    self.k_cache[li, b, :, :n] = k
-                    self.v_cache[li, b, :, :n] = v
-                atts.append(torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None], is_causal=True)[0].transpose(0, 1).reshape(n, H))
-            att = atts[0] if len(atts) == 1 else torch.cat(atts)
+            if starts is None:
+                atts = []
+                for b, r0, n in spans:
+                    q, k, v = (qkv[0, r0:r0 + n, i].transpose(0, 1) for i in range(3))  # [nh, n, hd]
+                    if cache:
+                        self.k_cache[li, b, :, :n] = k
+                        self.v_cache[li, b, :, :n] = v
+                    atts.append(torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None], is_causal=True)[0].transpose(0, 1).reshape(n, H))
+                att = atts[0] if len(atts) == 1 else torch.cat(atts)
+            else:
+                for b, r0, n in spans:
+                    p = starts[b]
+                    self.k_cache[li, b, :, p:p + n] = qkv[0, r0:r0 + n, 1].transpose(0, 1)
+                    self.v_cache[li, b, :, p:p + n] = qkv[0, r0:r0 + n, 2].transpose(0, 1)
+                att = ops.cached_attention(qkv.view(total, 3 * H)[:, :H], self.k_cache[li], self.v_cache[li], [(b, starts[b], n) for b, _, n in spans])
             x = x + ops.matmul248(att, *ly['o'].parts(), ly['o'].bits, groupsize=ly['o'].hint)
             h = ops.fused_mlp(ops.rmsnorm(x, ly['post_norm'], self.model.rms_eps), ly['gate'].parts(), ly['up'].parts(), ly['gate'].bits, ly['gate'].hint)
             x = x + ops.matmul248(h, *ly['down'].parts(), ly['down'].bits, groupsize=ly['down'].hint)
@@ -288,10 +319,36 @@ class LlamaDecoder:
         ns = [max(len(p) - 1, 0) for p in prompts]
         if any(n > self.max_seq for n in ns):
             raise ValueError(f'prompt does not fit the KV cache (max_seq = {self.max_seq})')
-        if sum(ns) == 0:
-            return ns
-        self._forward_rows([p[:n] for p, n in zip(prompts, ns)], cache=True)
+        if sum(ns) > 0:
+            self._forward_rows([p[:n] for p, n in zip(prompts, ns)], cache=True)
+        for b, (p, n) in enumerate(zip(prompts, ns)):
+            self.cached_tokens[b] = []
+            self._record(b, 0, [int(t) for t in p[:n]])
         return ns
+
+    @torch.no_grad()
+    def extend(self, chunks):
+        """Append chunks[b] (a list of token ids, possibly empty) to sequence b, after the lengths[b] positions its KV cache already holds, in one
+        ragged pass (_forward_rows with starts = lengths): the new rows attend to the cached prefix and to each other through
+        gptq_cached_attention, and their keys and values are written to cache rows lengths[b] .. lengths[b] + len - 1.  An empty chunk leaves its
+        sequence untouched.  The decode buffers and the captured graph are not touched; the next step(s) continue at the new lengths.
+        Everything is validated before anything is written.  Returns the new lengths."""
+        if self.tp is not None:
+            raise ValueError('extend() is not supported under tensor parallelism')
+        if len(chunks) != self.batch:
+            raise ValueError(f'expected {self.batch} chunks, got {len(chunks)}')
+        seqs = [c.reshape(-1).tolist() if isinstance(c, torch.Tensor) else [int(t) for t in c] for c in chunks]
+        for b, s in enumerate(seqs):
+            if any(t < 0 or t >= self.vocab for t in s):
+                raise ValueError(f'token id outside the vocabulary (0..{self.vocab - 1})')
+            if self.lengths[b] + len(s) > self.max_seq:
+                raise ValueError(f'sequence {b}: {self.lengths[b]} cached + {len(s)} new positions do not fit the KV cache (max_seq = {self.max_seq})')
+        if any(seqs):
+            self._forward_rows(seqs, cache=True, starts=list(self.lengths))
+        for b, s in enumerate(seqs):
+            if s:
+                self._record(b, self.lengths[b], s)
+        return list(self.lengths)
 
     @torch.no_grad()
     def score(self, sequences):
@@ -367,25 +424,59 @@ class LlamaDecoder:
                     out[b].append(nxt[b])
         return out
 
+    def _reuse(self, prompts, extend=True):
+        """Keep what each sequence's cache shares with its prompt (reusable_prefix) and drop the rest of the record; with `extend`, append the
+        uncached prompt tokens but the last in one extend() pass.  Returns the positions the decode steps start from."""
+        if self.tp is not None:
+            raise ValueError('reuse_cache is not supported under tensor parallelism')
+        prompts = [[int(t) for t in p] for p in prompts]
+        keep = [reusable_prefix(p, self.cached_tokens[b][:self.lengths[b]]) for b, p in enumerate(prompts)]
+        for b, c in enumerate(keep):
+            self.lengths[b] = c
+            self.cached_tokens[b] = self.cached_tokens[b][:c]
+        if not extend:
+            return keep
+        self.extend([p[c:len(p) - 1] for p, c in zip(prompts, keep)])
+        return [len(p) - 1 for p in prompts]
+
     @torch.no_grad()
-    def generate(self, prompt_ids, max_new_tokens, prefill=True):
+    def generate(self, prompt_ids, max_new_tokens, prefill=True, reuse_cache=False):
         """Greedy decode (batch 1).  One engine, two phases: the prompt is prefilled in one batched pass (wgmma GEMM path) into the static KV
-        cache, then the persistent decode kernel takes over token by token; prefill=False feeds the prompt through the decode step instead."""
+        cache, then the persistent decode kernel takes over token by token; prefill=False feeds the prompt through the decode step instead.
+        reuse_cache=True keeps the cached positions the prompt starts with (e.g. the conversation so far, when the prompt is that conversation
+        plus a new turn) and computes only the rest (with extend(), or through the decode step with prefill=False)."""
         assert self.batch == 1
         self._check_prompts([prompt_ids], max_new_tokens)
+        if reuse_cache:
+            return self._decode([prompt_ids], max_new_tokens, self._reuse([prompt_ids], extend=prefill))[0]
         self.reset()
         start = self.prefill(prompt_ids) if (prefill and self.tp is None) else 0
         return self._decode([prompt_ids], max_new_tokens, [start])[0]
 
     @torch.no_grad()
-    def generate_batch(self, prompts, max_new_tokens):
+    def generate_batch(self, prompts, max_new_tokens, reuse_cache=False):
         """Greedy decode of `batch` prompts of different lengths: one ragged prefill (prefill_batch), then every sequence is stepped in
         lock-step at its own position by the decode step (the persistent kernel decodes them all in one launch).  Returns one token list per
-        prompt: the prompt followed by its max_new_tokens generated tokens."""
+        prompt: the prompt followed by its max_new_tokens generated tokens.
+        reuse_cache=True: sequence b keeps the longest prefix its cache shares with prompt b (at most len(prompt) - 1 positions) and only the
+        rest of the prompt but its last token goes through one ragged extend() pass, so a second turn -- the previous output plus the new
+        turn -- costs the new turn only.  The result is that of reuse_cache=False up to fp rounding."""
         self._check_prompts(prompts, max_new_tokens)
+        if reuse_cache:
+            return self._decode(prompts, max_new_tokens, self._reuse(prompts))
         self.reset()
         starts = self.prefill_batch(prompts)
         return self._decode(prompts, max_new_tokens, starts)
+
+
+def reusable_prefix(prompt, cached):
+    """How many leading positions of a cache holding the token ids `cached` a new `prompt` can keep: the length of their common prefix, at most
+    len(prompt) - 1, because the prompt's last token must still go through the decode step (it produces the first logits)."""
+    n = min(len(prompt) - 1, len(cached))
+    c = 0
+    while c < n and int(prompt[c]) == int(cached[c]):
+        c += 1
+    return c
 
 
 def synthetic_llama(size='7b', bits=4, groupsize=128, act_order=False, vocab=32000, device='cuda:0', seed=0, n_layers=None, **kw):

@@ -5,6 +5,7 @@ fused_mlp                        <- QuantLlamaMLP.triton_llama_mlp, quant/fused_
 rotate_half_                     <- triton_rotate_half_, quant/fused_attn.py:61-93
 rmsnorm                          <- TritonLlamaRMSNorm.forward, quant/triton_norm.py:50-67
 lm_head_logprob                  <- lm_head + shifted CrossEntropyLoss of llama_eval, llama.py:246-256 (per-token, fp32)
+cached_attention                 <- causal SDPA of new rows over a sequence's cached prefix (the engine's extend path; no reference counterpart)
 
 torch is plumbing here (device memory, current stream); all arithmetic happens in libgptq_b200.so.
 """
@@ -200,6 +201,37 @@ def lm_head_logprob(x, weight, targets):
         check(
             lib.gptq_lm_head_logprob(x.data_ptr(), x.stride(0) if M > 1 else K, weight.data_ptr(), weight.stride(0) if V > 1 else K, M, K, V,
                                      targets.data_ptr(), out.data_ptr(), ws.data_ptr(), ws_bytes, _stream(x)))
+    return out
+
+
+def cached_attention(q, k_cache, v_cache, spans):
+    """fp16 [M, n_heads * head_dim]: causal attention of new query rows over their sequences' cached prefixes, read in place from one layer's
+    slice of the KV cache (k_cache / v_cache fp16 [batch, n_heads, max_seq, head_dim], keys after RoPE; see gptq_cached_attention).
+    `spans` lists (seq, start, rows): the next `rows` rows of q (fp16 [M, >= n_heads * head_dim], rows may be strided, e.g. the q part of the
+    fused qkv output) are sequence seq's positions start .. start + rows - 1, whose K and V rows the caller has already written."""
+    _require_cuda(q, k_cache, v_cache)
+    if q.dim() != 2 or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
+        raise ValueError(f'expected q [M, heads * head_dim] and caches [batch, heads, max_seq, head_dim], got {tuple(q.shape)}, {tuple(k_cache.shape)}, '
+                         f'{tuple(v_cache.shape)}')
+    if q.dtype != torch.float16 or k_cache.dtype != torch.float16 or v_cache.dtype != torch.float16:
+        raise ValueError('cached_attention expects float16 q and caches')
+    if not (k_cache.is_contiguous() and v_cache.is_contiguous()):
+        raise ValueError('the KV cache slices must be contiguous')
+    B, nh, S, hd = k_cache.shape
+    spans = [(int(b), int(s), int(n)) for b, s, n in spans]
+    M = sum(n for _, _, n in spans)
+    if q.shape[0] != M or q.shape[1] != nh * hd:
+        raise ValueError(f'q has shape {tuple(q.shape)}, the spans need [{M}, {nh * hd}]')
+    out = torch.empty((M, nh * hd), device=q.device, dtype=torch.float16)
+    if M == 0:
+        return out
+    if q.stride(1) != 1:
+        q = q.contiguous()
+    arr = lambda i: (ctypes.c_int32 * len(spans))(*[sp[i] for sp in spans])
+    with torch.cuda.device(q.device):
+        check(
+            lib.gptq_cached_attention(q.data_ptr(), q.stride(0) if M > 1 else nh * hd, k_cache.data_ptr(), v_cache.data_ptr(), B, nh, hd, S, len(spans), arr(0),
+                                      arr(1), arr(2), out.data_ptr(), nh * hd, _stream(q)))
     return out
 
 

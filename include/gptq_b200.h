@@ -39,7 +39,8 @@ extern "C" {
 
 #define GPTQ_B200_ABI_VERSION 6 /* 2: act-order input gathers; 3: gptq_llama_persistent_scratch_offset; 4: tensor parallelism (gptq_llama_tp, gptq_ipc_*);
                                    5: persistent path at batch 2..8 ([batch][hidden] residual rows in the persistent region);
-                                   6: gptq_lm_head_logprob (scoring) */
+                                   6: gptq_lm_head_logprob (scoring); gptq_cached_attention added later without a change to any
+                                   existing struct or signature */
 
 typedef void* gptq_stream_t; /* cudaStream_t */
 
@@ -206,6 +207,22 @@ size_t gptq_llama_persistent_scratch_offset(const gptq_llama_model* model, int b
 size_t gptq_lm_head_logprob_workspace_bytes(int M, int V);
 int gptq_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int K, int V, const int32_t* targets, float* logprob,
                          void* workspace, size_t ws_bytes, gptq_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Extending cached sequences (LlamaDecoder.extend, generate(..., reuse_cache=True)).
+ * Causal attention of new rows over a sequence's cached prefix, read in place from the decode engine's KV cache (one layer's slice:
+ * fp16 [batch, n_heads, max_seq, head_dim], keys after RoPE).  Span i = (seq[i], start[i], rows[i]): its query rows are the next rows[i]
+ * rows of q (spans in order, no gaps), at positions start[i] .. start[i] + rows[i] - 1; row j attends to keys 0 .. start[i] + j of
+ * sequence seq[i], whose rows start[i] .. start[i] + rows[i] - 1 the caller has already written.  Cache rows at or past
+ * start[i] + rows[i] are never read into the result (they may hold anything).  span_* are HOST arrays; sequences are distinct.
+ * q / out: fp16 rows of n_heads * head_dim (ldq / ldo elements apart; q may be the q part of the fused qkv output).
+ * head_dim must be 128 (GPTQ_ERR_UNSUPPORTED otherwise); 0 <= n_spans <= 64; ldq, ldo multiples of 8 (GPTQ_ERR_SHAPE otherwise); q, the
+ * caches and out 16-byte aligned.  Zero rows in total launch nothing.  Arithmetic: fp32 scores and online softmax, P rounded to fp16 for
+ * the P.V product, fp32 accumulation, one fp16 rounding of the output.  A span's result is bit-for-bit the same whatever the other spans
+ * of the call are and in whatever order they come. */
+int gptq_cached_attention(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int head_dim, int max_seq,
+                          int n_spans, const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
+                          gptq_stream_t stream);
 
 /* Device memory that other processes of the node can map (CUDA IPC), for the tensor-parallel scratch / logits buffers:
  * alloc returns a zero-filled device buffer and its 64-byte handle (to be sent to the peers, e.g. with torch.distributed);
