@@ -481,20 +481,22 @@ def reusable_prefix(prompt, cached):
 
 def synthetic_llama(size='7b', bits=4, groupsize=128, act_order=False, vocab=32000, device='cuda:0', seed=0, n_layers=None, **kw):
     """Random-init GPTQ LLaMA of the named size (no checkpoints are reachable offline): every layer has its
-    own distinct packed tensors so that a decode step streams the full model from HBM."""
+    own distinct packed tensors so that a decode step streams the full model from HBM.  groupsize -1: one group per linear (the
+    reference's --groupsize -1, where QuantLinear takes groupsize = infeatures): hidden for qkv / o / gate / up, intermediate for down."""
     hidden, inter, layers, heads = LLAMA_SHAPES[size]
     layers = n_layers or layers
+    gs_h, gs_i = (hidden, inter) if groupsize == -1 else (groupsize, groupsize)
     dev = torch.device(device)
     gen = torch.Generator(device=dev).manual_seed(seed)
     L = []
     for _ in range(layers):
-        gate = random_qlayer(hidden, inter, bits, groupsize, dev, gen, act_order)
-        up = random_qlayer(hidden, inter, bits, groupsize, dev, gen, act_order)
+        gate = random_qlayer(hidden, inter, bits, gs_h, dev, gen, act_order)
+        up = random_qlayer(hidden, inter, bits, gs_h, dev, gen, act_order)
         if act_order:  # gate and up see the same input, hence the same Hessian diagonal and the same act-order map (gptq.py:210-216)
-            up = QLayerWeights(up.qweight, up.scales, up.qzeros, gate.g_idx.clone(), bits, groupsize)
+            up = QLayerWeights(up.qweight, up.scales, up.qzeros, gate.g_idx.clone(), bits, gs_h)
         L.append(
-            dict(qkv=random_qlayer(hidden, 3 * hidden, bits, groupsize, dev, gen, act_order), o=random_qlayer(hidden, hidden, bits, groupsize, dev, gen, act_order),
-                 gate=gate, up=up, down=random_qlayer(inter, hidden, bits, groupsize, dev, gen, act_order),
+            dict(qkv=random_qlayer(hidden, 3 * hidden, bits, gs_h, dev, gen, act_order), o=random_qlayer(hidden, hidden, bits, gs_h, dev, gen, act_order),
+                 gate=gate, up=up, down=random_qlayer(inter, hidden, bits, gs_i, dev, gen, act_order),
                  input_norm=(torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half(),
                  post_norm=(torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half()))
     # q/k/v share their input, hence their act-order map (quant/fused_attn.py:180): nothing to do, qkv is one layer here
@@ -529,8 +531,9 @@ def shard_for_rank(layers, lm_head, n_heads, head_dim, rank, size):
 
 def synthetic_llama_tp(size_name, rank, world, bits=4, groupsize=128, vocab=32000, device='cuda:0', seed=0, n_layers=None, full=None, reduce_mode=0, **kw):
     """One tensor-parallel rank of the random-init model `synthetic_llama(size_name, seed=seed)` (every rank generates the same full model from the same
-    seed layer by layer and keeps its shard), or of the given `full` decoder's weights."""
+    seed layer by layer and keeps its shard), or of the given `full` decoder's weights.  groupsize -1 as in synthetic_llama."""
     hidden, inter, layers, heads = LLAMA_SHAPES[size_name]
+    gs_h, gs_i = (hidden, inter) if groupsize == -1 else (groupsize, groupsize)
     layers = n_layers or layers
     dev = torch.device(device)
     hd = hidden // heads
@@ -541,10 +544,10 @@ def synthetic_llama_tp(size_name, rank, world, bits=4, groupsize=128, vocab=3200
     L = []
     fake_head = torch.empty(0, hidden, device=dev)
     for _ in range(layers):  # shard as we go: a 65B model never exists whole on one GPU
-        gate = random_qlayer(hidden, inter, bits, groupsize, dev, gen)
-        up = random_qlayer(hidden, inter, bits, groupsize, dev, gen)
-        ly = dict(qkv=random_qlayer(hidden, 3 * hidden, bits, groupsize, dev, gen), o=random_qlayer(hidden, hidden, bits, groupsize, dev, gen), gate=gate, up=up,
-                  down=random_qlayer(inter, hidden, bits, groupsize, dev, gen), input_norm=(torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half(),
+        gate = random_qlayer(hidden, inter, bits, gs_h, dev, gen)
+        up = random_qlayer(hidden, inter, bits, gs_h, dev, gen)
+        ly = dict(qkv=random_qlayer(hidden, 3 * hidden, bits, gs_h, dev, gen), o=random_qlayer(hidden, hidden, bits, gs_h, dev, gen), gate=gate, up=up,
+                  down=random_qlayer(inter, hidden, bits, gs_i, dev, gen), input_norm=(torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half(),
                   post_norm=(torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half())
         L.append(shard_for_rank([ly], fake_head, heads, hd, rank, world)[0][0])
         del ly, gate, up

@@ -72,6 +72,34 @@ def test_decode_steps_match_oracle(size, bits, act, use_graph):
         assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
 
 
+@pytest.mark.parametrize('gs', [-1, 32])
+def test_hf_checkpoint_groupsizes_decode_on_the_persistent_kernel(gs):
+    """The route a real checkpoint takes (the reference's load_quant recipe on the quant modules -> engine.from_hf_quant_model) at
+    --groupsize -1 (QuantLinear takes groupsize = infeatures: 256 for qkv / o / gate / up, 768 for down) and 32: the persistent kernel
+    serves it with every groupsize hint intact, and six decode steps match the oracle at the bound of test_decode_steps_match_oracle."""
+    import quant
+    from gptq_b200 import engine
+    from test_gpu_modules import _tiny_quant_llama
+    model = _tiny_quant_llama(gs=gs, hidden=256, intermediate=768, heads=2)
+    quant.make_quant_attn(model)
+    quant.make_quant_norm(model)
+    quant.make_fused_mlp(model)
+    dec = engine.from_hf_quant_model(model.cuda(), max_seq=16)
+    assert dec.launches_per_step() == 1
+    for kl in dec.klayers:
+        for name in ('qkv', 'o', 'gate', 'up', 'down'):
+            K = kl[name].g_idx.numel()
+            assert kl[name].hint == (K if gs == -1 else gs), f'{name}: groupsize hint {kl[name].hint}'
+    toks = torch.randint(0, dec.vocab, (6, ), generator=torch.Generator().manual_seed(gs + 2)).tolist()
+    ref = _oracle_decode(dec, toks)
+    for pos, tok in enumerate(toks):
+        dec.set_input(tok, pos)
+        dec.step()
+        torch.cuda.synchronize()
+        assert_rel_close(dec.logits[0], ref[pos], rel=2e-2, what=f'gs={gs} pos={pos}')
+        assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
+
+
 @pytest.mark.parametrize('size', ['tiny', 'tiny256'])
 def test_long_context_attention_splits(size):
     """Positions beyond one attention chunk: split-KV partials + combine against the oracle (both engines)."""

@@ -3,7 +3,8 @@
 The small-model tests (test_gpu_engine.py) cannot reach the stream-K ranges, attention unit splits, ring wrap-arounds and
 staging sizes of the 7B / 13B configurations, so here the kernel runs LLaMA-7B-shaped (int4 g128, BASELINE config 2) and
 LLaMA-13B-shaped (int3 g128 act-order, config 4) layers -- two of them, which exercises every inter-layer hand-off -- on a
-randomly filled KV cache at the context positions {0, 255, 256, 2046, 2047}, against the oracle (oracle/gptq_oracle.py).
+randomly filled KV cache at the context positions {0, 255, 256, 2046, 2047}, against the oracle (oracle/gptq_oracle.py); and 7B at
+the groupsizes 32, 1024 and -1 (one group per linear) at the positions {0, 2047}.
 
 Checked per BLOCK, each block's oracle fed with the kernel's own input to that block (read back from its scratch), so that a
 1e-3-class bound stays meaningful: a decoder is a chain of fp16 rounding points, and a one-ulp difference early on (any other
@@ -46,7 +47,8 @@ class Exact:
     persistent kernel computes (it applies scale and zero per group on the fp32 accumulator).  The attention block is checked against it
     because a softmax over 2048 keys amplifies one-ulp changes in q: at context 2047 of the 7B case the reference's per-weight fp16
     rounding of the qkv weights alone moves the block by twice ATTN_BLOCK_TOL.  Each QuantLinear is held to the reference's rounding
-    within 1e-3 by tests/test_gpu_parity.py and tests/test_gpu_modules.py, and the appended K / V rows below are held to it here."""
+    within 1e-3 by tests/test_gpu_parity.py and tests/test_gpu_modules.py, and the appended K / V rows below are held to it here (the K
+    rows of the groupsize -1 case excepted, see _run_case) as well as to Exact."""
 
     @staticmethod
     def qlinear_fwd(x, qweight, scales, qzeros, g_idx, bits):
@@ -107,8 +109,10 @@ def _resid_buffers(dec):
     return [r[0].cpu() for r in resid_buffers(dec)]
 
 
-def _check_last_layer_blocks(dec, layers, n_layers, tok, pos, kc, vc, what):
-    """Run one step of `dec` (n_layers deep) and check its last layer block by block from the kernel's own intermediate values."""
+def _check_last_layer_blocks(dec, layers, n_layers, tok, pos, kc, vc, what, k_row_vs_reference=True):
+    """Run one step of `dec` (n_layers deep) and check its last layer block by block from the kernel's own intermediate values.
+    The appended K / V rows are held to Exact and to the reference's per-weight fp16 rounding (the K row to the latter only with
+    k_row_vs_reference)."""
     dec.tokens.fill_(tok)
     dec.positions.fill_(pos)
     dec.step()
@@ -118,20 +122,26 @@ def _check_last_layer_blocks(dec, layers, n_layers, tok, pos, kc, vc, what):
     if n_layers == 1:  # the input of layer 0 is the embedding row, exactly
         assert torch.equal(x_in, dec.embed[tok].cpu()), f'{what}: residual entering layer 0 is not the embedding row'
     _, k_new, v_new = oracle_attn_block(dec, layers[li], x_in[None, :], pos, kc[li], vc[li])
-    ref_attn = oracle_attn_block(dec, layers[li], x_in[None, :], pos, kc[li], vc[li], Q=Exact)[0]
+    ref_attn, k_ex, v_ex = oracle_attn_block(dec, layers[li], x_in[None, :], pos, kc[li], vc[li], Q=Exact)
     check(x_attn, ref_attn[0], rel=ATTN_BLOCK_TOL, what=f'{what}: attention block of layer {li}')
-    check(dec.k_cache[li, 0, :, pos], k_new, rel=KV_ROW_TOL, what=f'{what}: appended K row, layer {li}')
+    if k_row_vs_reference:
+        check(dec.k_cache[li, 0, :, pos], k_new, rel=KV_ROW_TOL, what=f'{what}: appended K row, layer {li}')
     check(dec.v_cache[li, 0, :, pos], v_new, rel=KV_ROW_TOL, what=f'{what}: appended V row, layer {li}')
+    check(dec.k_cache[li, 0, :, pos], k_ex, rel=KV_ROW_TOL, what=f'{what}: appended K row vs Exact, layer {li}')
+    check(dec.v_cache[li, 0, :, pos], v_ex, rel=KV_ROW_TOL, what=f'{what}: appended V row vs Exact, layer {li}')
     ref_logits = oracle_head(dec, oracle_mlp_block(layers[li], x_attn[None, :]))
     check(dec.logits[0], ref_logits, rel=MLP_HEAD_TOL, what=f'{what}: MLP block of layer {li} + lm_head')
     assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
     return dec.logits[0].float().cpu()
 
 
-def _run_case(size, bits, act, positions, vocab, seed):
+def _run_case(size, bits, act, positions, vocab, seed, gs=128):
     from gptq_b200 import engine
-    dec2 = engine.synthetic_llama(size, bits=bits, groupsize=128, act_order=act, vocab=vocab, seed=seed, max_seq=2048, n_layers=2)
+    dec2 = engine.synthetic_llama(size, bits=bits, groupsize=gs, act_order=act, vocab=vocab, seed=seed, max_seq=2048, n_layers=2)
     assert dec2.launches_per_step() == 1, 'the persistent kernel must be the path under test'
+    for name, ly in dec2.klayers[0].items():
+        if hasattr(ly, 'qweight'):
+            assert ly.hint == (ly.g_idx.numel() if gs == -1 else gs), f'{name}: groupsize hint {ly.hint}'
     dec1 = engine.LlamaDecoder(dec2.layers[:1], dec2.embed, dec2.final_norm, dec2.lm_head, dec2.n_heads, max_seq=2048)
     assert dec1.launches_per_step() == 1
     gen = torch.Generator(device=dec2.dev).manual_seed(seed + 100)
@@ -141,11 +151,17 @@ def _run_case(size, bits, act, positions, vocab, seed):
     layers = _cpu_layers(dec2)
     for i, pos in enumerate(positions):
         tok = (17 * i + 3) % vocab
-        what = f'{size} int{bits} act={act} pos={pos}'
+        what = f'{size} int{bits} g{gs} act={act} pos={pos}'
         dec1.k_cache.copy_(dec2.k_cache[:1])
         dec1.v_cache.copy_(dec2.v_cache[:1])
-        _check_last_layer_blocks(dec1, layers, 1, tok, pos, kc, vc, what + ' (1 layer)')
-        logits2 = _check_last_layer_blocks(dec2, layers, 2, tok, pos, kc, vc, what + ' (2 layers)')
+        # The K row is rotated after the fp16 rounding of k, so a one-ulp difference in k before RoPE can land on a small element of the
+        # rotated row, whose bound is relative to the row's rms: whether the reference's per-weight fp16 rounding does that is a matter of
+        # the random draw, not of the groupsize.  The draw of the gs -1 case does it: at context 2047, layer 1, one K-row element is
+        # 1.15 of its bound from the reference rounding, while the kernel equals Exact there (measured: fp64 9.289385, kernel and Exact
+        # 9.2890625, the nearest fp16; reference rounding 9.296875).  That case holds its K rows to Exact only.
+        kw = dict(k_row_vs_reference=gs != -1)
+        _check_last_layer_blocks(dec1, layers, 1, tok, pos, kc, vc, what + ' (1 layer)', **kw)
+        logits2 = _check_last_layer_blocks(dec2, layers, 2, tok, pos, kc, vc, what + ' (2 layers)', **kw)
         # end to end from the embedding
         x = dec2.embed[tok].cpu()[None, :].clone()
         for li in range(2):
@@ -160,6 +176,13 @@ def _run_case(size, bits, act, positions, vocab, seed):
 def test_mega_kernel_7b_int4_g128_matches_oracle():
     """BASELINE config 2 shapes (hidden 4096, intermediate 11008, 32 heads, vocab 32000), the configuration bench.py times."""
     _run_case('7b', 4, False, [0, 255, 256, 2046, 2047], 32000, seed=11)
+
+
+@pytest.mark.parametrize('gs', [32, 1024, -1])
+def test_mega_kernel_7b_int4_groupsizes_match_oracle(gs):
+    """The same 7B check at the other groupsizes of published checkpoints: 32 (one k-step per stage), 1024 (down_proj's K = 11008 ends
+    in a partial group of 768) and -1 (one group per linear: 4096, and 11008 on down_proj)."""
+    _run_case('7b', 4, False, [0, 2047], 32000, seed=14, gs=gs)
 
 
 def test_mega_kernel_13b_int3_actorder_matches_oracle():

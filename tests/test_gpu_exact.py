@@ -198,8 +198,45 @@ def test_kernel_form_onehot(ops, bits, act):
         assert_equal(out, X.onehot_expect(L.W, rows, mult), what, lambda r, n: f"m={r % M} k'={ks[r]} (stored row {rows[r]}) n={n}")
 
 
+@pytest.mark.parametrize('M', [1, 5, 8, 129])
+def test_onehot_partial_last_group(ops, M):
+    """down_proj at gs 1024: K = 11008 = 10 x 1024 + 768, so the last of the 11 groups is partial.  One-hot rows at every k % 8, both
+    sides of every group boundary (the last one at 10240 included), the first / last 64 k and the matvec's CTA-range edges, through the
+    split-K matvec (M <= 8) and the wgmma GEMM (M = 129)."""
+    K, N, gs = 11008, 4096, 1024
+    L = random_layer(K, N, 4, gs, seed=K + gs)
+    ks0 = X.sampled_ks(K, gs, X.matvec_cta_ks(K, N), seed=gs)
+    assert {10239, 10240, K - 1} <= set(ks0)
+    ks = cyclic(ks0, M)
+    x, mult = X.onehot_rows(ks, K, salt=M)
+    what = f'one-hot partial last group K={K} gs={gs} M={M}'
+    fn = lambda xc: ops.matmul248(xc, *L.dev, 4, 15, groupsize=gs)
+    if M <= 8:
+        out = batched_calls(fn, x.cuda(), M, MATVEC, what)
+        where = lambda r, n: X.matvec_where(K, N, gs, r % M, n, ks[r]) + f', call {r // M}'
+    else:
+        out = batched_calls(fn, x.cuda(), M, gemm_kernel(M), what)
+        where = lambda r, n: X.gemm_where(M, K, gs, r % M, n, ks[r]) + f', call {r // M}'
+    assert_equal(out, X.onehot_expect(L.W, ks, mult), what, where)
+
+
 # ============================================================================= integer-exact sums at full size
 SHAPES_7B = [(4096, 4096), (4096, 12288), (11008, 4096)]
+
+
+@pytest.mark.parametrize('M', [1, 5, 8, 129, 512])
+def test_integer_exact_partial_last_group(ops, M):
+    """down_proj at gs 1024 (the last of 11 groups holds 768 k) and power-of-two scales per (group, column): out == fp16(exact) through
+    the matvec (M <= 8) and the wgmma GEMM, so a scale or zero of the partial group read from the wrong row shows in every column."""
+    K, N, gs = 11008, 4096, 1024
+    L = pow2_layer(K, N, gs, seed=K + gs)
+    assert L.cpu[1].shape[0] == 11
+    x = X.int_x(M, K, -2, 2, seed=M).cuda()
+    what = f'integer-exact partial last group K={K} gs={gs} M={M}'
+    out = run_kernel(lambda: ops.matmul248(x, *L.dev, 4, 15, groupsize=gs), MATVEC if M <= 8 else gemm_kernel(M), what)
+    exp = fp16_from_fp64(X.exact_product(x, L.W)).cuda()
+    where = (lambda m, n: X.matvec_where(K, N, gs, m, n)) if M <= 8 else (lambda m, n: X.gemm_where(M, K, gs, m, n))
+    assert_equal(out, exp, what, where)
 
 
 @pytest.mark.parametrize('K,N', SHAPES_7B)

@@ -4,16 +4,16 @@ and the prefill, on both engines (tiny: kernel chain, tiny256: persistent kernel
 import pytest
 import torch
 
-from gpu_util import assert_rel_close
+from gpu_util import assert_rel_close, run_kernel
 
 pytestmark = pytest.mark.gpu
 
 MODELS = [('tiny', 4, False), ('tiny256', 4, False), ('tiny256', 3, True)]
 
 
-def _model(size, bits, act, seed, **kw):
+def _model(size, bits, act, seed, gs=64, **kw):
     from gptq_b200 import engine
-    return engine.synthetic_llama(size, bits=bits, groupsize=64, act_order=act, vocab=300, seed=seed, **kw)
+    return engine.synthetic_llama(size, bits=bits, groupsize=gs, act_order=act, vocab=300, seed=seed, **kw)
 
 
 def _ids(n, seed):
@@ -31,7 +31,19 @@ def _step_all(dec, toks, start):
 def test_extend_after_decode_matches_stepping(size, bits, act):
     """10 decode steps, then extend() with the next 29 tokens: the same cache rows as stepping them (1e-2) and the same logits at the next
     step (2e-2), the bounds of test_prefill_then_decode_matches_token_by_token."""
-    dec = _model(size, bits, act, seed=5, max_seq=96)
+    _extend_after_decode(_model(size, bits, act, seed=5, max_seq=96))
+
+
+@pytest.mark.parametrize('gs, kernel', [(32, 'qlinear_generic_kernel'), (-1, 'qgemm_wgmma_kernel')])
+def test_extend_after_decode_at_groupsizes(gs, kernel):
+    """The same on the persistent-kernel model at groupsize 32 and -1 (one group per linear: 256, and 768 on down_proj).  The 29-row pass
+    asserts its kernels: the wgmma GEMM needs groupsize % 64 == 0, so at 32 every quantized linear of it runs on the generic kernel."""
+    dec = _model('tiny256', 4, False, seed=5, gs=gs, max_seq=96)
+    assert dec.launches_per_step() == 1
+    _extend_after_decode(dec, kernel, f'gs={gs}')
+
+
+def _extend_after_decode(dec, kernel=None, what=''):
     prompt = _ids(40, 2)
     _step_all(dec, prompt, 0)
     ref_logits, ref_k, ref_v = dec.logits[0].float().clone(), dec.k_cache[:, 0, :, :40].float().clone(), dec.v_cache[:, 0, :, :40].float().clone()
@@ -40,14 +52,19 @@ def test_extend_after_decode_matches_stepping(size, bits, act):
     dec.v_cache.zero_()
     _step_all(dec, prompt[:10], 0)
     assert dec.lengths == [10] and dec.cached_tokens == [prompt[:10]]
-    assert dec.extend([prompt[10:39]]) == [39]
+
+    def extend():  # repeatable (run_kernel may trace it again): from the 10 cached positions each time
+        dec.lengths, dec.cached_tokens = [10], [prompt[:10]]
+        return dec.extend([prompt[10:39]])
+
+    assert (extend() if kernel is None else run_kernel(extend, kernel, f'extend of 29 rows {what}')) == [39]
     assert dec.lengths == [39] and dec.cached_tokens == [prompt[:39]]
-    assert_rel_close(dec.k_cache[:, 0, :, 10:39], ref_k[:, :, 10:39], rel=1e-2, what='extended K rows')
-    assert_rel_close(dec.v_cache[:, 0, :, 10:39], ref_v[:, :, 10:39], rel=1e-2, what='extended V rows')
+    assert_rel_close(dec.k_cache[:, 0, :, 10:39], ref_k[:, :, 10:39], rel=1e-2, what=f'extended K rows {what}')
+    assert_rel_close(dec.v_cache[:, 0, :, 10:39], ref_v[:, :, 10:39], rel=1e-2, what=f'extended V rows {what}')
     dec.set_input(prompt[39], 39)
     dec.step()
     torch.cuda.synchronize()
-    assert_rel_close(dec.logits[0], ref_logits, rel=2e-2, what='logits after extend + 1 decode step')
+    assert_rel_close(dec.logits[0], ref_logits, rel=2e-2, what=f'logits after extend + 1 decode step {what}')
 
 
 @pytest.mark.parametrize('size, bits, act', MODELS)

@@ -7,9 +7,10 @@ asserts which kernel served it: the tuned paths fall back to the generic kernel 
 
   * wgmma GEMM: an explicit table over M (tile edges 128 / 256 / 384, ragged and fully out-of-bounds TMA boxes), K (1 and 3
     K steps, i.e. the prologue / tail guards of the TMA and register rings; 172 steps at 11008), N (1 .. 96 column tiles),
-    groupsize (64, 128, K), bias and a strided activation, so that each instantiation meets every edge at least once;
+    groupsize (64, 128, K, and 1024 on K = 11008: a partial last group), bias and a strided activation, so that each instantiation
+    meets every edge at least once;
   * split-K matvec: M = 1..8 at the 7B shapes (two slabs per CTA: workspace partials, last-arriver reduction), a ragged N and
-    groupsizes 32 / 96 / 128 / K; after every call the workspace counters must be back to zero;
+    groupsizes 32 / 96 / 128 / K, and 1024 on K = 11008; after every call the workspace counters must be back to zero;
   * documented fallbacks (misaligned x, groupsize 32 or N = 96 at M > 8) must reach the generic kernel and still be right;
   * determinism: repeated calls, and a call between two shapes that share the workspace, give bit-identical results.
 """
@@ -76,8 +77,9 @@ def workspace_counters(ops, dev, N):
 
 
 # ============================================================================= wgmma GEMM
-# (M, K, N, gs, bias, ldx): rows 1-7 run <false, 1, 6> (M <= 128), rows 8-14 <false, 2, 4>.  Each block holds every K, N, gs in
-# {64, 128, K}, bias on and off and a strided x at least once.
+# (M, K, N, gs, bias, ldx): rows with M <= 128 run <false, 1, 6>, the others <false, 2, 4>.  Each instantiation meets every K, N, gs in
+# {64, 128, K}, a partial last group (gs 1024 on K = 11008), bias on and off and a strided x at least once
+# (test_wgmma_table_covers_every_edge_per_instantiation).
 GEMM_TABLE = [
     (9, 64, 128, 64, True, None),         # 1 K step, gs = K, one column tile
     (64, 192, 384, 64, False, 192 + 64),  # 3 K steps (fewer than the B register ring and the TMA lookahead), strided x
@@ -93,6 +95,11 @@ GEMM_TABLE = [
     (384, 11008, 4096, 128, False, 11008 + 64),  # 1.5 tiles: the last tile's second box out of bounds; strided
     (1000, 4096, 4096, 4096, True, None),  # one group, ragged last tile
     (384, 192, 384, 192, True, None),     # gs = K = 192
+    # down_proj at the groupsizes of published checkpoints: 1024 (11008 = 10 x 1024 + 768: a partial last group) and full (gs = K)
+    (9, 11008, 4096, 1024, False, None),
+    (128, 11008, 4096, 11008, True, None),
+    (257, 11008, 4096, 1024, True, 11008 + 64),
+    (1000, 11008, 4096, 11008, False, None),
 ]
 
 
@@ -104,7 +111,10 @@ def test_wgmma_gemm_edges(ops, M, K, N, gs, bias, ldx):
     what = f'wgmma M={M} K={K} N={N} gs={gs} bias={bias} ldx={ldx or K}'
     kernel = GEMM_2 if M > 128 else GEMM_1
     out = run_kernel(lambda: ops.matmul248(x, *L.dev, 4, 15, bias=L.bias, groupsize=gs), kernel, what)
-    note(f'wgmma {kernel}', check_fp64_bound(out, x, L.W, L.bias, what, locate=lambda m, n: X.gemm_where(M, K, gs, m, n)))
+    ratio = check_fp64_bound(out, x, L.W, L.bias, what, locate=lambda m, n: X.gemm_where(M, K, gs, m, n))
+    note(f'wgmma {kernel}', ratio)
+    if gs in (1024, 11008):
+        note('wgmma, K = 11008 at gs 1024 / 11008', ratio)
 
 
 def test_wgmma_table_covers_every_edge_per_instantiation():
@@ -113,6 +123,7 @@ def test_wgmma_table_covers_every_edge_per_instantiation():
         assert {r[1] for r in rows} == {64, 128, 192, 4096, 11008}
         assert {r[2] for r in rows} == {128, 384, 4096, 12288}
         assert {64, 128} <= {r[3] for r in rows} and any(r[3] == r[1] for r in rows)
+        assert any(r[1] % r[3] for r in rows) and any(r[1] == r[3] == 11008 for r in rows)  # a partial last group; down_proj at gs = K
         assert {r[4] for r in rows} == {True, False} and any(r[5] for r in rows)
     assert {r[0] for r in GEMM_TABLE} == {9, 64, 127, 128, 129, 255, 256, 257, 384, 1000}
 
@@ -131,6 +142,7 @@ def test_wgmma_fused_mlp_edges(ops, M, K, gs):
 MATVEC_SHAPES = [(4096, 4096), (4096, 12288), (11008, 4096), (4096, 4096 + 96), (256, 96)]
 MATVEC_CASES = [(M, K, N, 128) for K, N in MATVEC_SHAPES for M in range(1, 9)]
 MATVEC_CASES += [(M, K, N, gs) for K, N in MATVEC_SHAPES for gs in (32, 96, K) for M in (2, 5, 8)]
+MATVEC_CASES += [(M, 11008, 4096, 1024) for M in (1, 2, 5, 8)]  # partial last group: 11008 = 10 x 1024 + 768
 
 
 @pytest.mark.parametrize('M,K,N,gs', MATVEC_CASES)
@@ -143,7 +155,10 @@ def test_matvec_edges(ops, M, K, N, gs):
     torch.cuda.synchronize()
     ctr = workspace_counters(ops, x.device, N)
     assert int(ctr.count_nonzero()) == 0, f'{what}: workspace counters left non-zero'
-    note('matvec', check_fp64_bound(out, x, L.W, L.bias, what, locate=lambda m, n: X.matvec_where(K, N, gs, m, n)))
+    ratio = check_fp64_bound(out, x, L.W, L.bias, what, locate=lambda m, n: X.matvec_where(K, N, gs, m, n))
+    note('matvec', ratio)
+    if gs in (1024, 11008):
+        note('matvec, K = 11008 at gs 1024 / 11008', ratio)
 
 
 @pytest.mark.parametrize('M', range(1, 9))

@@ -6,7 +6,7 @@ import math
 import pytest
 import torch
 
-from gpu_util import launched_kernels, report, ulp16
+from gpu_util import launched_kernels, report, run_kernel, ulp16
 from test_gpu_engine import _oracle_decode
 
 pytestmark = pytest.mark.gpu
@@ -149,15 +149,28 @@ def test_score_matches_the_oracle(size, bits, act):
     and the logsumexp move by at most that each: 2 x 2e-2 x max|ref logits| per element."""
     from gptq_b200 import engine
     dec = engine.synthetic_llama(size, bits=bits, groupsize=64, act_order=act, vocab=300, seed=bits + act, max_seq=16, use_graph=False)
-    g = torch.Generator().manual_seed(bits)
+    _score_against_oracle(dec, bits, f'{size} bits={bits} act={act}')
+
+
+@pytest.mark.parametrize('gs, kernel', [(32, 'qlinear_generic_kernel'), (-1, 'qgemm_wgmma_kernel')])
+def test_score_matches_the_oracle_at_groupsizes(gs, kernel):
+    """The same at groupsize 32 and -1 (one group per linear: 256, and 768 on down_proj).  The 34-row pass asserts its kernels: the wgmma
+    GEMM needs groupsize % 64 == 0, so at 32 every quantized linear of it runs on the generic kernel."""
+    from gptq_b200 import engine
+    dec = engine.synthetic_llama('tiny256', bits=4, groupsize=gs, vocab=300, seed=7, max_seq=16, use_graph=False)
+    _score_against_oracle(dec, 4, f'tiny256 gs={gs}', kernel)
+
+
+def _score_against_oracle(dec, seed, what, kernel=None):
+    g = torch.Generator().manual_seed(seed)
     seqs = [torch.randint(0, 300, (n, ), generator=g).tolist() for n in (9, 2, 23)]
-    out = dec.score(seqs)
+    out = dec.score(seqs) if kernel is None else run_kernel(lambda: dec.score(seqs), kernel, f'{what}: score')
     assert [o.shape[0] for o in out] == [8, 1, 22] and all(o.dtype == torch.float32 for o in out)
     for s, lp in zip(seqs, out):
         logits = _oracle_decode(dec, s)[:-1].double()
         ref = torch.log_softmax(logits, -1).gather(1, torch.tensor(s[1:])[:, None])[:, 0]
         bound = 2 * 2e-2 * logits.abs().amax(-1)
-        report(((lp.cpu().double() - ref).abs() / bound).max().item(), f'{size} bits={bits} act={act} n={len(s)}')
+        report(((lp.cpu().double() - ref).abs() / bound).max().item(), f'{what} n={len(s)}')
 
 
 def test_perplexity_matches_the_reference_formula_on_the_hf_modules():
