@@ -23,7 +23,8 @@
 //    same arithmetic as the reference's tl.dot (fp16 operands, fp32 accumulate) at 1/4 of the issue
 //    slots a CUDA-core FMA loop needs; the k-order inside a run of 8 is permuted identically in x and W.
 //  * Partials of CTAs that share a slab go through a workspace; the last arriver (atomic counter, which
-//    it resets) reduces them in a fixed order -> deterministic results, no memset between launches.
+//    it resets) reduces them in a fixed order and zeroes them -> deterministic results, no memset between
+//    launches, and the workspace is left zeroed for any shape or kernel that uses it next.
 //  * Optional RMSNorm prologue (the reference's rms_norm_fwd_fused, quant/triton_norm.py:21-39) and
 //    residual epilogue so that a decoder layer needs 5 launches; PDL hooks (griddepcontrol) let the
 //    weight prefetch of kernel n+1 overlap the tail of kernel n.
@@ -385,7 +386,7 @@ __global__ void __launch_bounds__(kThreads, 2) qmatvec_int4_kernel(const SkinnyP
             const int slab = pend_slab_s[i], ncontrib = pend_nc_s[i];
             const int col0 = slab * kSlabCols;
             const int ncols = min(kSlabCols, N - col0);
-            const float* sp = p.ws_partial + (size_t)slab * p.max_contrib * (NW * p.M * kSlabCols);
+            float* sp = p.ws_partial + (size_t)slab * p.max_contrib * (NW * p.M * kSlabCols);
             if (tid < ncols) {
                 for (int m = 0; m < p.M; ++m) {
                     float a = 0.f, b = 0.f;
@@ -405,6 +406,11 @@ __global__ void __launch_bounds__(kThreads, 2) qmatvec_int4_kernel(const SkinnyP
                             if (c0 + j < ncontrib) {
                                 a += va[j];
                                 if constexpr (DUAL) b += vb[j];
+                                // leave the workspace zeroed (gptq_b200.h): a later call with more slabs has its counters where these
+                                // partials lie, and other kernels sharing the workspace accumulate into it
+                                float* pc = sp + (size_t)(c0 + j) * (NW * p.M * kSlabCols);
+                                pc[(size_t)m * kSlabCols + tid] = 0.f;
+                                if constexpr (DUAL) pc[(size_t)(p.M + m) * kSlabCols + tid] = 0.f;
                             }
                         }
                     }

@@ -30,7 +30,8 @@ import torch
 from gpu_util import fp16_from_fp64
 from oracle import gptq_oracle as O
 
-SHAPES = {'7b': (4096, 11008, 32), '13b': (5120, 13824, 40)}  # hidden, intermediate, heads (engine.LLAMA_SHAPES)
+# hidden, intermediate, heads (engine.LLAMA_SHAPES)
+SHAPES = {'7b': (4096, 11008, 32), '13b': (5120, 13824, 40), '33b': (6656, 17920, 52), '65b': (8192, 22016, 64)}
 POS_FEATS = 64  # every embedding row is +2^-4 on these features: the gate taps read x = +1
 STAGE_K = 128   # k per stage of the persistent kernel (4 k-steps of 32), inside one group
 STEP_K = 32
@@ -146,6 +147,11 @@ def fp16(v):
     return fp16_from_fp64(v).to(v.device)
 
 
+def product(x, lin, device, cols=4096):
+    """float64 x [B, K] @ lin.weight(), built column block by column block (a 65B qkv weight is 1.6 GB in float64)."""
+    return torch.cat([x @ lin.weight(slice(c, c + cols), device=device) for c in range(0, lin.N, cols)], 1)
+
+
 class Expect:
     """The exact outputs of one step at position 0 for input rows x_in [B, H] (fp16 embedding rows), all float64 / fp16 on `device`."""
 
@@ -154,14 +160,14 @@ class Expect:
         self.x_in = x_in.to(device)
         self.x = self.x_in.double() * 16  # RMSNorm output, exactly +-1
         H = L.H
-        self.qkv64 = self.x @ L.qkv.weight(device=device)
+        self.qkv64 = product(self.x, L.qkv, device)
         self.k, self.v = fp16(self.qkv64[:, H:2 * H]), fp16(self.qkv64[:, 2 * H:])
-        self.o64 = self.v.double() @ L.o.weight(device=device)
+        self.o64 = product(self.v.double(), L.o, device)
         self.x_attn = fp16(self.x_in.double() + fp16(self.o64).double())  # o-probe: MLP scales 0
-        self.a = self.x @ L.gate.weight(device=device)
-        self.b = self.x @ L.up.weight(device=device)
+        self.a = product(self.x, L.gate, device)
+        self.b = product(self.x, L.up, device)
         self.h = fp16(self.a * self.b)  # sigmoid(a) == 1 in fp32 (module docstring)
-        self.d64 = self.h.double() @ L.down.weight(device=device)
+        self.d64 = product(self.h.double(), L.down, device)
         self.x_mlp = fp16(self.x_in.double() + fp16(self.d64).double())  # mlp-probe: o_proj scales 0
 
 
@@ -246,10 +252,32 @@ def teeth(L, x_in, cols=1024):
     return res
 
 
-# (size, gs, bits, act_order, batch, engine): the GPU cases of tests/test_gpu_decode_groupsize.py
+# (size, gs, bits, act_order, batch, engine): the GPU cases of tests/test_gpu_decode_groupsize.py.  batch 'max' is the largest batch the
+# persistent plan takes at that shape, 'max+1' one sequence more (the kernel chain); both depend on the device (max_persistent_batch).
 CASES = [('7b', gs, 4, False, B, 'persistent') for gs in (32, 64, 128, 1024, 'full') for B in (1, 8)]
 CASES += [('13b', 32, 3, True, 1, 'persistent'), ('13b', 32, 4, False, 7, 'chain'), ('13b', 'full', 4, False, 7, 'chain')]
+# 65B: hidden 8192 (the persistent kernel's limit), one lm_head row per stage; gs 1024 ends down_proj (K = 22016) in a partial group of 512.
+# 33B at gs 1024: every linear ends in a partial group of 512 (6656 = 6 x 1024 + 512, 17920 = 17 x 1024 + 512).
+CASES += [('65b', 128, 4, False, 1, 'persistent'), ('65b', 128, 4, False, 'max', 'persistent'), ('65b', 128, 4, False, 'max+1', 'chain'),
+          ('65b', 1024, 4, False, 1, 'persistent'), ('65b', 128, 4, True, 1, 'persistent'),
+          ('33b', 1024, 4, False, 1, 'persistent'), ('33b', 1024, 4, False, 'max', 'persistent'), ('33b', 'full', 4, False, 'max+1', 'chain')]
 VOCAB = 64
+
+
+def max_persistent_batch(n_heads, sms):
+    """The largest batch the persistent plan takes: one attention team per (sequence, head) pair, 2 teams per SM (mega_plan), at most 8."""
+    return min(8, 2 * sms // n_heads)
+
+
+def resolve_batch(B, n_heads, sms):
+    """A case's batch on a device with `sms` SMs (CASES)."""
+    if B == 'max':
+        return max_persistent_batch(n_heads, sms)
+    if B == 'max+1':
+        b = max_persistent_batch(n_heads, sms)
+        assert b < 8, f'{n_heads} heads: every batch fits the persistent plan on {sms} SMs'
+        return b + 1
+    return B
 
 
 def tokens(B):
@@ -258,5 +286,5 @@ def tokens(B):
 
 def layer_for(size, gs, bits, act_order):
     """The probe layer of a case (a fixed seed per configuration, so the CPU and GPU tests see the same fields)."""
-    seed = {'7b': 1, '13b': 2}[size] * 100000 + (0 if gs == 'full' else gs) * 10 + bits + 5 * int(act_order)
+    seed = {'7b': 1, '13b': 2, '33b': 3, '65b': 4}[size] * 100000 + (0 if gs == 'full' else gs) * 10 + bits + 5 * int(act_order)
     return ProbeLayer(size, gs, bits, act_order, seed)

@@ -5,7 +5,7 @@
   stay above the fp16 subnormal grid after the 1/16 pre-scaling of the odd nibbles.
 * Teeth: a kernel that read the neighbouring group's scale or zero for one stage, took another sequence's sum of x, or dropped or repeated
   one k-step would produce an observed output (K row, x after attention, x after the layer) that differs from the anchor in many
-  elements, at every groupsize, the partial last group of down_proj at 1024 included.
+  elements, at every groupsize, the partial last group of down_proj at 1024 included, and at the 65B and 33B probe layers.
 """
 from functools import lru_cache
 
@@ -41,7 +41,17 @@ def test_probe_sums_are_exact_in_fp32(size, gs, bits, act):
 @pytest.mark.parametrize('gs', [32, 128, 1024, 'full'])
 def test_probe_anchors_have_teeth(gs):
     """At batch 8: each corruption moves many of the observed elements (at least a quarter of them; the sum-of-x one only sequence 1)."""
-    L = layer('7b', gs, 4, False)
+    check_teeth('7b', gs)
+
+
+@pytest.mark.parametrize('size,gs', [('65b', 128), ('65b', 1024), ('33b', 1024)])
+def test_probe_anchors_have_teeth_large(size, gs):
+    """The same at the 65B and 33B probe layers; at 33B gs 1024 every corruption lands in a partial last group of 512."""
+    check_teeth(size, gs)
+
+
+def check_teeth(size, gs):
+    L = layer(size, gs, 4, False)
     x_in = P.embed_rows(P.VOCAB, L.H)[torch.tensor(P.tokens(8))]
     res = P.teeth(L, x_in)
     names = {n for _, n in res}
@@ -50,6 +60,6 @@ def test_probe_anchors_have_teeth(gs):
         assert {'neighbour scale', 'neighbour zero'} <= names
     for (lin, name), (diff, total) in sorted(res.items()):
         frac = diff / total
-        print(f'  gs={gs} {lin} {name}: {diff} / {total} observed elements differ')
+        print(f'  {size} gs={gs} {lin} {name}: {diff} / {total} observed elements differ')
         need = 0.25 / 8 if name == 'other sequence sum of x' else 0.25
-        assert frac >= need, f'gs={gs} {lin} {name}: only {diff} / {total} elements differ'
+        assert frac >= need, f'{size} gs={gs} {lin} {name}: only {diff} / {total} elements differ'

@@ -87,6 +87,28 @@ def test_ragged_positions_match_single_sequence_steps(size, bits, act, positions
     _check_rows(dec.logits, singles, f'{size} int{bits} act={act}')
 
 
+def test_ragged_positions_match_single_sequence_steps_65b():
+    """The same at bench.py's 65B shapes (int4 g128, 2 layers) and the largest batch the persistent plan takes there (64 heads: 4 sequences on
+    132 SMs)."""
+    from gptq_b200 import engine
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    B = min(8, 2 * sms // 64)
+    positions = [0, 2047, 256, 1023, 31, 32, 255, 2046][:B]
+    dec = engine.synthetic_llama('65b', bits=4, groupsize=128, vocab=8192, seed=23, max_seq=2048, n_layers=2, batch=B)
+    assert dec.launches_per_step() == 1, f'batch {B}: {dec.launches_per_step()} launches'
+    dec1 = _single_twin(dec)
+    assert dec1.launches_per_step() == 1
+    gen = torch.Generator(device=dec.dev).manual_seed(24)
+    dec.k_cache.normal_(0, 0.5, generator=gen)
+    dec.v_cache.normal_(0, 0.5, generator=gen)
+    toks = [(37 * b + 5) % 8192 for b in range(B)]
+    singles = _singles(dec1, dec, toks, positions)
+    dec.set_input(toks, positions)
+    dec.step()
+    torch.cuda.synchronize()
+    _check_rows(dec.logits, singles, f'65b batch {B}')
+
+
 def test_batched_step_writes_only_its_own_cache_rows():
     """A batched step rewrites one K row and one V row per sequence and layer, at that sequence's position; a position outside the cache
     is clamped for its own sequence only."""
@@ -175,4 +197,32 @@ def test_fallback_boundary_13b():
         dec.step()
         torch.cuda.synchronize()
         _check_rows(dec.logits, singles, f'13b batch {B}')
+        del dec
+
+
+@pytest.mark.parametrize('size', ['65b', '33b'])
+def test_fallback_boundary_large(size):
+    """The same boundary at 65B (64 heads: 4 sequences persistent on 132 SMs, 5 on the kernel chain) and 33B (52 heads: 5, then 6), on one
+    layer: the chain and the batch-1 persistent step differ in fp32 summation order, and behind a second layer that difference re-rolled to
+    3.0e-3 of the rms at 33B in one of two runs, the spread bound itself."""
+    from gptq_b200 import engine
+    nh = engine.LLAMA_SHAPES[size][3]
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    b_in = min(8, 2 * sms // nh)
+    assert b_in < 8
+    positions = [0, 100, 200, 255, 256, 300, 400, 511]
+    dec1 = None
+    for B in (b_in, b_in + 1):
+        dec = engine.synthetic_llama(size, bits=4, groupsize=128, vocab=4096, seed=33, max_seq=512, n_layers=1, batch=B)
+        assert (dec.launches_per_step() == 1) == (B == b_in), f'{size} batch {B}: {dec.launches_per_step()} launches'
+        dec1 = dec1 or _single_twin(dec)
+        gen = torch.Generator(device=dec.dev).manual_seed(34)
+        dec.k_cache.normal_(0, 0.5, generator=gen)
+        dec.v_cache.normal_(0, 0.5, generator=gen)
+        toks = [(11 * b + 1) % 4096 for b in range(B)]
+        singles = _singles(dec1, dec, toks, positions[:B])
+        dec.set_input(toks, positions[:B])
+        dec.step()
+        torch.cuda.synchronize()
+        _check_rows(dec.logits, singles, f'{size} batch {B}')
         del dec

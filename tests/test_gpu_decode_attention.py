@@ -207,6 +207,49 @@ def test_chain_13b_batch7():
     run_sweeps(probe, 'chain 13b batch 7', [[0, 1, 255, 256, 511, 800, 1023], [1023, 0, 1, 2, 3, 4, 256]])
 
 
+# ----------------------------------------------------------------------------- the 65B and 33B shapes
+def max_persistent_batch(size):
+    """The largest batch the persistent plan takes at `size`: one attention team per (sequence, head) pair, 2 teams per SM, at most 8."""
+    from gptq_b200 import engine
+    nh = engine.LLAMA_SHAPES[size][3]
+    return min(8, 2 * torch.cuda.get_device_properties(0).multi_processor_count // nh)
+
+
+@pytest.mark.parametrize('size', ['65b', '33b'])
+def test_persistent_large_positions(size):
+    """LLaMA-65B (64 heads, 4 or 5 teams per head on 132 SMs) and LLaMA-33B (52 heads, 5 or 6) at batch 1: the unit, split and team edges
+    of POS_7B and of this shape's team partition; at 65B every key of the 2047-key context is heavy once."""
+    probe = P.Probe(size, max_seq=2048)
+    assert probe.persistent and probe.dec.launches_per_step() == 1
+    assert probe.nb // probe.nh + 1 <= 12, 'the general merge would serve this shape'
+    positions = sorted(set(POS_7B) | set(P.team_edge_positions(probe.nh, probe.nb)))
+    run_sweeps(probe, size, [[p] for p in positions], full_rotation=(2047, ) if size == '65b' else ())
+
+
+def _ragged(B):
+    return [[2047, 0, 255, 256, 1023, 31, 32, 1500][:B], [0] * B]
+
+
+@pytest.mark.parametrize('size', ['65b', '33b'])
+def test_persistent_large_largest_batch(size):
+    """The largest batch the persistent plan takes at 65B / 33B (4 / 5 sequences on 132 SMs): every team serves one (sequence, head) pair or
+    a share of one; ragged positions and every sequence at position 0."""
+    B = max_persistent_batch(size)
+    probe = P.Probe(size, batch=B, max_seq=2048)
+    assert probe.persistent and probe.dec.launches_per_step() == 1, f'{size} batch {B}'
+    run_sweeps(probe, f'{size} batch {B}', _ragged(B))
+
+
+@pytest.mark.parametrize('size', ['65b', '33b'])
+def test_chain_large_above_the_plan(size):
+    """One sequence more than the persistent plan takes at 65B / 33B: the kernel chain serves the batch."""
+    B = max_persistent_batch(size) + 1
+    assert B <= 8
+    probe = P.Probe(size, batch=B, max_seq=1024)
+    assert not probe.persistent and probe.dec.launches_per_step() > 1, f'{size} batch {B}'
+    run_sweeps(probe, f'chain {size} batch {B}', [[1023, 0, 1, 255, 256, 511, 800, 31][:B], [0] * B])
+
+
 # ----------------------------------------------------------------------------- lm_head and greedy token
 @pytest.mark.parametrize('size,batch,vocab,dups,persistent', [
     ('7b', 1, 32001, [1001, 1002, 32000], True),
@@ -215,6 +258,20 @@ def test_chain_13b_batch7():
     ('tiny', 3, 600, [7, 8, 599], False),
 ])
 def test_lm_head_and_greedy_token(size, batch, vocab, dups, persistent):
+    lm_head_and_greedy_token(size, batch, vocab, dups, persistent)
+
+
+@pytest.mark.parametrize('size,batch,persistent', [('65b', 1, True), ('65b', 'max', True), ('65b', 'max+1', False), ('33b', 1, True),
+                                                   ('33b', 'max', True)])
+def test_lm_head_and_greedy_token_large(size, batch, persistent):
+    """The same at 65B (one 16384-byte lm_head row fills a stage: every row is a stage of its own) and 33B (13312-byte rows), at batch 1,
+    the largest persistent batch and, at 65B, one sequence more (the kernel chain); vocab 32001."""
+    if batch != 1:
+        batch = max_persistent_batch(size) + (batch == 'max+1')
+    lm_head_and_greedy_token(size, batch, 32001, [1001, 1002, 32000], persistent)
+
+
+def lm_head_and_greedy_token(size, batch, vocab, dups, persistent):
     """A pos-0 step, where the head's input x = fp16(x_in + v_new) is known exactly (and its sum of squares is exact, so the final RMSNorm is
     reproduced bit for bit in float32): the logits within check_fp64_bound, and duplicate maximal rows on both sides of an lm_head stage
     boundary (the persistent kernel stages 2 rows at 7B; vocab 32001 leaves row 32000 alone in a partial last stage) give bitwise equal
@@ -224,7 +281,7 @@ def test_lm_head_and_greedy_token(size, batch, vocab, dups, persistent):
     lm =(torch.randn(vocab, H, generator=torch.Generator().manual_seed(5)) * 0.02).half()
     lm[dups] = 2.0**-6
     probe = P.Probe(size, batch=batch, max_seq=64, vocab=vocab, lm_head=lm)
-    assert probe.persistent == persistent
+    assert probe.persistent == persistent and (probe.dec.launches_per_step() == 1) == persistent
     toks = [(977 * b + 5) % vocab for b in range(batch)]
     positions = [0] * batch
     probe.learn(toks, positions)

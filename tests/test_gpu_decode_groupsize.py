@@ -8,10 +8,16 @@ the step leaves it; every anchor must hold exactly (torch.equal against fp16 of 
 The groupsizes: 32 (one k-step per stage of the persistent kernel, per-step boxes), 64, 128, 1024 (a group spans 8 stages; down_proj's K =
 11008 ends in a partial group of 768) and full (each linear's K: 4096, and 11008 on down_proj -- the reference's --groupsize -1).  At batch
 8 the eight sequences carry distinct tokens, so each lane group of the batched kernel feeds its own x and the epilogue its own sums of x.
+At LLaMA-65B shapes (hidden 8192, the persistent kernel's limit) the cases are gs 128 at batch 1, at the largest persistent batch and one
+sequence above it (the kernel chain), gs 1024 (down_proj, K = 22016, ends in a partial group of 512) and int4 act-order gs 128 (the
+qkv_perm / mlp_perm gathers at H = 8192); at LLaMA-33B gs 1024, where every linear ends in a partial group of 512, at batch 1 and the
+largest persistent batch, and gs full on the kernel chain.  The batch limits come from the device's SM count (gs_probe.resolve_batch).
 Each case asserts its path: the launch count and the groupsize hint of every kernel layer.  tests/test_decode_groupsize_fixtures.py shows
 on the CPU that the fixtures are exact and that a group, sequence or k-step mix-up would break these anchors; the last test here shows it
 on the device.
 """
+from functools import lru_cache
+
 import pytest
 import torch
 
@@ -73,8 +79,19 @@ def x_after(dec, engine_name, B, H, which):
     return dec.scratch[:B * H * 2].view(torch.float16).view(B, H).clone()
 
 
+@lru_cache(maxsize=1)
+def probe_layer(size, gs, bits, act):
+    """The cases of one configuration follow each other in P.CASES: a 65B layer takes tens of seconds to draw on the CPU."""
+    return P.layer_for(size, gs, bits, act)
+
+
+def sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
 def run_case(size, gs, bits, act, B, engine_name):
-    L = P.layer_for(size, gs, bits, act)
+    L = probe_layer(size, gs, bits, act)
+    B = P.resolve_batch(B, L.nh, sms())
     H, dev = L.H, torch.device('cuda:0')
     toks = P.tokens(B)
     x_in = P.embed_rows(P.VOCAB, H)[torch.tensor(toks)]
@@ -114,7 +131,15 @@ def test_decode_linears_bit_exact(size, gs, bits, act, B, engine_name):
 def test_swapped_scale_rows_break_the_anchors():
     """Two adjacent groups' scale rows of qkv swapped in the device copy only (every column has different scales in the two, gs_probe):
     the K rows must then miss their anchor in most elements -- the anchors see a group mix-up in the kernel's indexing."""
-    L = P.layer_for('7b', 128, 4, False)
+    swapped_scale_rows(P.layer_for('7b', 128, 4, False))
+
+
+def test_swapped_scale_rows_break_the_anchors_65b():
+    """The same at LLaMA-65B shapes (hidden 8192): the anchors of the largest configuration see a group mix-up too."""
+    swapped_scale_rows(probe_layer('65b', 128, 4, False))
+
+
+def swapped_scale_rows(L):
     dev = torch.device('cuda:0')
     toks = P.tokens(1)
     E = P.Expect(L, P.embed_rows(P.VOCAB, L.H)[torch.tensor(toks)], device=dev)
@@ -128,7 +153,7 @@ def test_swapped_scale_rows_break_the_anchors():
     step(dec, toks)
     got = dec.k_cache[0, 0, :, 0].reshape(-1)
     off = int((got != E.k[0]).sum())
-    print(f'  qkv scale rows 3 and 4 swapped: {off} / {got.numel()} K-row elements miss the anchor')
+    print(f'  {L.size}: qkv scale rows 3 and 4 swapped: {off} / {got.numel()} K-row elements miss the anchor')
     assert off >= got.numel() // 2, f'only {off} elements moved'
     sc[[3, 4]] = sc[[4, 3]].clone()
     step(dec, toks)

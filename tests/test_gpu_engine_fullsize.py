@@ -4,7 +4,9 @@ The small-model tests (test_gpu_engine.py) cannot reach the stream-K ranges, att
 staging sizes of the 7B / 13B configurations, so here the kernel runs LLaMA-7B-shaped (int4 g128, BASELINE config 2) and
 LLaMA-13B-shaped (int3 g128 act-order, config 4) layers -- two of them, which exercises every inter-layer hand-off -- on a
 randomly filled KV cache at the context positions {0, 255, 256, 2046, 2047}, against the oracle (oracle/gptq_oracle.py); and 7B at
-the groupsizes 32, 1024 and -1 (one group per linear) at the positions {0, 2047}.
+the groupsizes 32, 1024 and -1 (one group per linear) at the positions {0, 2047}.  LLaMA-65B-shaped layers (int4 g128, bench.py
+--config 65b: hidden 8192, the kernel's limit) run at the same five positions, LLaMA-33B-shaped ones at gs 1024 (every linear ends in a
+partial group of 512) at {0, 2047}.
 
 Checked per BLOCK, each block's oracle fed with the kernel's own input to that block (read back from its scratch), so that a
 1e-3-class bound stays meaningful: a decoder is a chain of fp16 rounding points, and a one-ulp difference early on (any other
@@ -66,22 +68,23 @@ MLP_HEAD_TOL = 5e-3       # gate/up -> SwiGLU -> down -> residual -> final norm 
 END_TO_END_TOL = 1.5e-2   # whole step from the embedding: sanity only (see the module docstring)
 
 
-def _cpu_layers(dec):
+def _cpu_layer(ly):
     cpu = lambda t: t.detach().cpu()
-    out = []
-    for ly in dec.layers:
-        d = {k: ((cpu(v.qweight), cpu(v.scales), cpu(v.qzeros), cpu(v.g_idx)), v.bits) for k, v in ly.items() if hasattr(v, 'qweight')}
-        d['input_norm'], d['post_norm'] = cpu(ly['input_norm']), cpu(ly['post_norm'])
-        out.append(d)
-    return out
+    d = {k: ((cpu(v.qweight), cpu(v.scales), cpu(v.qzeros), cpu(v.g_idx)), v.bits) for k, v in ly.items() if hasattr(v, 'qweight')}
+    d['input_norm'], d['post_norm'] = cpu(ly['input_norm']), cpu(ly['post_norm'])
+    return d
 
 
-def oracle_attn_block(dec, ly, x, pos, kc_l, vc_l, Q=Q):
+def _cpu_layers(dec):
+    return [_cpu_layer(ly) for ly in dec.layers]
+
+
+def oracle_attn_block(dec, ly, x, pos, kc_l, vc_l, Q=Q, eps=1e-6):
     """x [1, H] entering a layer -> (x after the attention block, new k rows [nh, hd], new v rows); cache rows [0, pos) of the layer."""
     H, nh = dec.hidden, dec.n_heads
     hd = H // nh
     (w, bits) = ly['qkv']
-    qkv = Q.qlinear_fwd(O.rmsnorm_fwd(x, ly['input_norm'], 1e-6), *w, bits).view(1, 1, 3, nh, hd).clone()
+    qkv = Q.qlinear_fwd(O.rmsnorm_fwd(x, ly['input_norm'], eps), *w, bits).view(1, 1, 3, nh, hd).clone()
     O.rope_inplace(qkv[:, :, :2], torch.tensor([[pos]]))
     q, k, v = qkv[0, 0, 0], qkv[0, 0, 1], qkv[0, 0, 2]
     K = torch.cat([kc_l[0, :, :pos], k[:, None, :]], 1).float()  # [nh, pos+1, hd]
@@ -92,15 +95,15 @@ def oracle_attn_block(dec, ly, x, pos, kc_l, vc_l, Q=Q):
     return x + Q.qlinear_fwd(att, *w, bits), k.clone(), v.clone()
 
 
-def oracle_mlp_block(ly, x):
+def oracle_mlp_block(ly, x, eps=1e-6):
     (wg, bits), (wu, _) = ly['gate'], ly['up']
-    hmid = Q.fused_mlp_fwd(O.rmsnorm_fwd(x, ly['post_norm'], 1e-6), wg, wu, bits)
+    hmid = Q.fused_mlp_fwd(O.rmsnorm_fwd(x, ly['post_norm'], eps), wg, wu, bits)
     (w, bits) = ly['down']
     return x + Q.qlinear_fwd(hmid, *w, bits)
 
 
-def oracle_head(dec, x):
-    xn = O.rmsnorm_fwd(x, dec.final_norm.detach().cpu(), 1e-6)
+def oracle_head(dec, x, eps=1e-6):
+    xn = O.rmsnorm_fwd(x, dec.final_norm.detach().cpu(), eps)
     return (xn.float() @ dec.lm_head.detach().cpu().float().t()).half()[0]
 
 
@@ -109,9 +112,9 @@ def _resid_buffers(dec):
     return [r[0].cpu() for r in resid_buffers(dec)]
 
 
-def _check_last_layer_blocks(dec, layers, n_layers, tok, pos, kc, vc, what, k_row_vs_reference=True):
-    """Run one step of `dec` (n_layers deep) and check its last layer block by block from the kernel's own intermediate values.
-    The appended K / V rows are held to Exact and to the reference's per-weight fp16 rounding (the K row to the latter only with
+def _check_last_layer_blocks(dec, layers, n_layers, tok, pos, kc, vc, what, k_row_vs_reference=True, eps=1e-6):
+    """Run one step of `dec` (n_layers deep, RMSNorm epsilon eps) and check its last layer block by block from the kernel's own intermediate
+    values.  The appended K / V rows are held to Exact and to the reference's per-weight fp16 rounding (the K row to the latter only with
     k_row_vs_reference)."""
     dec.tokens.fill_(tok)
     dec.positions.fill_(pos)
@@ -121,15 +124,15 @@ def _check_last_layer_blocks(dec, layers, n_layers, tok, pos, kc, vc, what, k_ro
     li = n_layers - 1
     if n_layers == 1:  # the input of layer 0 is the embedding row, exactly
         assert torch.equal(x_in, dec.embed[tok].cpu()), f'{what}: residual entering layer 0 is not the embedding row'
-    _, k_new, v_new = oracle_attn_block(dec, layers[li], x_in[None, :], pos, kc[li], vc[li])
-    ref_attn, k_ex, v_ex = oracle_attn_block(dec, layers[li], x_in[None, :], pos, kc[li], vc[li], Q=Exact)
+    _, k_new, v_new = oracle_attn_block(dec, layers[li], x_in[None, :], pos, kc[li], vc[li], eps=eps)
+    ref_attn, k_ex, v_ex = oracle_attn_block(dec, layers[li], x_in[None, :], pos, kc[li], vc[li], Q=Exact, eps=eps)
     check(x_attn, ref_attn[0], rel=ATTN_BLOCK_TOL, what=f'{what}: attention block of layer {li}')
     if k_row_vs_reference:
         check(dec.k_cache[li, 0, :, pos], k_new, rel=KV_ROW_TOL, what=f'{what}: appended K row, layer {li}')
     check(dec.v_cache[li, 0, :, pos], v_new, rel=KV_ROW_TOL, what=f'{what}: appended V row, layer {li}')
     check(dec.k_cache[li, 0, :, pos], k_ex, rel=KV_ROW_TOL, what=f'{what}: appended K row vs Exact, layer {li}')
     check(dec.v_cache[li, 0, :, pos], v_ex, rel=KV_ROW_TOL, what=f'{what}: appended V row vs Exact, layer {li}')
-    ref_logits = oracle_head(dec, oracle_mlp_block(layers[li], x_attn[None, :]))
+    ref_logits = oracle_head(dec, oracle_mlp_block(layers[li], x_attn[None, :], eps), eps)
     check(dec.logits[0], ref_logits, rel=MLP_HEAD_TOL, what=f'{what}: MLP block of layer {li} + lm_head')
     assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
     return dec.logits[0].float().cpu()
@@ -188,6 +191,17 @@ def test_mega_kernel_7b_int4_groupsizes_match_oracle(gs):
 def test_mega_kernel_13b_int3_actorder_matches_oracle():
     """BASELINE config 4 shapes (hidden 5120, intermediate 13824, 40 heads), int3 g128 with act-order g_idx."""
     _run_case('13b', 3, True, [0, 2047], 8192, seed=12)
+
+
+def test_mega_kernel_65b_int4_g128_matches_oracle():
+    """bench.py --config 65b shapes (hidden 8192, intermediate 22016, 64 heads, vocab 32000) at two of its 80 layers."""
+    _run_case('65b', 4, False, [0, 255, 256, 2046, 2047], 32000, seed=16)
+
+
+def test_mega_kernel_33b_int4_g1024_matches_oracle():
+    """LLaMA-33B shapes (hidden 6656, intermediate 17920, 52 heads) at gs 1024: 6656 = 6 x 1024 + 512 and 17920 = 17 x 1024 + 512, so
+    every linear ends in a partial group."""
+    _run_case('33b', 4, False, [0, 2047], 32000, seed=17, gs=1024)
 
 
 def test_mega_kernel_run_to_run_spread_7b():
