@@ -184,6 +184,20 @@ int gptq_cached_attention(const void* q, int64_t ldq, const void* k_cache, const
                                                static_cast<cudaStream_t>(stream)));
 }
 
+int gptq_sample_tokens(const void* logits, int64_t ld, int batch, int vocab, const int32_t* positions, const gptq_sampling* params,
+                       int32_t* next_tokens, gptq_stream_t stream) {
+    if (logits == nullptr || positions == nullptr || params == nullptr || next_tokens == nullptr) return GPTQ_ERR_NULL;
+    if (params->temperature == nullptr || params->top_k == nullptr || params->top_p == nullptr || params->seed == nullptr ||
+        params->eos_token == nullptr || params->min_length == nullptr)
+        return GPTQ_ERR_NULL;
+    if (batch < 1 || batch > kSampleMaxBatch || vocab < 1 || ld < vocab) return GPTQ_ERR_SHAPE;
+    if (vocab > kSampleMaxVocab) return GPTQ_ERR_UNSUPPORTED;
+    if (!aligned(logits, 2) || !aligned(positions, 4) || !aligned(next_tokens, 4) || !aligned(params->temperature, 4) || !aligned(params->top_k, 4) ||
+        !aligned(params->top_p, 4) || !aligned(params->seed, 8) || !aligned(params->eos_token, 4) || !aligned(params->min_length, 4))
+        return GPTQ_ERR_ALIGN;
+    return cuda_status(launch_sample_tokens(logits, ld, batch, vocab, positions, *params, next_tokens, static_cast<cudaStream_t>(stream)));
+}
+
 int gptq_ipc_alloc(size_t bytes, void** ptr, unsigned char handle[64]) {
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "handle size");
     if (ptr == nullptr || handle == nullptr || bytes == 0) return GPTQ_ERR_NULL;

@@ -62,6 +62,11 @@ cudaError_t launch_cached_attention(const void* q, int64_t ldq, const void* k_ca
                                     const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
                                     cudaStream_t stream);
 
+// sample.cu -- one token per row of decode-step logits: temperature / top-k / top-p / Philox draw, or the argmax (gptq_sample_tokens)
+constexpr int kSampleMaxBatch = 8, kSampleMaxVocab = 131072;
+cudaError_t launch_sample_tokens(const void* logits, int64_t ld, int batch, int vocab, const int32_t* positions, const gptq_sampling& params,
+                                 int32_t* next_tokens, cudaStream_t stream);
+
 // decode_mega.cu -- persistent single-kernel decode step (batch 1 to 8, int4 kernel-form layers)
 bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st);
 size_t mega_scratch_bytes(const gptq_llama_model& m, int batch);

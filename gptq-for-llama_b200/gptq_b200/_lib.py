@@ -60,6 +60,11 @@ class LlamaState(ctypes.Structure):
                 ('logits', c_void_p), ('next_tokens', c_void_p), ('scratch', c_void_p), ('scratch_bytes', c_size_t), ('tp', ctypes.POINTER(LlamaTP))]
 
 
+class Sampling(ctypes.Structure):
+    """struct gptq_sampling (device arrays of `batch` entries)."""
+    _fields_ = [('temperature', c_void_p), ('top_k', c_void_p), ('top_p', c_void_p), ('seed', c_void_p), ('eos_token', c_void_p), ('min_length', c_void_p)]
+
+
 # name -> (restype, argtypes); must list every symbol include/gptq_b200.h declares
 SIGNATURES = {
     'gptq_abi_version': (c_int, []),
@@ -84,6 +89,7 @@ SIGNATURES = {
     'gptq_lm_head_logprob': (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'gptq_cached_attention': (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                                       c_void_p]),
+    'gptq_sample_tokens': (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, ctypes.POINTER(Sampling), c_void_p, c_void_p]),
     'gptq_ipc_alloc':(c_int, [c_size_t, ctypes.POINTER(c_void_p), ctypes.c_char_p]),
     'gptq_ipc_open': (c_int, [ctypes.c_char_p, ctypes.POINTER(c_void_p)]),
     'gptq_ipc_close': (c_int, [c_void_p]),

@@ -12,7 +12,7 @@ import math
 import torch
 
 from . import ops
-from ._lib import LlamaLayer, LlamaModel, LlamaState, LlamaTP, check, lib
+from ._lib import LlamaLayer, LlamaModel, LlamaState, LlamaTP, Sampling, check, lib
 from .ops import QLayerWeights
 
 c_void_p, c_int, c_float, c_size_t = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_size_t
@@ -142,6 +142,9 @@ class LlamaDecoder:
         self.cached_tokens = [[] for _ in range(batch)]
         self.n_launches = None
         self.graph = None
+        self._sampling = None  # the gptq_sampling struct while set_sampling is in force
+        self._sampling_arrays = self._sampling_struct = None  # its device arrays: allocated once, the sampled graph reads them in place
+        self.sample_graph = None  # the decode step followed by gptq_sample_tokens, captured on first sampled use
         self._stream = torch.cuda.Stream(self.dev)
         if use_graph:
             self._capture()
@@ -219,11 +222,73 @@ class LlamaDecoder:
         return int(lib.gptq_llama_persistent_scratch_offset(ctypes.byref(self.model), self.batch, self.max_seq))
 
     def step(self, stream=None):
-        """Run one decode step on the tokens/positions currently in device memory."""
-        if self.graph is not None:
+        """Run one decode step on the tokens/positions currently in device memory.  With set_sampling in force, next_tokens is then drawn
+        from the step's logits by gptq_sample_tokens (one more launch, in a second captured graph)."""
+        if self._sampling is not None:
+            if self.graph is None:
+                s = stream or torch.cuda.current_stream(self.dev)
+                self._enqueue(s)
+                self._enqueue_sample(s)
+                return
+            if self.sample_graph is None:
+                self._capture_sampled()
+            self.sample_graph.replay()
+        elif self.graph is not None:
             self.graph.replay()
         else:
             self._enqueue(stream or torch.cuda.current_stream(self.dev))
+
+    def set_sampling(self, temperature, top_k, top_p, seed, eos_token_id=None, min_length=0):
+        """Draw next_tokens from each step's logits from now on (gptq_sample_tokens; clear_sampling ends it).  Every argument is one value for
+        all sequences or a list of `batch`: temperature (0: greedy), top_k (0: off), top_p (1: off), seed (64-bit), eos_token_id (None: no eos)
+        and min_length (eos is suppressed while position + 1 < min_length)."""
+        if self.tp is not None:
+            raise ValueError('sampling and eos stopping are not supported under tensor parallelism')
+        t, k, p = sampling_lists(self.batch, temperature, top_k, top_p)
+        seeds = [int(v) % 2**64 for v in _per_seq(self.batch, seed, 'seed')]
+        eos = [-1 if v is None else int(v) for v in _per_seq(self.batch, eos_token_id, 'eos_token_id')]
+        if any(not -1 <= e < self.vocab for e in eos):
+            raise ValueError(f'eos_token_id outside the vocabulary (0..{self.vocab - 1})')
+        ml = [int(v) for v in _per_seq(self.batch, min_length, 'min_length')]
+        if self._sampling_struct is None:
+            with torch.cuda.device(self.dev):
+                arrs = dict(temperature=torch.zeros(self.batch, dtype=torch.float32, device=self.dev),
+                            top_k=torch.zeros(self.batch, dtype=torch.int32, device=self.dev),
+                            top_p=torch.zeros(self.batch, dtype=torch.float32, device=self.dev),
+                            seed=torch.zeros(self.batch, dtype=torch.int64, device=self.dev),
+                            eos_token=torch.zeros(self.batch, dtype=torch.int32, device=self.dev),
+                            min_length=torch.zeros(self.batch, dtype=torch.int32, device=self.dev))
+            st = Sampling(**{f: a.data_ptr() for f, a in arrs.items()})
+            self._sampling_arrays, self._sampling_struct = arrs, st
+        a = self._sampling_arrays
+        a['temperature'].copy_(torch.tensor(t, dtype=torch.float32))
+        a['top_k'].copy_(torch.tensor(k, dtype=torch.int32))
+        a['top_p'].copy_(torch.tensor(p, dtype=torch.float32))
+        a['seed'].copy_(torch.tensor([v - 2**64 if v >= 2**63 else v for v in seeds], dtype=torch.int64))  # uint64 bits
+        a['eos_token'].copy_(torch.tensor(eos, dtype=torch.int32))
+        a['min_length'].copy_(torch.tensor(ml, dtype=torch.int32))
+        self._sampling = self._sampling_struct
+
+    def clear_sampling(self):
+        """step() takes the argmax again (the decode step's own next_tokens)."""
+        self._sampling = None
+
+    def _enqueue_sample(self, stream):
+        check(lib.gptq_sample_tokens(self.logits.data_ptr(), self.vocab, self.batch, self.vocab, self.positions.data_ptr(), ctypes.byref(self._sampling),
+                                     self.next_tokens.data_ptr(), ctypes.c_void_p(stream.cuda_stream)))
+
+    def _capture_sampled(self):
+        with torch.cuda.device(self.dev):
+            torch.cuda.synchronize()
+            with torch.cuda.stream(self._stream):
+                self._enqueue_sample(self._stream)  # warm-up outside capture: reads the current logits, writes next_tokens only
+                self._stream.synchronize()
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g, stream=self._stream):
+                    self._enqueue(self._stream)
+                    self._enqueue_sample(self._stream)
+            self.sample_graph = g
+            torch.cuda.synchronize()
 
     def reset(self):
         self.positions.zero_()
@@ -408,21 +473,46 @@ class LlamaDecoder:
             if any(int(t) < 0 or int(t) >= self.vocab for t in p):
                 raise ValueError(f'prompt token id outside the vocabulary (0..{self.vocab - 1})')
 
-    def _decode(self, prompts, max_new_tokens, starts):
-        """Greedy lock-step decode: sequence b is stepped from position starts[b] (its cache holds the positions before it) until it has
-        max_new_tokens new tokens; the prompts' remaining tokens are fed first.  Every sequence takes the same number of steps."""
+    def _decode(self, prompts, max_new_tokens, starts, eos=None):
+        """Lock-step decode: sequence b is stepped from position starts[b] (its cache holds the positions before it) until it has
+        max_new_tokens new tokens or has emitted eos[b]; the prompts' remaining tokens are fed first.  The steps end when every sequence is
+        done; a finished sequence is stepped along meanwhile, and the cache rows it writes then are dropped from its record."""
         out = [[int(t) for t in p] for p in prompts]
         steps = len(prompts[0]) + max_new_tokens - 1 - starts[0]
         assert all(len(p) + max_new_tokens - 1 - s == steps for p, s in zip(prompts, starts))
+        stopped = [False] * len(prompts)
         for k in range(steps):
             pos = [s + k for s in starts]
             self.set_input([p[i] if i < len(p) else o[-1] for p, o, i in zip(prompts, out, pos)], pos)
             self.step()
             nxt = self.next_tokens.tolist()
             for b, (p, i) in enumerate(zip(prompts, pos)):
-                if i >= len(p) - 1:
+                if i >= len(p) - 1 and not stopped[b]:
                     out[b].append(nxt[b])
+                    stopped[b] = eos is not None and nxt[b] == eos[b]
+            if all(stopped):
+                break
+        for b, o in enumerate(out):
+            if stopped[b]:  # the record covers the returned tokens but the last, as for a sequence that ran to max_new_tokens
+                self.lengths[b] = len(o) - 1
+                self.cached_tokens[b] = self.cached_tokens[b][:len(o) - 1]
         return out
+
+    def _sampled_decode(self, prompts, max_new_tokens, starts, do_sample, temperature, top_k, top_p, seed, eos_token_id, min_new_tokens):
+        """_decode with gptq_sample_tokens after every step when sampling or an eos token is asked for (else exactly the greedy decode).
+        Sequence b draws with seed + b (seed None: a random 64-bit seed from torch's host RNG) and cannot emit eos before
+        min_new_tokens new tokens (min_length = len(prompt) + min_new_tokens)."""
+        if not do_sample and eos_token_id is None:
+            return self._decode(prompts, max_new_tokens, starts)
+        if seed is None:
+            seed = int(torch.randint(-2**63, 2**63 - 1, (1, ), dtype=torch.int64)) % 2**64
+        eos = [None if v is None else int(v) for v in _per_seq(self.batch, eos_token_id, 'eos_token_id')]
+        self.set_sampling(temperature if do_sample else 0.0, top_k if do_sample else 0, top_p if do_sample else 1.0,
+                          [int(seed) + b for b in range(self.batch)], eos, [len(p) + int(min_new_tokens) for p in prompts])
+        try:
+            return self._decode(prompts, max_new_tokens, starts, [-1 if e is None else e for e in eos])
+        finally:
+            self.clear_sampling()
 
     def _reuse(self, prompts, extend=True):
         """Keep what each sequence's cache shares with its prompt (reusable_prefix) and drop the rest of the record; with `extend`, append the
@@ -439,34 +529,81 @@ class LlamaDecoder:
         self.extend([p[c:len(p) - 1] for p, c in zip(prompts, keep)])
         return [len(p) - 1 for p in prompts]
 
+    def _check_sampling_args(self, do_sample, temperature, top_k, top_p, eos_token_id, min_new_tokens):
+        """Everything generate / generate_batch are given is validated before the cache or the record is touched."""
+        if (do_sample or eos_token_id is not None) and self.tp is not None:
+            raise ValueError('sampling and eos stopping are not supported under tensor parallelism')
+        if do_sample:
+            sampling_lists(self.batch, temperature, top_k, top_p)
+        if any(v is not None and not 0 <= int(v) < self.vocab for v in _per_seq(self.batch, eos_token_id, 'eos_token_id')):
+            raise ValueError(f'eos_token_id outside the vocabulary (0..{self.vocab - 1})')
+        if int(min_new_tokens) < 0:
+            raise ValueError('min_new_tokens must be >= 0')
+
     @torch.no_grad()
-    def generate(self, prompt_ids, max_new_tokens, prefill=True, reuse_cache=False):
-        """Greedy decode (batch 1).  One engine, two phases: the prompt is prefilled in one batched pass (wgmma GEMM path) into the static KV
+    def generate(self, prompt_ids, max_new_tokens, prefill=True, reuse_cache=False, do_sample=False, temperature=1.0, top_k=50, top_p=1.0, seed=None,
+                 eos_token_id=None, min_new_tokens=0):
+        """Greedy decode (batch 1), or with do_sample=True sampled as HF's model.generate samples (llama_inference.py:119-127): temperature,
+        top-k, top-p and one draw per token on the device (gptq_sample_tokens; the defaults are HF's).  seed None draws a random one; the same
+        seed gives the same tokens.  With eos_token_id, generation stops after that token (greedy or sampled; it ends the returned list), but
+        not before min_new_tokens new tokens.  One engine, two phases: the prompt is prefilled in one batched pass (wgmma GEMM path) into the static KV
         cache, then the persistent decode kernel takes over token by token; prefill=False feeds the prompt through the decode step instead.
         reuse_cache=True keeps the cached positions the prompt starts with (e.g. the conversation so far, when the prompt is that conversation
         plus a new turn) and computes only the rest (with extend(), or through the decode step with prefill=False)."""
         assert self.batch == 1
         self._check_prompts([prompt_ids], max_new_tokens)
+        self._check_sampling_args(do_sample, temperature, top_k, top_p, eos_token_id, min_new_tokens)
+        samp = (do_sample, temperature, top_k, top_p, seed, eos_token_id, min_new_tokens)
         if reuse_cache:
-            return self._decode([prompt_ids], max_new_tokens, self._reuse([prompt_ids], extend=prefill))[0]
+            return self._sampled_decode([prompt_ids], max_new_tokens, self._reuse([prompt_ids], extend=prefill), *samp)[0]
         self.reset()
         start = self.prefill(prompt_ids) if (prefill and self.tp is None) else 0
-        return self._decode([prompt_ids], max_new_tokens, [start])[0]
+        return self._sampled_decode([prompt_ids], max_new_tokens, [start], *samp)[0]
 
     @torch.no_grad()
-    def generate_batch(self, prompts, max_new_tokens, reuse_cache=False):
+    def generate_batch(self, prompts, max_new_tokens, reuse_cache=False, do_sample=False, temperature=1.0, top_k=50, top_p=1.0, seed=None,
+                       eos_token_id=None, min_new_tokens=0):
         """Greedy decode of `batch` prompts of different lengths: one ragged prefill (prefill_batch), then every sequence is stepped in
         lock-step at its own position by the decode step (the persistent kernel decodes them all in one launch).  Returns one token list per
         prompt: the prompt followed by its max_new_tokens generated tokens.
         reuse_cache=True: sequence b keeps the longest prefix its cache shares with prompt b (at most len(prompt) - 1 positions) and only the
         rest of the prompt but its last token goes through one ragged extend() pass, so a second turn -- the previous output plus the new
-        turn -- costs the new turn only.  The result is that of reuse_cache=False up to fp rounding."""
+        turn -- costs the new turn only.  The result is that of reuse_cache=False up to fp rounding.
+        do_sample, temperature, top_k, top_p, seed, eos_token_id, min_new_tokens: as in generate; the sampling parameters may be lists of one
+        value per sequence, and sequence b draws with seed + b, so row b is comparable with a batch-1 run seeded seed + b.  A sequence that
+        emits eos stops (its list ends with it) while the others go on; afterwards each sequence's record (lengths, cached_tokens) covers its
+        returned tokens but the last, so a following reuse_cache=True turn extends from there."""
         self._check_prompts(prompts, max_new_tokens)
+        self._check_sampling_args(do_sample, temperature, top_k, top_p, eos_token_id, min_new_tokens)
+        samp = (do_sample, temperature, top_k, top_p, seed, eos_token_id, min_new_tokens)
         if reuse_cache:
-            return self._decode(prompts, max_new_tokens, self._reuse(prompts))
+            return self._sampled_decode(prompts, max_new_tokens, self._reuse(prompts), *samp)
         self.reset()
         starts = self.prefill_batch(prompts)
-        return self._decode(prompts, max_new_tokens, starts)
+        return self._sampled_decode(prompts, max_new_tokens, starts, *samp)
+
+
+def _per_seq(batch, v, name):
+    """One value per sequence: a list of `batch` values, or one value for all."""
+    vals = list(v) if isinstance(v, (list, tuple)) else [v] * batch
+    if len(vals) != batch:
+        raise ValueError(f'{name}: expected one value or {batch}, got {len(vals)}')
+    return vals
+
+
+def sampling_lists(batch, temperature, top_k, top_p):
+    """Per-sequence temperature, top_k and top_p, checked as HF checks its warpers: temperature >= 0 (0: greedy), top_k >= 0 (0: off),
+    0 < top_p <= 1 (1: off)."""
+    t = [float(v) for v in _per_seq(batch, temperature, 'temperature')]
+    k = [int(v) for v in _per_seq(batch, top_k, 'top_k')]
+    p = [float(v) for v in _per_seq(batch, top_p, 'top_p')]
+    if any(not (v >= 0 and math.isfinite(v)) for v in t):
+        raise ValueError(f'temperature must be a finite value >= 0 (0: greedy), got {temperature}')
+    if any(v < 0 for v in k):
+        raise ValueError(f'top_k must be >= 0 (0: off), got {top_k}')
+    if any(not 0 < v <= 1 for v in p):
+        raise ValueError(f'top_p must be in (0, 1], got {top_p}')
+    return t, k, p
 
 
 def reusable_prefix(prompt, cached):

@@ -6,6 +6,7 @@ rotate_half_                     <- triton_rotate_half_, quant/fused_attn.py:61-
 rmsnorm                          <- TritonLlamaRMSNorm.forward, quant/triton_norm.py:50-67
 lm_head_logprob                  <- lm_head + shifted CrossEntropyLoss of llama_eval, llama.py:246-256 (per-token, fp32)
 cached_attention                 <- causal SDPA of new rows over a sequence's cached prefix (the engine's extend path; no reference counterpart)
+sample_tokens                    <- HF's temperature / top-k / top-p warpers + torch.multinomial of model.generate(do_sample=True), llama_inference.py:119-127
 
 torch is plumbing here (device memory, current stream); all arithmetic happens in libgptq_b200.so.
 """
@@ -232,6 +233,33 @@ def cached_attention(q, k_cache, v_cache, spans):
         check(
             lib.gptq_cached_attention(q.data_ptr(), q.stride(0) if M > 1 else nh * hd, k_cache.data_ptr(), v_cache.data_ptr(), B, nh, hd, S, len(spans), arr(0),
                                       arr(1), arr(2), out.data_ptr(), nh * hd, _stream(q)))
+    return out
+
+
+def sample_tokens(logits, positions, temperature, top_k, top_p, seed, eos_token=None, min_length=None, out=None):
+    """int32 [B]: one token per row of the fp16 logits [B, V] (gptq_sample_tokens, the rule in include/gptq_b200.h).  positions int32 [B] are
+    the rows' decode positions (the draw's counter); the parameters are device tensors of B entries -- temperature / top_p float32, top_k /
+    eos_token / min_length int32, seed int64 (read as uint64) -- eos_token None: no eos."""
+    _require_cuda(logits, positions, temperature, top_k, top_p, seed, eos_token, min_length, out)
+    if logits.dim() != 2 or logits.dtype != torch.float16 or logits.stride(1) != 1:
+        raise ValueError('sample_tokens expects fp16 logits [B, V] with unit column stride')
+    B, V = logits.shape
+    dev = logits.device
+    if eos_token is None:
+        eos_token = torch.full((B, ), -1, dtype=torch.int32, device=dev)
+    if min_length is None:
+        min_length = torch.zeros(B, dtype=torch.int32, device=dev)
+    want = dict(positions=(positions, torch.int32), temperature=(temperature, torch.float32), top_k=(top_k, torch.int32), top_p=(top_p, torch.float32),
+                seed=(seed, torch.int64), eos_token=(eos_token, torch.int32), min_length=(min_length, torch.int32))
+    for name, (t, dt) in want.items():
+        if t.dtype != dt or t.numel() != B or not t.is_contiguous():
+            raise ValueError(f'{name}: expected a contiguous {dt} tensor of {B} entries')
+    out = torch.empty(B, dtype=torch.int32, device=dev) if out is None else out
+    prm = _lib.Sampling(temperature=temperature.data_ptr(), top_k=top_k.data_ptr(), top_p=top_p.data_ptr(), seed=seed.data_ptr(),
+                        eos_token=eos_token.data_ptr(), min_length=min_length.data_ptr())
+    with torch.cuda.device(dev):
+        check(lib.gptq_sample_tokens(logits.data_ptr(), logits.stride(0) if B > 1 else V, B, V, positions.data_ptr(), ctypes.byref(prm), out.data_ptr(),
+                                     _stream(logits)))
     return out
 
 

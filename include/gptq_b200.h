@@ -39,8 +39,8 @@ extern "C" {
 
 #define GPTQ_B200_ABI_VERSION 6 /* 2: act-order input gathers; 3: gptq_llama_persistent_scratch_offset; 4: tensor parallelism (gptq_llama_tp, gptq_ipc_*);
                                    5: persistent path at batch 2..8 ([batch][hidden] residual rows in the persistent region);
-                                   6: gptq_lm_head_logprob (scoring); gptq_cached_attention added later without a change to any
-                                   existing struct or signature */
+                                   6: gptq_lm_head_logprob (scoring); gptq_cached_attention and gptq_sample_tokens added later without a
+                                   change to any existing struct or signature */
 
 typedef void* gptq_stream_t; /* cudaStream_t */
 
@@ -223,6 +223,41 @@ int gptq_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw,
 int gptq_cached_attention(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int head_dim, int max_seq,
                           int n_spans, const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
                           gptq_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Sampling (model.generate(do_sample=True, ...) of llama_inference.py:119-127, with HF's warpers in HF's order): one token per row of the
+ * fp16 logits a decode step leaves in gptq_llama_state.logits, written to next_tokens[b].  A launch of its own after the step, so one kernel
+ * serves both decode engines.  Every gptq_sampling field is a DEVICE array of `batch` entries (read when the kernel runs, so a CUDA graph
+ * can replay the call with new values).  For row b, with l the fp16 logits, p = positions[b] (the step's position):
+ *   1. eos: if 0 <= eos_token[b] < vocab and p + 1 < min_length[b] (HF MinLengthLogitsProcessor: cur_len = p + 1), l[eos] = -inf.
+ *      NaN counts as -inf.
+ *   2. temperature[b] <= 0 (or NaN): the argmax, lowest id on ties (the decode step's next_tokens, with eos excluded while suppressed).
+ *      Otherwise z_v = fp32(float(l_v) / T), the correctly rounded fp32 division (HF TemperatureLogitsWarper on logits.float()).
+ *   3. top-k (0 < top_k[b] < vocab, else off): keep v iff z_v >= z_(k), the k-th largest z counted with multiplicity (HF TopKLogitsWarper).
+ *   4. weights over the top-k set: w_v = exp((double)z_v - (double)z_max) in fp64; if some z is +inf, those entries weigh 1 and all others 0.
+ *   5. top-p (top_p[b] < 1, else off): keep v iff (weight of top-k tokens with z_u > z_v) / (top-k weight) < top_p.  For distinct values this
+ *      is HF's TopPLogitsWarper (cumsum <= 1 - top_p removed); a tie group straddling the boundary is kept whole, where HF keeps the part
+ *      torch.sort happens to put first.  The largest z is always kept.
+ *   6. draw: (x0, x1, x2, x3) = Philox4x32-10(counter (p, 0, 0, 0), key (seed lo 32 bits, seed hi 32 bits)),
+ *      u = ((x0 >> 5) * 2^26 + (x1 >> 6)) * 2^-53; the token is the first kept id, ascending, whose inclusive fp64 running weight exceeds
+ *      u * W (W: the kept weight); if rounding leaves none, the last kept id.
+ *   7. a row with nothing above -inf gives 0.
+ * The token depends only on the row's logits, its parameters and its position: no float atomics, every float sum in a fixed order.  The
+ * counter is the position, so a re-run or resumed sequence draws the same u at the same position.  Running weights are summed per block of
+ * ids and then over the blocks, so they can differ from a sequential sum in the last bits: a draw whose u * W lies that close to a
+ * cumulative boundary may take the neighbouring token.
+ * batch 1..8, vocab >= 1, ld >= vocab (GPTQ_ERR_SHAPE); vocab > 131072 gives GPTQ_ERR_UNSUPPORTED; logits 2-byte, seed 8-byte and the other
+ * arrays 4-byte aligned.  No workspace. */
+typedef struct gptq_sampling {
+    const float* temperature;
+    const int32_t* top_k;
+    const float* top_p;
+    const uint64_t* seed;
+    const int32_t* eos_token;  /* < 0: none */
+    const int32_t* min_length;
+} gptq_sampling;
+int gptq_sample_tokens(const void* logits, int64_t ld, int batch, int vocab, const int32_t* positions, const gptq_sampling* params,
+                       int32_t* next_tokens, gptq_stream_t stream);
 
 /* Device memory that other processes of the node can map (CUDA IPC), for the tensor-parallel scratch / logits buffers:
  * alloc returns a zero-filled device buffer and its 64-byte handle (to be sent to the peers, e.g. with torch.distributed);
