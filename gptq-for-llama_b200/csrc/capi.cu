@@ -105,6 +105,8 @@ int gptq_qlinear_transpose_fwd(const void* g, int64_t ldg, const gptq_qweight* w
     if (g == nullptr || out == nullptr) return GPTQ_ERR_NULL;
     if (M < 0 || ldg < w->N || ldo < w->K) return GPTQ_ERR_SHAPE;
     if (M == 0) return GPTQ_OK;
+    if (gemm_t_tc_supported(g, ldg, *w, out, ldo, M))
+        return cuda_status(launch_qlinear_transpose_tc(g, ldg, *w, out, ldo, M, static_cast<cudaStream_t>(stream)));
     return cuda_status(launch_qlinear_transpose_generic(g, ldg, *w, out, ldo, M, static_cast<cudaStream_t>(stream)));
 }
 

@@ -51,6 +51,10 @@ cudaError_t launch_qlinear_skinny(const QLinearArgs& a, bool pdl);
 bool gemm_tc_supported(const QLinearArgs& a);
 cudaError_t launch_qlinear_gemm_tc(const QLinearArgs& a);
 
+// qgemm_wgmma_t.cu -- transposed int4 GEMM on wgmma (the gradient w.r.t. a quantized linear's input), M > 8
+bool gemm_t_tc_supported(const void* g, int64_t ldg, const gptq_qweight& w, const void* out, int64_t ldo, int M);
+cudaError_t launch_qlinear_transpose_tc(const void* g, int64_t ldg, const gptq_qweight& w, void* out, int64_t ldo, int M, cudaStream_t stream);
+
 // lm_head_logprob.cu -- per-row log-probability of a target through the fp16 lm_head (wgmma + fused log-softmax), and its combine pass
 size_t lm_head_logprob_workspace_bytes(int M, int V);
 cudaError_t launch_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int K, int V, const int32_t* targets, float* logprob,

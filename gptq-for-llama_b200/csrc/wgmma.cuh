@@ -1,6 +1,6 @@
-// Hopper tensor-core helpers shared by the wgmma kernels (qgemm_wgmma.cu, lm_head_logprob.cu, cached_attention.cu): shared-memory matrix
-// descriptors, the wgmma fence / commit / wait protocol, the m64n128k16 f16 MMAs (both operands in shared memory; A in registers with a
-// transposed B), and the TMA tensor map of a K-major fp16 matrix with its box load.
+// Hopper tensor-core helpers shared by the wgmma kernels (qgemm_wgmma.cu, qgemm_wgmma_t.cu, lm_head_logprob.cu, cached_attention.cu):
+// shared-memory matrix descriptors, the wgmma fence / commit / wait protocol, the m64n128k16 f16 MMAs (both operands in shared memory, B
+// K-major or transposed; A in registers with a transposed B), and the TMA tensor map of a K-major fp16 matrix with its box load.
 #pragma once
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -56,6 +56,27 @@ __device__ __forceinline__ uint64_t smem_desc_mn(uint32_t saddr, uint32_t lbo) {
     return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 
+// D[64 x 128] += A[64 x 16] . B[16 x 128], both operands in shared memory: A K-major (smem_desc), B MN-major (smem_desc_mn, transposed)
+__device__ __forceinline__ void wgmma_m64n128k16_tn(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, "
+        "%30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, "
+        "%58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+          "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+          "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(1));
+}
+
 // D[64 x 128] += A[64 x 16] . B[16 x 128], A from registers (four f16x2 per thread, the layout of an m64nNk16 accumulator fragment:
 // a[0] = row r cols c, c+1; a[1] = row r+8; a[2] = cols c+8, c+9; a[3] = row r+8, cols c+8, c+9), B MN-major in shared memory (transposed)
 __device__ __forceinline__ void wgmma_m64n128k16_rs_tn(float (&d)[64], const uint32_t (&a)[4], uint64_t db) {
@@ -100,8 +121,13 @@ inline bool make_kmajor_tensor_map(CUtensorMap* tm, const void* base, int rows, 
     const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};            // bytes between rows
     const cuuint32_t box[2] = {(cuuint32_t)kWgmmaBK, 128};         // 64 halves (128 B) x 128 rows
     const cuuint32_t estr[2] = {1, 1};
-    return encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    auto go = [&] {
+        return encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    };
+    // The encode is a driver call and needs a context current on the calling thread.  A host thread whose first CUDA work is this launch
+    // (an autograd worker running a backward) has none until a runtime call binds the primary context: bind it and try once more.
+    return go() || (cudaFree(nullptr) == cudaSuccess && go());
 }
 
 }  // namespace gptq

@@ -87,7 +87,12 @@ int gptq_qlinear_fwd(const void* x, int64_t ldx, const gptq_qweight* w, const vo
 int gptq_fused_mlp_fwd(const void* x, int64_t ldx, const gptq_qweight* gate, const gptq_qweight* up, void* out, int64_t ldo, int M, void* workspace,
                        size_t ws_bytes, gptq_stream_t stream);
 
-/* grad_in[M,K] = g[M,N] . deq(W)^T.  Replaces transpose_matmul248 (quant/quant_linear.py:272-279, :191-258). */
+/* grad_in[M,K] = g[M,N] . deq(W)^T.  Replaces transpose_matmul248 (quant/quant_linear.py:272-279, :191-258).
+ * Arithmetic on every route: each weight is dequantised as in the forward, fp16((q - z) * s); products accumulate in fp32; one fp16
+ * rounding at the store.  No atomics and no workspace: a row of the result depends on its own row of g only and repeats bit for bit.
+ * Routing: the wgmma kernel (tensor cores) serves bits == 4 with groupsize > 0 and a multiple of 32, M > 8, K % 128 == 0, N % 64 == 0,
+ * g and out 16-byte aligned with ldg % 8 == 0 and ldo % 8 == 0; every other request goes to the generic CUDA-core kernel (any bits,
+ * any g_idx, any M).  Act-order and 2/3-bit layers reach the wgmma kernel through their kernel form (regrouped rows, widened fields). */
 int gptq_qlinear_transpose_fwd(const void* g, int64_t ldg, const gptq_qweight* w, void* out, int64_t ldo, int M, gptq_stream_t stream);
 
 /* In-place rotary embedding on q and k.  Replaces triton_rotate_half_ / rotate_half_kernel
