@@ -56,9 +56,12 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) __nanosleep(200);
 }
-// `bytes` (multiple of 16) contiguous bytes global -> shared; completion is signalled on `bar` (complete_tx)
-__device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+// `bytes` (multiple of 16) contiguous bytes global -> shared; completion is signalled on `bar` (complete_tx); `policy`: L2 cache policy
+// (createpolicy) of the lines read
+__device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t policy) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst), "l"(src), "r"(bytes),
+                 "r"(bar), "l"(policy)
+                 : "memory");
 }
 
 __device__ __forceinline__ float ld_cg(const float* p) {

@@ -26,7 +26,8 @@ for l in range(1, 3):
     for k in range(12):
         c = (t[:, l * 12 + k] - t0) / 1e3
         print(f'  {names[k]:24s} {c.min().item():8.2f} {c.median().item():8.2f} {c.max().item():8.2f}')
-    print(f'  layer total {((t[:, (l + 1) * 12] - t[:, l * 12]) / 1e3).median().item():.2f} us')
+    if (l + 1) * 12 < 36:  # only ids below 36 are recorded: the next layer's start is known for layer 1 alone
+        print(f'  layer total {((t[:, (l + 1) * 12] - t[:, l * 12]) / 1e3).median().item():.2f} us')
 print('layer 2, team 0 of every CTA (median over CTAs): cycles in op / waiting for stages / stages / busy cycles per stage')
 for i, name in enumerate(['Q', 'A', 'O', 'G', 'D']):
     tot, wait, st = t[:, 48 + 3 * i], t[:, 49 + 3 * i], t[:, 50 + 3 * i]
