@@ -700,6 +700,9 @@ def from_hf_quant_model(model, batch=1, max_seq=2048, **kw):
     repo's quant package (make_quant_linear -> load_state_dict -> make_quant_attn / make_quant_norm / make_fused_mlp)."""
     import quant
     L = []
+    rope_bases = {layer.self_attn.rope_base for layer in model.model.layers if isinstance(layer.self_attn, quant.QuantLlamaAttention)}
+    if len(rope_bases) > 1:
+        raise ValueError(f'the attention layers disagree on the RoPE base: {sorted(rope_bases)}')
     for layer in model.model.layers:
         attn, mlp = layer.self_attn, layer.mlp
         if not isinstance(attn, quant.QuantLlamaAttention):
@@ -710,4 +713,4 @@ def from_hf_quant_model(model, batch=1, max_seq=2048, **kw):
                  input_norm=layer.input_layernorm.weight.data.half().contiguous(), post_norm=layer.post_attention_layernorm.weight.data.half().contiguous()))
     cfg = model.config
     return LlamaDecoder(L, model.model.embed_tokens.weight.data.half(), model.model.norm.weight.data.half().contiguous(), model.lm_head.weight.data.half(),
-                        cfg.num_attention_heads, rms_eps=cfg.rms_norm_eps, rope_base=getattr(cfg, 'rope_theta', 10000.0) or 10000.0, batch=batch, max_seq=max_seq, **kw)
+                        cfg.num_attention_heads, rms_eps=cfg.rms_norm_eps, rope_base=rope_bases.pop(), batch=batch, max_seq=max_seq, **kw)

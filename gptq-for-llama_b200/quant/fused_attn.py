@@ -25,15 +25,32 @@ def triton_rotate_half_(qk, position_ids, config=None):
     ops.rotate_half_(qk, position_ids)
 
 
+def rope_base_from_config(config):
+    """The RoPE base (theta) an HF LLaMA config asks for: rope_parameters['rope_theta'] (transformers >= 5), else rope_theta
+    (transformers 4.31 - 4.x), else 10000.  The kernels rotate by theta^(-2i/d) * pos on integer positions only, so a config
+    whose rope type is anything but 'default' (linear, dynamic, yarn, llama3, ...) raises ValueError instead of decoding
+    as if it were unscaled."""
+    params = getattr(config, 'rope_parameters', None)
+    if params is None:  # transformers 4.x: rope_theta beside an optional rope_scaling dict ('type' before 4.45, 'rope_type' after)
+        scaling = getattr(config, 'rope_scaling', None) or {}
+        params = {'rope_theta': getattr(config, 'rope_theta', None), 'rope_type': scaling.get('rope_type', scaling.get('type', 'default'))}
+    rope_type = params.get('rope_type', 'default')
+    if rope_type != 'default':
+        raise ValueError(f"RoPE type {rope_type!r} is not supported: only 'default' (unscaled) rotary embeddings are computed")
+    base = params.get('rope_theta')
+    return 10000.0 if base is None else float(base)
+
+
 class QuantLlamaAttention(nn.Module):
     """Multi-headed attention from 'Attention Is All You Need' paper"""
 
-    def __init__(self, hidden_size, num_heads, qkv_proj, o_proj, layer_idx=None):
+    def __init__(self, hidden_size, num_heads, qkv_proj, o_proj, layer_idx=None, rope_base=10000.0):
         super().__init__()
         self.hidden_size = hidden_size
         self.num_heads = num_heads
         self.head_dim = hidden_size // num_heads
         self.layer_idx = layer_idx
+        self.rope_base = float(rope_base)
         if (self.head_dim * num_heads) != self.hidden_size:
             raise ValueError(f"hidden_size must be divisible by num_heads (got `hidden_size`: {self.hidden_size}"
                              f" and `num_heads`: {num_heads}).")
@@ -58,7 +75,7 @@ class QuantLlamaAttention(nn.Module):
 
         qkv_states = self.qkv_proj(hidden_states)
         qkv_states = qkv_states.view(bsz, q_len, 3, self.num_heads, self.head_dim)
-        triton_rotate_half_(qkv_states[:, :, :2], position_ids)  # q and k rotated in place (:126)
+        ops.rotate_half_(qkv_states[:, :, :2], position_ids, base=self.rope_base)  # q and k rotated in place (:126)
 
         query_states, key_states, value_states = (t.squeeze(2).transpose(1, 2) for t in torch.split(qkv_states, 1, dim=2))
         del qkv_states
@@ -127,9 +144,10 @@ def make_quant_attn(model):
         kv_heads = getattr(m, 'num_key_value_heads', None) or getattr(cfg, 'num_key_value_heads', num_heads) or num_heads
         if kv_heads != num_heads:
             raise ValueError('fused QKV attention requires num_key_value_heads == num_attention_heads (LLaMA-1 style MHA)')
+        rope_base = rope_base_from_config(cfg if cfg is not None else model.config)
         qkv_layer = fuse_qkv(m.q_proj, m.k_proj, m.v_proj)
-        # the rotary embedding module is dropped: RoPE is computed in the kernel from position_ids
-        attn = QuantLlamaAttention(hidden_size, num_heads, qkv_layer, m.o_proj, layer_idx=getattr(m, 'layer_idx', None))
+        # the rotary embedding module is dropped: RoPE is computed in the kernel from position_ids and the config's base
+        attn = QuantLlamaAttention(hidden_size, num_heads, qkv_layer, m.o_proj, layer_idx=getattr(m, 'layer_idx', None), rope_base=rope_base)
         parent_name, _, child_name = name.rpartition('.')
         parent = model.get_submodule(parent_name) if parent_name else model
         setattr(parent, child_name, attn)

@@ -113,7 +113,7 @@ class Probe:
     kernel's rotated q) and V rows; run() is pass 2: it plants the cache, poisons the rows at and after each position with NaN, steps, checks
     that the appended rows are bit-identical to pass 1 and returns (x_in, x_out) [B, H] fp16."""
 
-    def __init__(self, size, batch=1, max_seq=2048, act_order=False, vocab=64, seed=0, lm_head=None):
+    def __init__(self, size, batch=1, max_seq=2048, act_order=False, vocab=64, seed=0, lm_head=None, rope_base=10000.0):
         from gptq_b200 import engine
         H, I, _, nh = engine.LLAMA_SHAPES[size]
         dev = torch.device('cuda:0')
@@ -128,8 +128,8 @@ class Probe:
         if lm_head is None:
             lm_head = (torch.randn(vocab, H, generator=torch.Generator().manual_seed(seed + 2)) * 0.02).half()
         self.dec = engine.LlamaDecoder([L], embed, torch.ones(H, dtype=torch.float16, device=dev), lm_head.to(dev), nh, rms_eps=0.0, batch=batch,
-                                       max_seq=max_seq)
-        self.H, self.nh, self.B, self.max_seq = H, nh, batch, max_seq
+                                       max_seq=max_seq, rope_base=rope_base)
+        self.H, self.nh, self.B, self.max_seq, self.rope_base = H, nh, batch, max_seq, rope_base
         self.persistent = self.dec.launches_per_step() == 1
         self.nb = 2 * torch.cuda.get_device_properties(dev).multi_processor_count
         self.q_rot = self.v_new = None
@@ -377,11 +377,12 @@ def emulate_persistent(q, K, V, ranges):
 
 
 # ----------------------------------------------------------------------------- RoPE of the appended K row
-def check_rope_row(k_row, q_exact, pos):
-    """The appended K row [nh, 128] (fp16) against fp64 RoPE of the exact q / k [H], the angle computed in fp32 as the reference formula does
-    (quant/fused_attn.py:43): within 1 ulp16, plus a 4-ulp difference in the fp32 angle and in cos / sin.  Returns the worst |err| / bound."""
+def check_rope_row(k_row, q_exact, pos, rope_base):
+    """The appended K row [nh, 128] (fp16) against fp64 RoPE of the exact q / k [H] at base rope_base, the angle computed in fp32 as the
+    reference formula does (quant/fused_attn.py:43): within 1 ulp16, plus a 4-ulp difference in the fp32 angle and in cos / sin.  Returns the
+    worst |err| / bound."""
     f = np.float32
-    inv_base = f(-2.0 * math.log(10000.0) / HD)
+    inv_base = f(-2.0 * math.log(rope_base) / HD)
     th = (np.exp(np.arange(64, dtype=f) * inv_base).astype(f) * f(pos)).astype(np.float64)
     x = q_exact.view(-1, HD)[:, :64].numpy()
     y = q_exact.view(-1, HD)[:, 64:].numpy()

@@ -9,7 +9,7 @@ REL_TOL = 1e-3  # north_star: outputs within 1e-3 relative of the reference's de
 
 
 def assert_rel_close(out: torch.Tensor, ref: torch.Tensor, rel: float = REL_TOL, what: str = ''):
-    """|out - ref| <= rel * max(|ref|, rms(ref)) element-wise.
+    """|out - ref| <= rel * max(|ref|, rms(ref)) element-wise; prints the worst |err| / bound (visible under -s).
 
     fp16 results that differ only by the fp32 summation order sit within one fp16 ulp (<= 9.8e-4 relative);
     the rms floor covers outputs that cancel to ~0, where a relative bound is meaningless."""
@@ -19,6 +19,7 @@ def assert_rel_close(out: torch.Tensor, ref: torch.Tensor, rel: float = REL_TOL,
     rms = ref32.pow(2).mean().sqrt().item()
     bound = rel * torch.maximum(ref32.abs(), torch.full_like(ref32, rms)) + 1e-7
     err = (out32 - ref32).abs()
+    print(f'  {what}: worst |err| / bound = {(err / bound).max().item():.3g} (bound {rel:g})')
     bad = err > bound
     assert not bad.any(), f'{what}: {int(bad.sum())} / {bad.numel()} elements off; max err {err.max().item():.3e}, rms(ref) {rms:.3e}'
 

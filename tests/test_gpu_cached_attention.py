@@ -16,7 +16,7 @@ pytestmark = pytest.mark.gpu
 
 U = 2.0**-24
 HD = 128
-STARTS = (0, 1, 63, 64, 65, 127, 128, 129, 1000, None)  # None: max_seq - rows
+STARTS = (0, 1, 63, 64, 65, 127, 128, 129, 1000, 2047, 2048, 4095, None)  # None: max_seq - rows
 ROWS = (1, 2, 63, 64, 65, 127, 128, 129, 300)
 
 
@@ -105,9 +105,9 @@ def run(q, kc, vc, spans, layer=1):
 
 @pytest.mark.parametrize('rows', ROWS)
 def test_against_fp64_softmax_at_every_edge(rows):
-    """Every start of STARTS with `rows` query rows, one span per sequence (8 per call, the last call partly filled); every cache row outside
-    the spans' reach is NaN."""
-    S, nh = 1300, 2
+    """Every start of STARTS with `rows` query rows, one span per sequence (8 per call, the last call partly filled), on a cache of CodeLlama's
+    16384 positions; every cache row outside the spans' reach is NaN."""
+    S, nh = 16384, 2
     starts = [S - rows if s is None else s for s in STARTS]
     worst = 0.0
     for c in range(0, len(starts), 8):

@@ -90,7 +90,7 @@ def sweep(probe, position_sets, profiles, gen, worst, rope, tok0=0, rotate_heavy
         probe.learn(toks, positions)
         for b, p in enumerate(positions):  # the appended K row (= q_rot) against fp64 RoPE of the exact q
             q_exact = P.exact_qv(probe.w, probe.dec.embed[toks[b]])[0]
-            rope.update(P.check_rope_row(probe.q_rot[b], q_exact, p), f'{what} seq {b}')
+            rope.update(P.check_rope_row(probe.q_rot[b], q_exact, p, probe.rope_base), f'{what} seq {b}')
         anchors(probe, toks, positions, gen, what)
         for kind in profiles:
             if kind == 'heavy':
@@ -156,6 +156,24 @@ def test_persistent_7b_positions():
     run_sweeps(probe, '7b', [[p] for p in positions], full_rotation=(2047, ))
 
 
+def test_persistent_7b_llama2_context():
+    """LLaMA-2-7B context (max_seq 4096): the unit, split and team edges, both sides of 2048 and the last position 4095."""
+    probe = P.Probe('7b', max_seq=4096)
+    assert probe.persistent
+    edges = {0, 1, 31, 32, 33, 255, 256, 257, 1023, 1024, 2047, 2048, 2049, 4063, 4064, 4094, 4095}
+    positions = sorted(edges | set(P.team_edge_positions(probe.nh, probe.nb)))
+    run_sweeps(probe, '7b max_seq 4096', [[p] for p in positions])
+
+
+def test_persistent_7b_codellama_context():
+    """CodeLlama-7B context (max_seq 16384, RoPE base 1e6): the team edges, both sides of 8192 and the last position 16383, where the 512
+    units of a head are split over 8 or 9 teams and every key is heavy once; the appended K row against fp64 RoPE at base 1e6."""
+    probe = P.Probe('7b', max_seq=16384, rope_base=1e6)
+    assert probe.persistent
+    positions = sorted({0, 1, 8191, 8192, 16383} | set(P.team_edge_positions(probe.nh, probe.nb)))
+    run_sweeps(probe, '7b max_seq 16384 base 1e6', [[p] for p in positions], full_rotation=(16383, ))
+
+
 def test_persistent_7b_last_unit_past_the_slot():
     """max_seq 2000: the last 32-key unit of a head at pos 1999 reaches past the end of the head's slot (only 16 rows are fetched)."""
     probe = P.Probe('7b', max_seq=2000)
@@ -172,17 +190,18 @@ def test_persistent_13b_act_order():
 
 
 # ----------------------------------------------------------------------------- batches
-@pytest.mark.parametrize('batch,position_sets', [
-    (2, [[2047, 1], [0, 0], [300, 2000]]),
-    (3, [[2047, 3, 500], [0, 0, 0], [31, 32, 33]]),
-    (8, [[0, 31, 32, 255, 256, 1023, 2046, 2047], [0] * 8, [2047, 0, 0, 0, 0, 0, 0, 5]]),
+@pytest.mark.parametrize('batch,position_sets,max_seq', [
+    pytest.param(2, [[2047, 1], [0, 0], [300, 2000]], 2048, id='2-position_sets0'),
+    pytest.param(3, [[2047, 3, 500], [0, 0, 0], [31, 32, 33]], 2048, id='3-position_sets1'),
+    pytest.param(8, [[0, 31, 32, 255, 256, 1023, 2046, 2047], [0] * 8, [2047, 0, 0, 0, 0, 0, 0, 5]], 2048, id='8-position_sets2'),
+    pytest.param(8, [[4095, 0, 2047, 2048, 31, 32, 1024, 4094], [0] * 8, [4095, 0, 0, 0, 0, 0, 0, 2048]], 4096, id='8-max_seq4096'),
 ])
-def test_persistent_7b_batched(batch, position_sets):
+def test_persistent_7b_batched(batch, position_sets, max_seq):
     """Batched persistent kernel at 7B: ragged positions (seq_teams gives each sequence a share of the teams in proportion to its
-    context), one long and one short sequence, everything at pos 0; stage_range_batch merges the records."""
-    probe = P.Probe('7b', batch=batch, max_seq=2048)
+    context), one long and one short sequence, everything at pos 0; stage_range_batch merges the records.  Also at the LLaMA-2 context."""
+    probe = P.Probe('7b', batch=batch, max_seq=max_seq)
     assert probe.persistent
-    run_sweeps(probe, f'7b batch {batch}', position_sets)
+    run_sweeps(probe, f'7b batch {batch} max_seq {max_seq}', position_sets)
 
 
 @pytest.mark.parametrize('batch,position_sets', [(2, [[599, 0], [300, 301], [37, 599], [0, 0]]), (3, [[599, 1, 256], [0, 0, 0]])])
@@ -205,6 +224,21 @@ def test_chain_13b_batch7():
     probe = P.Probe('13b', batch=7, max_seq=1024)
     assert not probe.persistent and probe.dec.launches_per_step() > 1
     run_sweeps(probe, 'chain 13b batch 7', [[0, 1, 255, 256, 511, 800, 1023], [1023, 0, 1, 2, 3, 4, 256]])
+
+
+def test_chain_13b_batch7_llama2_context():
+    """The kernel chain at LLaMA-2-13B's context (max_seq 4096: 16 splits of 256 keys per head)."""
+    probe = P.Probe('13b', batch=7, max_seq=4096)
+    assert not probe.persistent and probe.dec.launches_per_step() > 1
+    run_sweeps(probe, 'chain 13b batch 7 max_seq 4096', [[4095, 0, 1, 2047, 2048, 3839, 3840], [0, 4095, 256, 4094, 1, 2, 3]])
+
+
+def test_chain_tiny_codellama_context():
+    """The kernel chain at CodeLlama's context and RoPE base (max_seq 16384, base 1e6): 64 splits, so the combine reads 64 partials."""
+    probe = P.Probe('tiny', max_seq=16384, rope_base=1e6)
+    assert not probe.persistent and probe.dec.launches_per_step() > 1
+    run_sweeps(probe, 'chain tiny max_seq 16384 base 1e6', [[p] for p in (0, 1, 255, 256, 4095, 8191, 8192, 16127, 16128, 16382, 16383)],
+               full_rotation=(16383, ))
 
 
 # ----------------------------------------------------------------------------- the 65B and 33B shapes

@@ -5,12 +5,14 @@ import torch
 
 from oracle import gptq_oracle as O
 from gpu_util import assert_rel_close
+from test_gpu_modules import CODELLAMA, LLAMA1, scale_down_embedding_row
 
 pytestmark = pytest.mark.gpu
 
 
-def _oracle_decode(dec, token_ids):
-    """Reference: same math as the reference's decoder layer over its kernels, evaluated with the oracle on the CPU."""
+def _oracle_decode(dec, token_ids, eps=1e-6, base=10000.0):
+    """Reference: same math as the reference's decoder layer over its kernels, evaluated with the oracle on the CPU, at the RMSNorm epsilon
+    and RoPE base the caller chose (never the decoder's own settings: a decoder built with the wrong ones would agree with itself)."""
     H, nh = dec.hidden, dec.n_heads
     hd = H // nh
     cpu = lambda t: t.detach().cpu()
@@ -26,8 +28,8 @@ def _oracle_decode(dec, token_ids):
         x = embed[tok][None, :].clone()
         for li, ly in enumerate(layers):
             (w, bits) = ly['qkv']
-            qkv = O.qlinear_fwd(O.rmsnorm_fwd(x, ly['input_norm'], 1e-6), *w, bits).view(1, 1, 3, nh, hd).clone()
-            O.rope_inplace(qkv[:, :, :2], torch.tensor([[pos]]))
+            qkv = O.qlinear_fwd(O.rmsnorm_fwd(x, ly['input_norm'], eps), *w, bits).view(1, 1, 3, nh, hd).clone()
+            O.rope_inplace(qkv[:, :, :2], torch.tensor([[pos]]), base=base)
             q, k, v = qkv[0, 0, 0], qkv[0, 0, 1], qkv[0, 0, 2]
             kc[li].append(k.clone())
             vc[li].append(v.clone())
@@ -39,20 +41,29 @@ def _oracle_decode(dec, token_ids):
             (w, bits) = ly['o']
             x = x + O.qlinear_fwd(att, *w, bits)
             (wg, bits), (wu, _) = ly['gate'], ly['up']
-            hmid = O.fused_mlp_fwd(O.rmsnorm_fwd(x, ly['post_norm'], 1e-6), wg, wu, bits)
+            hmid = O.fused_mlp_fwd(O.rmsnorm_fwd(x, ly['post_norm'], eps), wg, wu, bits)
             (w, bits) = ly['down']
             x = x + O.qlinear_fwd(hmid, *w, bits)
-        xn = O.rmsnorm_fwd(x, fnorm, 1e-6)
+        xn = O.rmsnorm_fwd(x, fnorm, eps)
         outs.append((xn.float() @ head.float().t()).half()[0])
     return torch.stack(outs)
 
 
-@pytest.mark.parametrize('size,bits,act,use_graph', [('tiny', 4, False, True), ('tiny', 4, False, False), ('tiny', 4, True, True), ('tiny', 8, False, True),
-                                                     ('tiny', 3, True, True), ('tiny256', 4, False, True), ('tiny256', 4, False, False),
-                                                     ('tiny256', 4, True, True), ('tiny256', 3, True, True), ('tiny256', 3, False, True), ('tiny256', 2, True, False)])
-def test_decode_steps_match_oracle(size, bits, act, use_graph):
+DECODE_CASES = [('tiny', 4, False, True), ('tiny', 4, False, False), ('tiny', 4, True, True), ('tiny', 8, False, True), ('tiny', 3, True, True),
+                ('tiny256', 4, False, True), ('tiny256', 4, False, False), ('tiny256', 4, True, True), ('tiny256', 3, True, True), ('tiny256', 3, False, True),
+                ('tiny256', 2, True, False)]
+
+
+@pytest.mark.parametrize('size,bits,act,use_graph,rope', [pytest.param(*c, LLAMA1, id='-'.join(map(str, c))) for c in DECODE_CASES] +
+                         [pytest.param(size, 4, False, True, CODELLAMA, id=f'{size}-4-False-True-codellama') for size in ('tiny', 'tiny256')])
+def test_decode_steps_match_oracle(size, bits, act, use_graph, rope):
+    """Six decode steps against the oracle, on the kernel chain (tiny) and the persistent kernel (tiny256).  At the CodeLlama settings (RoPE
+    base 1e6, RMSNorm epsilon 1e-5) the first token's embedding row is scaled to a mean square of about 4e-6, near the epsilon, so that the
+    decoder's epsilon shows in the output."""
     from gptq_b200 import engine
-    dec = engine.synthetic_llama(size, bits=bits, groupsize=64, act_order=act, vocab=512, seed=bits, max_seq=600, use_graph=use_graph)
+    base, eps = rope
+    dec = engine.synthetic_llama(size, bits=bits, groupsize=64, act_order=act, vocab=512, seed=bits, max_seq=600, use_graph=use_graph, rope_base=base,
+                                 rms_eps=eps)
     if size == 'tiny256':
         # persistent single-kernel path, also for act-order (regrouped rows + input gathers) and 2/3-bit (nibble-widened) layers
         assert dec.launches_per_step() == 1
@@ -62,41 +73,49 @@ def test_decode_steps_match_oracle(size, bits, act, use_graph):
         assert dec.launches_per_step() > 1 and all(pm['qkv'] is None for pm in dec.perms)
     gen = torch.Generator().manual_seed(0)
     toks = torch.randint(0, 512, (6, ), generator=gen).tolist()
-    ref = _oracle_decode(dec, toks)
+    if rope != LLAMA1:
+        scale_down_embedding_row(dec.embed, toks[0], 8)
+    ref = _oracle_decode(dec, toks, eps=eps, base=base)
     for pos, tok in enumerate(toks):
         dec.tokens.fill_(tok)
         dec.positions.fill_(pos)
         dec.step()
         torch.cuda.synchronize()
-        assert_rel_close(dec.logits[0], ref[pos], rel=2e-2, what=f'bits={bits} act={act} pos={pos}')
+        assert_rel_close(dec.logits[0], ref[pos], rel=2e-2, what=f'{size} bits={bits} act={act} base={base:g} eps={eps:g} pos={pos}')
         assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
 
 
-@pytest.mark.parametrize('gs', [-1, 32])
-def test_hf_checkpoint_groupsizes_decode_on_the_persistent_kernel(gs):
+@pytest.mark.parametrize('gs,rope', [pytest.param(-1, LLAMA1, id='-1'), pytest.param(32, LLAMA1, id='32'), pytest.param(32, CODELLAMA, id='32-codellama')])
+def test_hf_checkpoint_groupsizes_decode_on_the_persistent_kernel(gs, rope):
     """The route a real checkpoint takes (the reference's load_quant recipe on the quant modules -> engine.from_hf_quant_model) at
     --groupsize -1 (QuantLinear takes groupsize = infeatures: 256 for qkv / o / gate / up, 768 for down) and 32: the persistent kernel
-    serves it with every groupsize hint intact, and six decode steps match the oracle at the bound of test_decode_steps_match_oracle."""
+    serves it with every groupsize hint intact, and six decode steps match the oracle at the bound of test_decode_steps_match_oracle.  At the
+    CodeLlama settings (config rope_theta 1e6, rms_norm_eps 1e-5) the decoder must take both from the checkpoint's config; the first token's
+    embedding row is scaled to a mean square of about 1.6e-6 (HF's init has std 0.02) so that the epsilon shows in the output."""
     import quant
     from gptq_b200 import engine
     from test_gpu_modules import _tiny_quant_llama
-    model = _tiny_quant_llama(gs=gs, hidden=256, intermediate=768, heads=2)
+    base, eps = rope
+    model = _tiny_quant_llama(gs=gs, hidden=256, intermediate=768, heads=2, rope_theta=base, rms_norm_eps=eps)
+    toks = torch.randint(0, model.config.vocab_size, (6, ), generator=torch.Generator().manual_seed(gs + 2)).tolist()
+    if rope != LLAMA1:
+        scale_down_embedding_row(model.model.embed_tokens.weight, toks[0], 4)
     quant.make_quant_attn(model)
     quant.make_quant_norm(model)
     quant.make_fused_mlp(model)
     dec = engine.from_hf_quant_model(model.cuda(), max_seq=16)
     assert dec.launches_per_step() == 1
+    assert (dec.model.rope_base, dec.model.rms_eps) == (base, pytest.approx(eps, rel=1e-7))
     for kl in dec.klayers:
         for name in ('qkv', 'o', 'gate', 'up', 'down'):
             K = kl[name].g_idx.numel()
             assert kl[name].hint == (K if gs == -1 else gs), f'{name}: groupsize hint {kl[name].hint}'
-    toks = torch.randint(0, dec.vocab, (6, ), generator=torch.Generator().manual_seed(gs + 2)).tolist()
-    ref = _oracle_decode(dec, toks)
+    ref = _oracle_decode(dec, toks, eps=eps, base=base)
     for pos, tok in enumerate(toks):
         dec.set_input(tok, pos)
         dec.step()
         torch.cuda.synchronize()
-        assert_rel_close(dec.logits[0], ref[pos], rel=2e-2, what=f'gs={gs} pos={pos}')
+        assert_rel_close(dec.logits[0], ref[pos], rel=2e-2, what=f'gs={gs} base={base:g} eps={eps:g} pos={pos}')
         assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
 
 

@@ -27,11 +27,14 @@ def _step_all(dec, toks, start):
     torch.cuda.synchronize()
 
 
-@pytest.mark.parametrize('size, bits, act', MODELS)
-def test_extend_after_decode_matches_stepping(size, bits, act):
-    """10 decode steps, then extend() with the next 29 tokens: the same cache rows as stepping them (1e-2) and the same logits at the next
-    step (2e-2), the bounds of test_prefill_then_decode_matches_token_by_token."""
-    _extend_after_decode(_model(size, bits, act, seed=5, max_seq=96))
+@pytest.mark.parametrize('size, bits, act, rope_base, cached', [pytest.param(*m, 10000.0, 10, id='-'.join(map(str, m))) for m in MODELS] +
+                         [pytest.param(size, 4, False, 1e6, 2060, id=f'{size}-4-False-base1e6-cached2060') for size in ('tiny', 'tiny256')])
+def test_extend_after_decode_matches_stepping(size, bits, act, rope_base, cached):
+    """`cached` decode steps, then extend() with the next 29 tokens: the same cache rows as stepping them (1e-2) and the same logits at the
+    next step (2e-2), the bounds of test_prefill_then_decode_matches_token_by_token.  At RoPE base 1e6 with 2060 cached positions the
+    extend pass rotates with the RoPE kernel and the stepping with the decode kernel, at positions past 2048."""
+    _extend_after_decode(_model(size, bits, act, seed=5, max_seq=cached + 86, rope_base=rope_base), what=f'{size} base={rope_base:g} cached={cached}',
+                         cached=cached)
 
 
 @pytest.mark.parametrize('gs, kernel', [(32, 'qlinear_generic_kernel'), (-1, 'qgemm_wgmma_kernel')])
@@ -43,25 +46,26 @@ def test_extend_after_decode_at_groupsizes(gs, kernel):
     _extend_after_decode(dec, kernel, f'gs={gs}')
 
 
-def _extend_after_decode(dec, kernel=None, what=''):
-    prompt = _ids(40, 2)
+def _extend_after_decode(dec, kernel=None, what='', cached=10):
+    c, e = cached, cached + 29
+    prompt = _ids(e + 1, 2)
     _step_all(dec, prompt, 0)
-    ref_logits, ref_k, ref_v = dec.logits[0].float().clone(), dec.k_cache[:, 0, :, :40].float().clone(), dec.v_cache[:, 0, :, :40].float().clone()
+    ref_logits, ref_k, ref_v = dec.logits[0].float().clone(), dec.k_cache[:, 0, :, :e + 1].float().clone(), dec.v_cache[:, 0, :, :e + 1].float().clone()
     dec.reset()
     dec.k_cache.zero_()
     dec.v_cache.zero_()
-    _step_all(dec, prompt[:10], 0)
-    assert dec.lengths == [10] and dec.cached_tokens == [prompt[:10]]
+    _step_all(dec, prompt[:c], 0)
+    assert dec.lengths == [c] and dec.cached_tokens == [prompt[:c]]
 
-    def extend():  # repeatable (run_kernel may trace it again): from the 10 cached positions each time
-        dec.lengths, dec.cached_tokens = [10], [prompt[:10]]
-        return dec.extend([prompt[10:39]])
+    def extend():  # repeatable (run_kernel may trace it again): from the c cached positions each time
+        dec.lengths, dec.cached_tokens = [c], [prompt[:c]]
+        return dec.extend([prompt[c:e]])
 
-    assert (extend() if kernel is None else run_kernel(extend, kernel, f'extend of 29 rows {what}')) == [39]
-    assert dec.lengths == [39] and dec.cached_tokens == [prompt[:39]]
-    assert_rel_close(dec.k_cache[:, 0, :, 10:39], ref_k[:, :, 10:39], rel=1e-2, what=f'extended K rows {what}')
-    assert_rel_close(dec.v_cache[:, 0, :, 10:39], ref_v[:, :, 10:39], rel=1e-2, what=f'extended V rows {what}')
-    dec.set_input(prompt[39], 39)
+    assert (extend() if kernel is None else run_kernel(extend, kernel, f'extend of 29 rows {what}')) == [e]
+    assert dec.lengths == [e] and dec.cached_tokens == [prompt[:e]]
+    assert_rel_close(dec.k_cache[:, 0, :, c:e], ref_k[:, :, c:e], rel=1e-2, what=f'extended K rows {what}')
+    assert_rel_close(dec.v_cache[:, 0, :, c:e], ref_v[:, :, c:e], rel=1e-2, what=f'extended V rows {what}')
+    dec.set_input(prompt[e], e)
     dec.step()
     torch.cuda.synchronize()
     assert_rel_close(dec.logits[0], ref_logits, rel=2e-2, what=f'logits after extend + 1 decode step {what}')

@@ -36,12 +36,12 @@ def test_quantlinear_module_forward_and_backward(bits, act):
     assert_rel_close(xd.grad, gref, what='module bwd')
 
 
-def _tiny_quant_llama(bits=4, gs=32, act=False, hidden=128, intermediate=352, heads=4):
+def _tiny_quant_llama(bits=4, gs=32, act=False, hidden=128, intermediate=352, heads=4, rope_theta=10000.0, rms_norm_eps=1e-6):
     import quant
     import utils
     from transformers import LlamaConfig, LlamaForCausalLM
     cfg = LlamaConfig(hidden_size=hidden, intermediate_size=intermediate, num_hidden_layers=2, num_attention_heads=heads, num_key_value_heads=heads,
-                      vocab_size=256, max_position_embeddings=128)
+                      vocab_size=256, max_position_embeddings=128, rope_theta=rope_theta, rms_norm_eps=rms_norm_eps)
     torch.manual_seed(0)
     model = LlamaForCausalLM(cfg).half().eval()
     layers = utils.find_layers(model)
@@ -59,9 +59,9 @@ def _tiny_quant_llama(bits=4, gs=32, act=False, hidden=128, intermediate=352, he
     return model
 
 
-def _ref_forward(model, ids):
-    """fp32 reference forward of the (not yet fused) quantized model using the CPU oracle for every op."""
-    import quant
+def _ref_forward(model, ids, base, eps):
+    """fp32 reference forward of the (not yet fused) quantized model using the CPU oracle for every op, at the RoPE base and RMSNorm
+    epsilon the caller chose (not the ones the model carries)."""
     cfg = model.config
     h = model.model.embed_tokens(ids).half()
     bsz, seq = ids.shape
@@ -73,29 +73,46 @@ def _ref_forward(model, ids):
 
     for layer in model.model.layers:
         a = layer.self_attn
-        x = O.rmsnorm_fwd(h, layer.input_layernorm.weight.data, layer.input_layernorm.variance_epsilon)
+        x = O.rmsnorm_fwd(h, layer.input_layernorm.weight.data, eps)
         qkv = torch.stack([lin(a.q_proj, x), lin(a.k_proj, x), lin(a.v_proj, x)], dim=2).view(bsz, seq, 3, nh, hd)
-        O.rope_inplace(qkv[:, :, :2], pos)
+        O.rope_inplace(qkv[:, :, :2], pos, base=base)
         q, k, v = (qkv[:, :, i].transpose(1, 2).float() for i in range(3))
         att = torch.nn.functional.scaled_dot_product_attention(q, k, v, is_causal=True).half()
         h = h + lin(a.o_proj, att.transpose(1, 2).reshape(bsz, seq, -1))
-        x = O.rmsnorm_fwd(h, layer.post_attention_layernorm.weight.data, layer.post_attention_layernorm.variance_epsilon)
+        x = O.rmsnorm_fwd(h, layer.post_attention_layernorm.weight.data, eps)
         m = layer.mlp
         inter = O.fused_mlp_fwd(x, (m.gate_proj.qweight, m.gate_proj.scales, m.gate_proj.qzeros, m.gate_proj.g_idx),
                                 (m.up_proj.qweight, m.up_proj.scales, m.up_proj.qzeros, m.up_proj.g_idx), m.gate_proj.bits)
         h = h + lin(m.down_proj, inter)
-    h = O.rmsnorm_fwd(h, model.model.norm.weight.data, model.model.norm.variance_epsilon)
+    h = O.rmsnorm_fwd(h, model.model.norm.weight.data, eps)
     return (h.float() @ model.lm_head.weight.data.float().t())
 
 
-@pytest.mark.parametrize('bits,act', [(4, False), (4, True), (3, True)])
-def test_load_quant_pipeline_on_tiny_llama(bits, act):
+def scale_down_embedding_row(embed, tok, shift):
+    """Multiply embedding row `tok` by 2^-shift in place, so that its mean square comes near the RMSNorm epsilon: only then does the
+    epsilon move the first norm by more than an fp16 ulp, and a norm that used another epsilon shows in the output."""
+    with torch.no_grad():
+        embed[tok] *= 2.0**-shift
+
+
+# LLaMA-1 (RoPE base 10000, RMSNorm epsilon 1e-6) and CodeLlama (base 1e6, epsilon 1e-5)
+LLAMA1, CODELLAMA = (10000.0, 1e-6), (1e6, 1e-5)
+
+
+@pytest.mark.parametrize('bits,act,rope', [pytest.param(4, False, LLAMA1, id='4-False'), pytest.param(4, True, LLAMA1, id='4-True'),
+                                           pytest.param(3, True, LLAMA1, id='3-True'), pytest.param(4, False, CODELLAMA, id='4-False-codellama')])
+def test_load_quant_pipeline_on_tiny_llama(bits, act, rope):
     """make_quant_linear -> (load) -> make_quant_attn / make_quant_norm / make_fused_mlp -> .to(DEV) -> forward,
-    prefill then one cached decode step, against the oracle-composed reference."""
+    prefill then one cached decode step, against the oracle-composed reference at the RoPE base and epsilon of the config.
+    At the CodeLlama settings the first token's embedding row is scaled to a mean square of about 1.6e-6 (HF's init has std 0.02),
+    where epsilon 1e-5 and 1e-6 give norms a factor 2 apart."""
     import quant
-    model = _tiny_quant_llama(bits=bits, act=act)
+    base, eps = rope
+    model = _tiny_quant_llama(bits=bits, act=act, rope_theta=base, rms_norm_eps=eps)
     ids = torch.randint(0, 256, (1, 9), generator=torch.Generator().manual_seed(0))
-    ref_logits = _ref_forward(model, ids)
+    if rope != LLAMA1:
+        scale_down_embedding_row(model.model.embed_tokens.weight, int(ids[0, 0]), 4)
+    ref_logits = _ref_forward(model, ids, base=base, eps=eps)
     quant.make_quant_attn(model)
     quant.make_quant_norm(model)
     quant.make_fused_mlp(model)
@@ -105,9 +122,10 @@ def test_load_quant_pipeline_on_tiny_llama(bits, act):
         assert model.model.layers[0].mlp.kernel_plan() is not None and model.model.layers[0].self_attn.qkv_proj.kernel_plan() is not None
     with torch.no_grad():
         out = model(ids[:, :8].cuda(), use_cache=True)
-        assert_rel_close(out.logits[0], ref_logits[0, :8], rel=2e-2, what='prefill logits')
+        what = f'bits={bits} act={act} base={base:g} eps={eps:g}'
+        assert_rel_close(out.logits[0], ref_logits[0, :8], rel=2e-2, what=f'{what}: prefill logits')
         step = model(ids[:, 8:9].cuda(), past_key_values=out.past_key_values, use_cache=True)
-        assert_rel_close(step.logits[0, 0], ref_logits[0, 8], rel=2e-2, what='decode logits')
+        assert_rel_close(step.logits[0, 0], ref_logits[0, 8], rel=2e-2, what=f'{what}: decode logits')
 
 
 @pytest.mark.parametrize('bits', [4, 3])

@@ -8,6 +8,7 @@ import torch
 
 from gpu_util import launched_kernels, report, run_kernel, ulp16
 from test_gpu_engine import _oracle_decode
+from test_gpu_modules import CODELLAMA, LLAMA1, scale_down_embedding_row
 
 pytestmark = pytest.mark.gpu
 
@@ -142,14 +143,18 @@ ENGINES = [('tiny', 4, False), ('tiny', 4, True), ('tiny', 3, True), ('tiny', 8,
            ('tiny256', 3, True), ('tiny256', 8, False)]
 
 
-@pytest.mark.parametrize('size,bits,act', ENGINES)
-def test_score_matches_the_oracle(size, bits, act):
+@pytest.mark.parametrize('size,bits,act,rope', [pytest.param(*e, LLAMA1, id='-'.join(map(str, e))) for e in ENGINES] +
+                         [pytest.param(size, 4, False, CODELLAMA, id=f'{size}-4-False-codellama') for size in ('tiny', 'tiny256')])
+def test_score_matches_the_oracle(size, bits, act, rope):
     """Three sequences of different lengths in one call against float64 log-softmaxes of the oracle's fp16 per-position logits.  The prefill
     and decode tests hold the logits to 2e-2 * max|ref logits| of the oracle; logsumexp is 1-Lipschitz in the max-norm, so the target logit
-    and the logsumexp move by at most that each: 2 x 2e-2 x max|ref logits| per element."""
+    and the logsumexp move by at most that each: 2 x 2e-2 x max|ref logits| per element.  Also at the CodeLlama settings (RoPE base 1e6,
+    RMSNorm epsilon 1e-5), with the first token's embedding row scaled near the epsilon."""
     from gptq_b200 import engine
-    dec = engine.synthetic_llama(size, bits=bits, groupsize=64, act_order=act, vocab=300, seed=bits + act, max_seq=16, use_graph=False)
-    _score_against_oracle(dec, bits, f'{size} bits={bits} act={act}')
+    base, eps = rope
+    dec = engine.synthetic_llama(size, bits=bits, groupsize=64, act_order=act, vocab=300, seed=bits + act, max_seq=16, use_graph=False, rope_base=base,
+                                 rms_eps=eps)
+    _score_against_oracle(dec, bits, f'{size} bits={bits} act={act} base={base:g} eps={eps:g}', rope=rope)
 
 
 @pytest.mark.parametrize('gs, kernel', [(32, 'qlinear_generic_kernel'), (-1, 'qgemm_wgmma_kernel')])
@@ -161,13 +166,16 @@ def test_score_matches_the_oracle_at_groupsizes(gs, kernel):
     _score_against_oracle(dec, 4, f'tiny256 gs={gs}', kernel)
 
 
-def _score_against_oracle(dec, seed, what, kernel=None):
+def _score_against_oracle(dec, seed, what, kernel=None, rope=LLAMA1):
     g = torch.Generator().manual_seed(seed)
     seqs = [torch.randint(0, 300, (n, ), generator=g).tolist() for n in (9, 2, 23)]
+    base, eps = rope
+    if rope != LLAMA1:
+        scale_down_embedding_row(dec.embed, seqs[0][0], 8)
     out = dec.score(seqs) if kernel is None else run_kernel(lambda: dec.score(seqs), kernel, f'{what}: score')
     assert [o.shape[0] for o in out] == [8, 1, 22] and all(o.dtype == torch.float32 for o in out)
     for s, lp in zip(seqs, out):
-        logits = _oracle_decode(dec, s)[:-1].double()
+        logits = _oracle_decode(dec, s, eps=eps, base=base)[:-1].double()
         ref = torch.log_softmax(logits, -1).gather(1, torch.tensor(s[1:])[:, None])[:, 0]
         bound = 2 * 2e-2 * logits.abs().amax(-1)
         report(((lp.cpu().double() - ref).abs() / bound).max().item(), f'{what} n={len(s)}')

@@ -81,10 +81,10 @@ def test_find_layers_and_make_quant_linear():
     quant.make_quant_linear(m, layers, 4, 32)  # idempotent
 
 
-def _tiny_llama():
+def _tiny_llama(**cfg_kw):
     from transformers import LlamaConfig, LlamaForCausalLM
     cfg = LlamaConfig(hidden_size=64, intermediate_size=96, num_hidden_layers=2, num_attention_heads=2, num_key_value_heads=2, vocab_size=128,
-                      max_position_embeddings=64)
+                      max_position_embeddings=64, **cfg_kw)
     torch.manual_seed(0)
     return LlamaForCausalLM(cfg).half().eval()
 
@@ -111,6 +111,49 @@ def test_load_quant_style_surgery_on_hf_llama():
     assert l0.mlp.gate_proj_qweight.shape == (8, 96) and isinstance(l0.mlp.down_proj, quant.QuantLinear)
     assert isinstance(l0.input_layernorm, quant.TritonLlamaRMSNorm) and isinstance(model.model.norm, quant.TritonLlamaRMSNorm)
     assert quant.autotune_warmup_linear(model) == 0 and quant.autotune_warmup_fused(model) == 0  # nothing on the GPU yet
+
+
+def test_rope_base_from_config():
+    """The base comes from rope_parameters (transformers >= 5, where a config has no rope_theta attribute), from rope_theta (4.31 - 4.x) or
+    defaults to 10000; any scaled rope type is refused, since the kernels rotate unscaled integer positions only."""
+    from types import SimpleNamespace
+    from transformers import LlamaConfig
+    from quant.fused_attn import rope_base_from_config
+    code_llama = LlamaConfig(rope_theta=1e6)
+    assert rope_base_from_config(code_llama) == 1e6
+    assert rope_base_from_config(LlamaConfig.from_dict({'rope_theta': 1e6})) == 1e6
+    assert rope_base_from_config(LlamaConfig()) == 10000.0
+    assert rope_base_from_config(SimpleNamespace(rope_theta=1e6, rope_scaling=None)) == 1e6
+    assert rope_base_from_config(SimpleNamespace()) == 10000.0
+    assert rope_base_from_config(SimpleNamespace(rope_theta=1e6, rope_scaling={'rope_type': 'default'})) == 1e6
+    for rope_type in ('linear', 'dynamic'):
+        with pytest.raises(ValueError, match=rope_type):
+            rope_base_from_config(LlamaConfig(rope_scaling={'type': rope_type, 'factor': 2.0}))
+        with pytest.raises(ValueError, match=rope_type):
+            rope_base_from_config(LlamaConfig(rope_parameters={'rope_type': rope_type, 'factor': 2.0, 'rope_theta': 1e4}))
+        with pytest.raises(ValueError, match=rope_type):
+            rope_base_from_config(SimpleNamespace(rope_theta=1e4, rope_scaling={'type': rope_type, 'factor': 4.0}))
+
+
+def test_make_quant_attn_takes_the_rope_base_from_the_config():
+    def surgery(model):
+        layers = utils.find_layers(model)
+        layers.pop('lm_head')
+        quant.make_quant_linear(model, layers, 4, 32)
+        quant.make_quant_attn(model)
+        return model
+
+    model = surgery(_tiny_llama(rope_theta=1e6))
+    assert [layer.self_attn.rope_base for layer in model.model.layers] == [1e6, 1e6]
+    model = surgery(_tiny_llama())
+    assert [layer.self_attn.rope_base for layer in model.model.layers] == [10000.0, 10000.0]
+    with pytest.raises(ValueError, match='linear'):
+        surgery(_tiny_llama(rope_scaling={'type': 'linear', 'factor': 2.0}))
+    # the decoder takes its one base from the attention modules, and refuses layers that disagree (before anything reaches the GPU)
+    from gptq_b200 import engine
+    model.model.layers[1].self_attn.rope_base = 1e6
+    with pytest.raises(ValueError, match='disagree'):
+        engine.from_hf_quant_model(model)
 
 
 def test_fuse_qkv_rejects_mismatched_act_order():
