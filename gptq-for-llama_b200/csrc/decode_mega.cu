@@ -21,11 +21,12 @@
 //      sum_k x_k (w_k - z) s  =  s * ( sum_k x_k w_k  -  z * sum_k x_k )
 // so the consumers feed the RAW nibbles to the tensor pipe (mma.sync m16n8k16, operands swapped: A = 16 output
 // columns x 16 k of weights, B = x): a nibble masked in place IS an fp16 subnormal (n * 2^-24, or 16 n * 2^-24 for
-// the odd nibbles, whose x is pre-scaled by 1/16 when it is staged), products and the fp32 accumulation are
-// exact, and scale / zero are applied ONCE per group on the fp32 accumulator together with the group's sum of
-// x (computed when x is staged).  5 integer instructions + 1 HMMA per packed word; the result differs from the
-// reference only by NOT rounding every dequantised weight to fp16 (it is closer to the exact product); the
-// 1e-3 tests in tests/ hold it to the oracle.
+// the odd nibbles, whose x carries a further 2^-4), products are exact and accumulate in fp32, and scale / zero are
+// applied ONCE per group on the fp32 accumulator together with the group's sum of x (computed when x is staged).
+// The staged x is scaled by a power of two per staged range (XScale) so that even the odd nibbles' copy of a small
+// input stays an fp16 normal; the column totals are scaled back once.  5 integer instructions + 1 HMMA per packed
+// word; the result differs from the reference only by NOT rounding every dequantised weight to fp16 (it is closer to
+// the exact product); tests/test_gpu_decode_input_ranges.py holds it to the float64 product from tiny to massive inputs.
 //
 // Split-K partial sums are accumulated with red.global.add.f32 into fp32 vectors that the NEXT operation
 // rounds to fp16 exactly where the reference rounds (a QuantLinear output is fp16); each vector is re-zeroed
@@ -508,32 +509,64 @@ __device__ __forceinline__ void zero_slice(float* buf, int n) {
     for (int i = lo + threadIdx.x; i < hi; i += kConsumers) reinterpret_cast<float4*>(buf)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
-__device__ __forceinline__ float block_sum(float v, float* red_s) {
+// sum of v and the maxima of the two 16-bit lanes of m over the consumer threads (red_s: 2 * kConsumerWarps words)
+__device__ __forceinline__ float block_sum(float v, uint32_t& m, float* red_s) {
     v = warp_sum(v);
+    const uint32_t mx = __reduce_max_sync(0xffffffffu, m & 0xffffu), my = __reduce_max_sync(0xffffffffu, m >> 16);
     cta_sync();
-    if ((threadIdx.x & 31) == 0) red_s[threadIdx.x >> 5] = v;
+    if ((threadIdx.x & 31) == 0) {
+        red_s[threadIdx.x >> 5] = v;
+        reinterpret_cast<uint32_t*>(red_s)[kConsumerWarps + (threadIdx.x >> 5)] = mx | (my << 16);
+    }
     cta_sync();
     float t = 0.f;
+    m = 0;
 #pragma unroll
-    for (int w = 0; w < kConsumerWarps; ++w) t += red_s[w];
+    for (int w = 0; w < kConsumerWarps; ++w) {
+        t += red_s[w];
+        m = __vmaxu2(m, reinterpret_cast<const uint32_t*>(red_s)[kConsumerWarps + w]);
+    }
     return t;
 }
 
 // ---- x staging ----------------------------------------------------------------------------------------------------------
 // Matvec input layout: 8 consecutive k (natural order, 4 half2 words w0..w3) are stored k-permuted as
-// (k0,k4)(k1,k5)(k2,k6)(k3,k7): the B fragments of the two MMAs of a packed word; the pairs that meet the ODD
-// nibbles (k1,k5 / k3,k7; mask 0x00f000f0 = 16 n) are pre-scaled by 1/16.
+// (k0,k4)(k1,k5)(k2,k6)(k3,k7): the B fragments of the two MMAs of a packed word.
 __device__ __forceinline__ uint4 perm8(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3) {
-    const __half2 sixteenth = __float2half2_rn(0.0625f);
-    uint4 o;
-    o.x = __byte_perm(w0, w2, 0x5410);
-    o.y = h2_as_u32(__hmul2(u32_as_h2(__byte_perm(w0, w2, 0x7632)), sixteenth));
-    o.z = __byte_perm(w1, w3, 0x5410);
-    o.w = h2_as_u32(__hmul2(u32_as_h2(__byte_perm(w1, w3, 0x7632)), sixteenth));
-    return o;
+    return make_uint4(__byte_perm(w0, w2, 0x5410), __byte_perm(w0, w2, 0x7632), __byte_perm(w1, w3, 0x5410), __byte_perm(w1, w3, 0x7632));
 }
-// position of natural index j (0..7) inside the permuted run of 8; the odd j are pre-scaled
+// position of natural index j (0..7) inside the permuted run of 8
 __device__ __forceinline__ int perm_pos(int j) { return ((j & 3) << 1) + (j >> 2); }
+
+// A staged range (the whole row of Q / G, a team's k-range of O / D; per sequence) is scaled by a power of two 2^e chosen from its largest
+// |x|, and the pairs that meet the ODD nibbles (k1,k5 / k3,k7; mask 0x00f000f0 = 16 n) by 2^(e - 4) more: the largest |x| lands in
+// [2^14, 2^15) (its odd-nibble copy in [2^10, 2^11)), so every staged value is an fp16 normal unless it lies 2^-29 below that maximum, and
+// the scaling is exact.  The step sums of x and the group epilogue's fp32 arithmetic scale with it (exactly: powers of two), and the
+// column totals are multiplied by 2^-e once before they leave.
+struct XScale {
+    float even, odd, inv;  // 2^e, 2^(e - 4), 2^-e
+};
+// from an upper bound m of the range's largest |x| (a tighter bound keeps more of the range exact; the staged values cannot overflow, as
+// e >= -1 and every |x| <= 65504)
+__device__ __forceinline__ XScale x_scale(float m) {
+    const int e = min(max(14 - ((int)((__float_as_uint(m) >> 23) & 255u) - 127), -1), 38);  // m = 0: any e (38)
+    return XScale{__int_as_float((127 + e) << 23), __int_as_float((123 + e) << 23), __int_as_float((127 - e) << 23)};
+}
+// running max of the fp16 magnitudes of the four half2 words of v (per 16-bit lane)
+__device__ __forceinline__ uint32_t max_abs8(uint32_t m, uint4 v) {
+    m = __vmaxu2(m, v.x & 0x7fff7fffu);
+    m = __vmaxu2(m, v.y & 0x7fff7fffu);
+    m = __vmaxu2(m, v.z & 0x7fff7fffu);
+    return __vmaxu2(m, v.w & 0x7fff7fffu);
+}
+__device__ __forceinline__ uint32_t scale_h2(uint32_t w, float f) {
+    const float2 v = __half22float2(u32_as_h2(w));
+    return h2_as_u32(__floats2half2_rn(v.x * f, v.y * f));
+}
+// one permuted run of 8 scaled for the tensor pipe
+__device__ __forceinline__ uint4 scale_run(uint4 v, const XScale& sc) {
+    return make_uint4(scale_h2(v.x, sc.even), scale_h2(v.y, sc.odd), scale_h2(v.z, sc.even), scale_h2(v.w, sc.odd));
+}
 
 // sum of the EFFECTIVE x of one staged run of 8 (what the tensor pipe will multiply the nibbles with)
 __device__ __forceinline__ float run_sum(uint4 v) {
@@ -541,27 +574,34 @@ __device__ __forceinline__ float run_sum(uint4 v) {
     const float even = (a.x + a.y) + (c.x + c.y), odd = (b.x + b.y) + (d.x + d.y);
     return fmaf(odd, 16.0f, even);
 }
-// xsum[s] = sum over the 32 k of step s of the staged x (4 runs of 8), for s < nsteps; `nthreads` threads (a multiple of 32) cooperate
-__device__ __forceinline__ void compute_xsum(const __half* xs, int nsteps, float* xsum, int tid, int nthreads) {
+// scales the nsteps k-steps staged at xs in place and sets xsum[s] = the sum over the 32 k of step s of the scaled x (4 runs of 8)
+__device__ __forceinline__ void scale_and_sum(__half* xs, int nsteps, float* xsum, const XScale& sc, int tid, int nthreads) {
     const int n4 = nsteps * 4;
     for (int base = 0; base < n4; base += nthreads) {
         const int idx = base + tid;
         float v = 0.f;
-        if (idx < n4) v = run_sum(*reinterpret_cast<const uint4*>(xs + idx * 8));
+        if (idx < n4) {
+            uint4* run = reinterpret_cast<uint4*>(xs + idx * 8);
+            const uint4 r = scale_run(*run, sc);
+            *run = r;
+            v = run_sum(r);
+        }
         v += __shfl_xor_sync(0xffffffffu, v, 1);
         v += __shfl_xor_sync(0xffffffffu, v, 2);
         if (idx < n4 && (idx & 3) == 0) xsum[idx >> 2] = v;
     }
 }
 
-// x = rmsnorm(src [+ fp16(acc)]) for the whole row (K = H), staged in xs (matvec layout, or natural order if PLAIN)
-// with its per-step sums in xsum; the updated residual stream (src + fp16(acc)) is written to resid_out by slices.
+// x = rmsnorm(src [+ fp16(acc)]) for the whole row (K = H), staged in xs (matvec layout and scaled, *xinv = 2^-e, or natural order if
+// PLAIN) with its per-step sums in xsum; the updated residual stream (src + fp16(acc)) is written to resid_out by slices.
 // All 512 consumer threads.  ACT: the matvec's packed rows were regrouped by the host: position k' holds feature perm[k'].
+// The staging scale comes from max|x| rstd max|w| >= max|x w rstd|, reduced with the sum of squares (no extra barrier).
 template <bool ACT, bool PLAIN>
 __device__ void stage_norm(const MegaParams& p, const __half* src, const float* acc, const __half* norm_w, __half* resid_out, __half* xs, float* xsum,
-                           __half* tmp, float* red_s, const int32_t* perm) {
+                           float* xinv, __half* tmp, float* red_s, const int32_t* perm) {
     const int H = p.H, tid = threadIdx.x, nch = H / 8;
     float ss = 0.f;
+    uint32_t xm = 0, wm = 0;  // largest fp16 magnitudes of x and of the norm weights (two 16-bit lanes each)
     uint4 nwv[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -584,11 +624,20 @@ __device__ void stage_norm(const MegaParams& p, const __half* src, const float* 
                 ss = fmaf(f.x, f.x, ss);
                 ss = fmaf(f.y, f.y, ss);
             }
-            *reinterpret_cast<uint4*>(tmp + c * 8) = make_uint4(xv[0], xv[1], xv[2], xv[3]);
+            const uint4 xq = make_uint4(xv[0], xv[1], xv[2], xv[3]);
+            *reinterpret_cast<uint4*>(tmp + c * 8) = xq;
+            xm = max_abs8(xm, xq);
+            wm = max_abs8(wm, nwv[i]);
         }
     }
-    const float tot = block_sum(ss, red_s);  // its barriers also publish tmp
+    uint32_t m = max(xm & 0xffffu, xm >> 16) | (max(wm & 0xffffu, wm >> 16) << 16);
+    const float tot = block_sum(ss, m, red_s);  // its barriers also publish tmp
     const float rstd = 1.0f / sqrtf(tot / (float)H + p.eps);
+    XScale sc{1.f, 1.f, 1.f};
+    if constexpr (!PLAIN) {
+        sc = x_scale(__half2float(__ushort_as_half((unsigned short)(m & 0xffffu))) * rstd * __half2float(__ushort_as_half((unsigned short)(m >> 16))) * 1.001f);
+        if (tid == 0) *xinv = sc.inv;
+    }
     if (resid_out != nullptr) {
         const int per = (nch + gridDim.x - 1) / gridDim.x;
         const int c = blockIdx.x * per + tid;
@@ -629,7 +678,7 @@ __device__ void stage_norm(const MegaParams& p, const __half* src, const float* 
             if constexpr (PLAIN) {
                 *reinterpret_cast<uint4*>(xs + c * 8) = make_uint4(o[0], o[1], o[2], o[3]);
             } else {
-                const uint4 pv = perm8(o[0], o[1], o[2], o[3]);
+                const uint4 pv = scale_run(perm8(o[0], o[1], o[2], o[3]), sc);
                 *reinterpret_cast<uint4*>(xs + c * 8) = pv;
                 // per-step sums of the staged x: the 4 runs of a k-step sit in 4 consecutive lanes (c < nch is uniform per warp)
                 float v = run_sum(pv);
@@ -684,6 +733,8 @@ struct TeamCtx {
     unsigned T, nb;            // global team index / number of teams
     __half* xseg;              // this team's half of the xs buffer (per-segment inputs of O and D)
     float* xsum_seg;
+    float* xinv_seg;           // [batch]: 2^-e of the staged segment (XScale)
+    uint32_t* xmax;            // [batch]: largest fp16 magnitude of the staged segment
     uint8_t* scratch;          // kTeamScratch bytes
 };
 
@@ -722,7 +773,7 @@ __device__ __forceinline__ float merge_records(const MegaParams& p, const HeadTe
 
 // Input of o_proj (XMODE == X_ATTN) / down_proj (X_SWIGLU) for the team's WHOLE unit range [u0, u1) (units = k-steps of 32, numbered
 // slab-major; the range wraps at most once from the end of one slab's k-range to the start of the next): staged once, in unit order,
-// into the team's half of the xs buffer with its per-step sums.  One L2 round trip for the common shapes.
+// into the team's half of the xs buffer, then scaled (XScale, per sequence) with its per-step sums.  One L2 round trip for the common shapes.
 // BATCH: sequence s of the range goes to xseg + s * xs_stride, its step sums to xsum_seg + s * H / 32.
 template <int XMODE, bool ACT, bool BATCH>
 __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int u0, int u1, const int32_t* perm) {
@@ -734,7 +785,8 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
         if (ks >= nk) ks -= nk;
         return ks * 32 + (e & 31);
     };
-    team_sync(tc.team);  // previous readers of xseg are done
+    if (tc.ttid < nbat) tc.xmax[tc.ttid] = 0;
+    team_sync(tc.team);  // previous readers of xseg (and of xmax) are done
     if constexpr (XMODE == X_SWIGLU) {  // h = fp16(silu(acc_gate) * acc_up)  (quant/fused_mlp.py:163-165)
         for (int c = tc.ttid; c < nun * 4 * nbat; c += kTeamThreads) {
             int s = 0, cs = c;  // sequence, 8-feature chunk of the range
@@ -751,17 +803,20 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
             const uint32_t o1 = h2_as_u32(__floats2half2_rn(swiglu(g0.z, a0.z), swiglu(g0.w, a0.w)));
             const uint32_t o2 = h2_as_u32(__floats2half2_rn(swiglu(g1.x, a1.x), swiglu(g1.y, a1.y)));
             const uint32_t o3 = h2_as_u32(__floats2half2_rn(swiglu(g1.z, a1.z), swiglu(g1.w, a1.w)));
-            *reinterpret_cast<uint4*>(tc.xseg + (size_t)s * p.xs_stride + cs * 8) = perm8(o0, o1, o2, o3);
+            const uint4 pv = perm8(o0, o1, o2, o3);
+            *reinterpret_cast<uint4*>(tc.xseg + (size_t)s * p.xs_stride + cs * 8) = pv;
+            const uint32_t m = max_abs8(0, pv);
+            atomicMax(tc.xmax + s, max(m & 0xffffu, m >> 16));
         }
     } else {
         // attention output: softmax-merge of the partial records (m, l, o[128]) of the head's teams (head_teams: contiguous, one
         // record each; BATCH: the head's teams inside the sequence's teams, seq_teams).
         constexpr int kBatch = 12;  // records fetched per round trip (a 7B head has 9 or 10 teams)
+        uint32_t vmax = 0;  // largest fp16 magnitude this thread put (per sequence: flushed into xmax)
         auto put = [&](__half* xseg, int e, float v) {
-            __half hv = __float2half_rn(v);
-            const int j8 = e & 7;
-            if (j8 & 1) hv = __hmul(hv, __float2half_rn(0.0625f));
-            xseg[(e & ~7) + perm_pos(j8)] = hv;
+            const __half hv = __float2half_rn(v);
+            xseg[(e & ~7) + perm_pos(e & 7)] = hv;
+            vmax = max(vmax, (uint32_t)(__half_as_ushort(hv) & 0x7fffu));
         };
         bool fast = false;
         if constexpr (!BATCH) {
@@ -821,6 +876,7 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
                     fetch(e);
                     emit(e);
                 }
+                atomicMax(tc.xmax, vmax);
             }
         }
         if (!fast) {
@@ -837,11 +893,17 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
                     ht.first += st.first;
                     put(tc.xseg + (size_t)s * p.xs_stride, e, merge_records<kBatch>(p, ht, d));
                 }
+                atomicMax(tc.xmax + s, vmax);
+                vmax = 0;
             }
         }
     }
     team_sync(tc.team);
-    for (int s = 0; s < nbat; ++s) compute_xsum(tc.xseg + (size_t)s * p.xs_stride, nun, tc.xsum_seg + s * (p.H / 32), tc.ttid, kTeamThreads);
+    for (int s = 0; s < nbat; ++s) {
+        const XScale sc = x_scale(__half2float(__ushort_as_half((unsigned short)tc.xmax[s])));
+        if (tc.ttid == 0) tc.xinv_seg[s] = sc.inv;
+        scale_and_sum(tc.xseg + (size_t)s * p.xs_stride, nun, tc.xsum_seg + s * (p.H / 32), sc, tc.ttid, kTeamThreads);
+    }
     team_sync(tc.team);
 }
 
@@ -851,7 +913,7 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
 // fragment columns), and out0 / out1 are [B][N].
 template <int NM, int XMODE, bool ACT = false, bool BATCH = false>
 __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& tc, int gs_steps, int K, int N, float* out0, float* out1, const __half* xs_full,
-                           const float* xsum_full, const int32_t* perm = nullptr, float* const* peers = nullptr) {
+                           const float* xsum_full, const float* xinv_full, const int32_t* perm = nullptr, float* const* peers = nullptr) {
     const int lane = tc.lane, g = lane >> 2, t = lane & 3;
     const int nk = K / 32, nslab = N / kSlabCols;
     int u, u_end;
@@ -977,20 +1039,26 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
             gpos += n;
             if (gpos == gs_steps) gpos = 0;
         }
+        // the totals are in units of the staged x: times 2^-e (exact)
+        const float* xinv = XMODE == X_FULL ? xinv_full : tc.xinv_seg;  // [sequence]
         if constexpr (BATCH) {  // the four columns of each of the lane's sequences: one 16-byte vector RED
             float* outq = (mi ? out1 : out0) + (slab_v - mi * nslab) * kSlabCols + tc.wt * 32 + 4 * cg;
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
+                const float inv = xinv[min(2 * t + j, B - 1)];
                 if (2 * t + j < B)
-                    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(outq + (size_t)(2 * t + j) * N), "f"(totb[0][j]), "f"(totb[1][j]),
-                                 "f"(totb[2][j]), "f"(totb[3][j])
+                    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(outq + (size_t)(2 * t + j) * N), "f"(totb[0][j] * inv), "f"(totb[1][j] * inv),
+                                 "f"(totb[2][j] * inv), "f"(totb[3][j] * inv)
                                  : "memory");
             }
-        } else if (peers == nullptr) {
-            asm volatile("red.global.add.f32 [%0], %1;" ::"l"(outp), "f"(tot) : "memory");  // the warp's 32 columns: one 128-byte line
-        } else {  // tensor parallelism, direct mode: the partial sum goes into out0's counterpart on every rank
-            const size_t off = (size_t)(outp - out0);
-            for (int q = 0; q < p.tp_size; ++q) asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(peers[q] + off), "f"(tot) : "memory");
+        } else {
+            tot *= xinv[0];
+            if (peers == nullptr) {
+                asm volatile("red.global.add.f32 [%0], %1;" ::"l"(outp), "f"(tot) : "memory");  // the warp's 32 columns: one 128-byte line
+            } else {  // tensor parallelism, direct mode: the partial sum goes into out0's counterpart on every rank
+                const size_t off = (size_t)(outp - out0);
+                for (int q = 0; q < p.tp_size; ++q) asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(peers[q] + off), "f"(tot) : "memory");
+            }
         }
         u += nseg;
     }
@@ -1321,7 +1389,9 @@ template <bool ACT, bool BATCH>
 __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __grid_constant__ MegaParams p) {
     extern __shared__ __align__(16) uint8_t smem_dyn[];
     uint8_t* smem_raw = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);  // TMA swizzle atoms: 1 KB aligned stages (1 KB of slack is allocated)
-    __shared__ float red_s[kConsumerWarps];
+    __shared__ float red_s[2 * kConsumerWarps];
+    __shared__ uint32_t xmax_s[kTeams][kMaxBatch];               // largest |x| of a team's staged O / D range (fp16 magnitude bits)
+    __shared__ float xinv_s[1 + kTeams][kMaxBatch];              // 2^-e of the staged x (XScale): [0] the rows of Q / G, [1 + team] the team's O / D range
     __shared__ __align__(8) unsigned long long bars_s[kTeams][2 * kMaxStages];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // smem (1 KB aligned): [team 0 ring][team 1 ring][xs: H halves][xsum: H/32 floats][tmp / team scratch]
@@ -1371,6 +1441,8 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
     tc.nb = nb;
     tc.xseg = xs + tc.team * (p.H / 2);
     tc.xsum_seg = xsum + tc.team * (p.H / 64);
+    tc.xinv_seg = xinv_s[1 + tc.team];
+    tc.xmax = xmax_s[tc.team];
     tc.scratch = tmp_raw + tc.team * kTeamScratch;
     ConsRing ring;
     ring.ring = smem_u32(smem_raw) + tc.team * ring_bytes;
@@ -1429,9 +1501,9 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
             const float* acc_s = acc != nullptr ? acc + (size_t)s * p.H : nullptr;
             __half* out_s = resid_out != nullptr ? resid_out + (size_t)s * p.H : nullptr;
             if (plain)
-                stage_norm<false, true>(p, src_s, acc_s, norm_w, out_s, xs + (size_t)s * p.xs_stride, xsum + s * (p.H / 32), tmp, red_s, nullptr);
+                stage_norm<false, true>(p, src_s, acc_s, norm_w, out_s, xs + (size_t)s * p.xs_stride, xsum + s * (p.H / 32), nullptr, tmp, red_s, nullptr);
             else
-                stage_norm<ACT, false>(p, src_s, acc_s, norm_w, out_s, xs + (size_t)s * p.xs_stride, xsum + s * (p.H / 32), tmp, red_s, perm);
+                stage_norm<ACT, false>(p, src_s, acc_s, norm_w, out_s, xs + (size_t)s * p.xs_stride, xsum + s * (p.H / 32), xinv_s[0] + s, tmp, red_s, perm);
         }
     };
 #pragma unroll 1
@@ -1446,7 +1518,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         zero_slice(p.acc_u, nbat * p.I);
         {
             OPTRACE_BEGIN(ring);
-            run_matvec<1, X_FULL, false, BATCH>(p, ring, tc, L.qkv.gs_steps, p.H, 3 * p.Hq, p.acc_qkv, nullptr, xs, xsum);
+            run_matvec<1, X_FULL, false, BATCH>(p, ring, tc, L.qkv.gs_steps, p.H, 3 * p.Hq, p.acc_qkv, nullptr, xs, xsum, xinv_s[0]);
             OPTRACE_END(ring, l, 0);
         }
         MTRACE(l * 12 + 2);
@@ -1467,9 +1539,9 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         {
             OPTRACE_BEGIN(ring);
             if constexpr (BATCH)
-                run_matvec<1, X_ATTN, ACT, true>(p, ring, tc, L.o.gs_steps, p.Hq, p.H, p.acc_o, nullptr, xs, xsum, L.o_perm);
+                run_matvec<1, X_ATTN, ACT, true>(p, ring, tc, L.o.gs_steps, p.Hq, p.H, p.acc_o, nullptr, xs, xsum, nullptr, L.o_perm);
             else
-                run_matvec<1, X_ATTN, ACT>(p, ring, tc, L.o.gs_steps, p.Hq, p.H, p.tp_exchange ? p.acc_o_loc : p.acc_o, nullptr, xs, xsum, L.o_perm, (p.tp_size > 1 && !p.tp_exchange) ? p.acc_o_peer : nullptr);
+                run_matvec<1, X_ATTN, ACT>(p, ring, tc, L.o.gs_steps, p.Hq, p.H, p.tp_exchange ? p.acc_o_loc : p.acc_o, nullptr, xs, xsum, nullptr, L.o_perm, (p.tp_size > 1 && !p.tp_exchange) ? p.acc_o_peer : nullptr);
             OPTRACE_END(ring, l, 2);
         }
         MTRACE(l * 12 + 6);
@@ -1481,7 +1553,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         MTRACE(l * 12 + 8);
         {
             OPTRACE_BEGIN(ring);
-            run_matvec<2, X_FULL, false, BATCH>(p, ring, tc, L.gate.gs_steps, p.H, p.I, p.acc_g, p.acc_u, xs, xsum);
+            run_matvec<2, X_FULL, false, BATCH>(p, ring, tc, L.gate.gs_steps, p.H, p.I, p.acc_g, p.acc_u, xs, xsum, xinv_s[0]);
             OPTRACE_END(ring, l, 3);
         }
         MTRACE(l * 12 + 9);
@@ -1492,9 +1564,9 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         {
             OPTRACE_BEGIN(ring);
             if constexpr (BATCH)
-                run_matvec<1, X_SWIGLU, false, true>(p, ring, tc, L.down.gs_steps, p.I, p.H, p.acc_d, nullptr, xs, xsum);
+                run_matvec<1, X_SWIGLU, false, true>(p, ring, tc, L.down.gs_steps, p.I, p.H, p.acc_d, nullptr, xs, xsum, nullptr);
             else
-                run_matvec<1, X_SWIGLU>(p, ring, tc, L.down.gs_steps, p.I, p.H, p.tp_exchange ? p.acc_d_loc : p.acc_d, nullptr, xs, xsum, nullptr, (p.tp_size > 1 && !p.tp_exchange) ? p.acc_d_peer : nullptr);
+                run_matvec<1, X_SWIGLU>(p, ring, tc, L.down.gs_steps, p.I, p.H, p.tp_exchange ? p.acc_d_loc : p.acc_d, nullptr, xs, xsum, nullptr, nullptr, (p.tp_size > 1 && !p.tp_exchange) ? p.acc_d_peer : nullptr);
             OPTRACE_END(ring, l, 4);
         }
         MTRACE(l * 12 + 11);
