@@ -25,7 +25,8 @@ for _p in (ROOT, os.path.join(ROOT, 'gptq-for-llama_b200')):  # as tests/conftes
         sys.path.insert(0, _p)
 
 import exact_fixtures as X  # noqa: E402
-from gpu_util import check_fp64_bound, fp16_from_fp64, launched_kernels, report  # noqa: E402
+from gpu_util import assert_equal, check_fp64_bound, fill_quant_linear, fp16_from_fp64, generic_t, launched_kernels, ops, recorded_transposes, \
+    report  # noqa: E402
 from oracle import gptq_oracle as O  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -38,10 +39,6 @@ def tc_kernel(M):
     return TC_2 if M > 128 else TC_1
 
 
-def generic_t(bits):
-    return f'qlinear_transpose_generic_kernel<{bits}, 2>'
-
-
 FAMILIES = ('qgemm_wgmma_t_kernel', 'qlinear_transpose_generic_kernel')
 FULL_K, FULL_N, FULL_GS = 4096, 4096, 128
 KERNEL_FORMS = [(4, True), (3, True), (2, False)]
@@ -50,7 +47,7 @@ KERNEL_FORMS = [(4, True), (3, True), (2, False)]
 def _kernel_form_layer(bits, act, K=1024, N=512, gs=128):
     import quant
     ql = quant.QuantLinear(bits, gs, K, N, False)
-    _fill(ql, bits, seed=30 + bits, act=act)
+    fill_quant_linear(ql, bits, seed=30 + bits, act=act)
     return ql.cuda()
 
 
@@ -121,31 +118,6 @@ def assert_route(routes, label, kernel):
     assert qk and all(strip(kernel) in strip(n) for n in qk), f'{label}: expected {kernel}, launched {qk}'
 
 
-class recorded_transposes:
-    """Records every ops.transpose_matmul248 request made inside the block (QuantLinearFunction.backward issues them from the autograd
-    worker thread); check() holds each to the form the wgmma kernel takes: int4 with a positive groupsize hint, more than 8 rows."""
-
-    def __enter__(self):
-        from gptq_b200 import ops as _ops
-        self.ops, self.shipped, self.calls = _ops, _ops.transpose_matmul248, []
-
-        def record(*args, **kw):
-            self.calls.append((args, kw))
-            return self.shipped(*args, **kw)
-
-        _ops.transpose_matmul248 = record
-        return self
-
-    def __exit__(self, *exc):
-        self.ops.transpose_matmul248 = self.shipped
-
-    def check(self, what, at_least=1):
-        assert len(self.calls) >= at_least, f'{what}: {len(self.calls)} transposed requests, expected at least {at_least}'
-        for args, kw in self.calls:
-            assert args[5] == 4 and kw.get('groupsize', 0) % 32 == 0 and kw.get('groupsize', 0) > 0 and args[0].shape[0] > 8, \
-                f'{what}: backward request with bits={args[5]}, hint={kw.get("groupsize")}, M={args[0].shape[0]}'
-
-
 @pytest.fixture(scope='module', autouse=True)
 def release_device_memory():
     """The full-size layers and their fp64 references are cached for the module; hand the memory back when it is done."""
@@ -153,12 +125,6 @@ def release_device_memory():
     random_layer.cache_clear()
     device_layer.cache_clear()
     torch.cuda.empty_cache()
-
-
-@pytest.fixture(scope='module')
-def ops():
-    from gptq_b200 import ops as _ops  # raises if libgptq_b200.so is missing: no fallback
-    return _ops
 
 
 class Layer:
@@ -203,15 +169,6 @@ def where(M, N, m, k, n=None):
     wt = 2 if M > 128 else 1
     s = f'm={m} k={k} tile (row {m // (128 * wt)}, feature {k // 128}) WT={wt} warpgroup {(m % (128 * wt)) // (64 * wt)}'
     return s if n is None else s + f' n={n} (step {n // 64}, n%64={n % 64})'
-
-
-def assert_equal(out, exp, what, locate):
-    assert out.shape == exp.shape, (what, out.shape, exp.shape)
-    if torch.equal(out, exp):
-        return
-    bad = out != exp
-    r, c = (int(i) for i in torch.nonzero(bad)[0])
-    raise AssertionError(f'{what}: {int(bad.sum())} / {bad.numel()} outputs differ; first at {locate(r, c)}: got {out[r, c].item()!r}, want {exp[r, c].item()!r}')
 
 
 # ============================================================================= routing
@@ -346,11 +303,6 @@ def test_nothing_past_row_M_is_read_into_the_result(ops, M):
 
 
 # ============================================================================= modules: kernel-form layers
-def _fill(ql, bits, seed, act=False):
-    qw, s, qz, g, _ = O.random_packed(ql.infeatures, ql.outfeatures, bits, ql.groupsize, act_order=act, seed=seed)
-    ql.qweight, ql.scales, ql.qzeros, ql.g_idx = qw, s, qz, g
-
-
 @pytest.mark.parametrize('bits,act', KERNEL_FORMS)
 @pytest.mark.parametrize('M', [40, 300])
 def test_kernel_form_layers_backpropagate_on_the_wgmma_kernel(ops, bits, act, M):
@@ -376,7 +328,7 @@ def test_backward_under_autocast_returns_the_inputs_dtype():
     """custom_fwd(cast_inputs=float16) semantics: an fp32 input under autocast gets an fp32 gradient (autograd casts it back)."""
     import quant
     ql = quant.QuantLinear(4, 128, 256, 128, False)
-    _fill(ql, 4, seed=40)
+    fill_quant_linear(ql, 4, seed=40)
     ql = ql.cuda()
     x = torch.randn(16, 256, device='cuda', requires_grad=True)
     with torch.autocast('cuda', dtype=torch.float16):
@@ -413,7 +365,7 @@ def test_lora_step_on_one_layer_matches_the_dense_twin(ops):
     import quant
     K, N, M, gs = 512, 256, 64, 128
     ql = quant.QuantLinear(4, gs, K, N, False)
-    _fill(ql, 4, seed=50)
+    fill_quant_linear(ql, 4, seed=50)
     ql = ql.cuda()
     W = ops.dequant(ql.qweight, ql.scales, ql.qzeros, ql.g_idx, 4, gs).float()
     dense = nn.Linear(K, N, bias=False).cuda()
@@ -454,7 +406,7 @@ def test_lora_finetuning_of_a_tiny_llama_matches_the_dense_twin(ops):
     for name, m in model.named_modules():
         if isinstance(m, quant.QuantLinear):
             seed += 1
-            _fill(m, 4, seed=60 + seed)
+            fill_quant_linear(m, 4, seed=60 + seed)
     model = model.cuda()
     for name, m in list(model.named_modules()):
         if isinstance(m, quant.QuantLinear):

@@ -4,7 +4,7 @@ import pytest
 import torch
 
 from gpu_util import assert_rel_close
-from test_gpu_engine import _oracle_decode
+from llama_oracle import LlamaOracle
 
 pytestmark = pytest.mark.gpu
 
@@ -56,7 +56,8 @@ def test_batch_columns_match_oracle(size, bits, act, batch):
     assert dec.launches_per_step() == 1
     assert (dec.perms[0]['qkv'] is not None) == act
     toks = torch.randint(0, 512, (batch, 6), generator=torch.Generator().manual_seed(batch)).tolist()
-    refs = [_oracle_decode(dec, t) for t in toks]
+    oracle = LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0)
+    refs = [oracle.logits(t) for t in toks]
     for pos in range(6):
         dec.set_input([t[pos] for t in toks], pos)
         dec.step()

@@ -2,7 +2,6 @@
 bound derived from the kernel's arithmetic, at every query-tile and key-tile edge; bit-exact anchors; NaN in every cache row the result must
 not read; determinism and independence of the spans; which kernels run."""
 import json
-import math
 import os
 import subprocess
 import sys
@@ -10,97 +9,12 @@ import sys
 import pytest
 import torch
 
-from gpu_util import report, ulp16
+from gpu_util import HD, check_cached_attention, make_kv_cache, report, run_cached_attention
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0**-24
-HD = 128
 STARTS = (0, 1, 63, 64, 65, 127, 128, 129, 1000, 2047, 2048, 4095, None)  # None: max_seq - rows
 ROWS = (1, 2, 63, 64, 65, 127, 128, 129, 300)
-
-
-def make_cache(B, nh, S, spans, seed=0, layers=3, layer=1, poison=True):
-    """q rows for `spans` and a [layers, B, nh, S, 128] cache whose slice `layer` holds random keys / values in every row a span may read
-    (rows 0 .. start + rows - 1 of its sequence), with heavy keys (scores a few units above the rest) on both sides of every 128-key tile edge
-    and on the diagonal of every span.  Every other cache row -- past a span's end, sequences without a span, the other layers -- is NaN
-    (poison) or random."""
-    g = torch.Generator(device='cuda').manual_seed(seed)
-    M = sum(n for _, _, n in spans)
-    u = torch.randn(HD, device='cuda', generator=g, dtype=torch.float64)
-    u = u / u.norm()
-    q = (torch.randn(M, nh, HD, device='cuda', generator=g, dtype=torch.float64) + 8 * u).half().view(M, nh * HD)
-    shape = (layers, B, nh, S, HD)
-    fill = float('nan') if poison else 0.0
-    kc = torch.full(shape, fill, device='cuda', dtype=torch.float16)
-    vc = torch.full(shape, fill, device='cuda', dtype=torch.float16)
-    if not poison:
-        kc.normal_(generator=g)
-        vc.normal_(generator=g)
-    for b, s, n in spans:
-        L = s + n
-        k = torch.randn(nh, L, HD, device='cuda', generator=g, dtype=torch.float64) * 0.5
-        heavy = [j for e in range(128, L + 128, 128) for j in (e - 2, e - 1, e, e + 1) if 0 <= j < L] + list(range(s, L, 7))
-        k[:, heavy] += 4 * u
-        kc[layer, b, :, :L] = k.half()
-        vc[layer, b, :, :L] = torch.randn(nh, L, HD, device='cuda', generator=g).half()
-    return q, kc, vc
-
-
-def reference(q, kc, vc, spans):
-    """float64 attention of each span and the per-element bound of the kernel's arithmetic (module docstring of csrc/cached_attention.cu):
-      scores      fp32 accumulation of 128 products, default depth 128 / 16 + 64 = 72 roundings, then * log2(e)/sqrt(128) in fp32 (the constant's
-                  rounding, the multiply, and the subtraction of the running max: <= 6 u |t|):  eps = max_j (72 u (|q|.|k_j|) / sqrt(128) + 6 u |t_j|)
-                  moves every normalised weight by a factor within exp(+-2 eps)
-      exp2f       2 ulp = 2^-22 relative, numerator and denominator
-      fp16(P)     numerator only: 2^-11 relative, or 2^-25 absolute (subnormal fp16, p <= 1 and the final row sum >= 1)
-      sums        P.V in fp32: 8 k-steps per key tile (+ 64 inside the MMA) and one rescale per tile; the row sum: 32 adds per tile per thread,
-                  a rescale per tile and 2 shuffles; the division: 1 rounding;  all relative to A = sum_j p_j |v_j|
-      output      one fp16 rounding: ulp16
-    Returns per span (ref [n, nh, 128], bound [n, nh, 128])."""
-    out, r0 = [], 0
-    nh = kc.shape[1]
-    for b, s, n in spans:
-        L = s + n
-        Q = q[r0:r0 + n].view(n, nh, HD).transpose(0, 1).double()  # [nh, n, 128]
-        K, V = kc[b, :, :L].double(), vc[b, :, :L].double()          # [nh, L, 128]
-        T = Q @ K.transpose(1, 2) / math.sqrt(HD)
-        Aqk = Q.abs() @ K.abs().transpose(1, 2) / math.sqrt(HD)
-        vis = torch.arange(L, device='cuda')[None, :] <= (s + torch.arange(n, device='cuda'))[:, None]  # [n, L]
-        T = T.masked_fill(~vis, -math.inf)
-        P = torch.softmax(T, -1)
-        ref = P @ V
-        A = P @ V.abs()
-        nkt = (L - 1) // 128 + 1
-        eps = (72 * U * Aqk + 6 * U * T.abs()).masked_fill(~vis, 0).amax(-1, keepdim=True)
-        Vsum = vis.double() @ V.abs()  # sum over the visible keys of |v_j|
-        rel = (torch.exp(2 * eps) - 1) + 2.0**-11 + 2 * 2.0**-22 + (8 * nkt + 64 + 2 * nkt + 32 * nkt + nkt + 2 + 2) * U
-        E = rel * A + 2.0**-25 * Vsum
-        bound = ulp16(ref.abs() + E) + E
-        out.append((ref.transpose(0, 1), bound.transpose(0, 1)))
-        r0 += n
-    return out
-
-
-def check(out, q, kc, vc, spans, what):
-    worst, r0 = 0.0, 0
-    nh = kc.shape[1]
-    assert torch.isfinite(out).all(), f'{what}: non-finite output'
-    for (b, s, n), (ref, bound) in zip(spans, reference(q, kc, vc, spans)):
-        got = out[r0:r0 + n].view(n, nh, HD).double()
-        ratio_t = (got - ref).abs() / bound
-        ratio = ratio_t.max().item()
-        assert ratio <= 1, f'{what}: span (seq {b}, start {s}, rows {n}): first bad (row, head, dim) {tuple(int(i) for i in torch.nonzero(ratio_t > 1)[0])}'
-        worst = max(worst, ratio)
-        r0 += n
-    return worst
-
-
-def run(q, kc, vc, spans, layer=1):
-    from gptq_b200 import ops
-    out = ops.cached_attention(q, kc[layer], vc[layer], spans)
-    torch.cuda.synchronize()
-    return out
 
 
 @pytest.mark.parametrize('rows', ROWS)
@@ -112,35 +26,35 @@ def test_against_fp64_softmax_at_every_edge(rows):
     worst = 0.0
     for c in range(0, len(starts), 8):
         spans = [(b, s, rows) for b, s in enumerate(starts[c:c + 8])]
-        q, kc, vc = make_cache(8, nh, S, spans, seed=rows * 100 + c)
-        out = run(q, kc, vc, spans)
-        worst = max(worst, check(out, q, kc[1], vc[1], spans, f'rows {rows}'))
+        q, kc, vc = make_kv_cache(8, nh, S, spans, seed=rows * 100 + c)
+        out = run_cached_attention(q, kc, vc, spans)
+        worst = max(worst, check_cached_attention(out, q, kc[1], vc[1], spans, f'rows {rows}'))
     report(worst, f'{rows} rows at starts {starts}')
 
 
 def test_llama_7b_shape():
     """32 heads, max_seq 2048: 128 rows at start 1920 (the span ends at the last cache row), next to a ragged second sequence."""
     spans = [(0, 1920, 128), (1, 700, 77)]
-    q, kc, vc = make_cache(2, 32, 2048, spans, seed=7, layers=2, layer=1)
-    report(check(run(q, kc, vc, spans), q, kc[1], vc[1], spans, '7B shape'), '32 heads, start 1920, 128 rows')
+    q, kc, vc = make_kv_cache(2, 32, 2048, spans, seed=7, layers=2, layer=1)
+    report(check_cached_attention(run_cached_attention(q, kc, vc, spans), q, kc[1], vc[1], spans, '7B shape'), '32 heads, start 1920, 128 rows')
 
 
 def test_strided_q_from_the_fused_qkv_output():
     """q read in place from the q columns of a [M, 3 * H] qkv tensor (row pitch 3 H), as the engine passes it."""
     from gptq_b200 import ops
     spans = [(0, 5, 40), (1, 0, 130)]
-    q, kc, vc = make_cache(2, 2, 256, spans, seed=8)
+    q, kc, vc = make_kv_cache(2, 2, 256, spans, seed=8)
     qkv = torch.randn(q.shape[0], 3 * q.shape[1], device='cuda').half()
     qkv[:, :q.shape[1]] = q
     out = ops.cached_attention(qkv[:, :q.shape[1]], kc[1], vc[1], spans)
-    assert torch.equal(out, run(q, kc, vc, spans))
+    assert torch.equal(out, run_cached_attention(q, kc, vc, spans))
 
 
 # ----------------------------------------------------------------------------- bit-exact anchors
 def test_position_zero_returns_its_own_value_row():
     spans = [(0, 0, 200), (1, 0, 1), (2, 0, 129)]
-    q, kc, vc = make_cache(3, 2, 512, spans, seed=9)
-    out = run(q, kc, vc, spans)
+    q, kc, vc = make_kv_cache(3, 2, 512, spans, seed=9)
+    out = run_cached_attention(q, kc, vc, spans)
     r0 = 0
     for b, _, n in spans:
         assert torch.equal(out[r0].view(2, HD), vc[1, b, :, 0]), f'sequence {b}: position 0'
@@ -153,7 +67,7 @@ def test_equal_keys_and_alternating_values_cancel_exactly():
     leaves a nonzero output."""
     S, nh = 1300, 2
     spans = [(0, 0, 300), (1, 1, 129), (2, 127, 130), (3, 1000, 300), (4, 64, 1), (5, 65, 2)]
-    q, kc, vc = make_cache(6, nh, S, spans, seed=10)
+    q, kc, vc = make_kv_cache(6, nh, S, spans, seed=10)
     g = torch.Generator(device='cuda').manual_seed(11)
     M = q.shape[0]
     q.copy_((torch.randint(-1, 2, (M, nh * HD), device='cuda', generator=g) * 0.25).half())
@@ -163,7 +77,7 @@ def test_equal_keys_and_alternating_values_cancel_exactly():
         w = (torch.randint(-32, 33, (nh, 1, HD), device='cuda', generator=g) / 16).half()
         sign = 1 - 2 * (torch.arange(L, device='cuda') % 2).half()
         vc[1, b, :, :L] = w * sign[None, :, None]
-    out = run(q, kc, vc, spans)
+    out = run_cached_attention(q, kc, vc, spans)
     r0, checked = 0, 0
     for b, s, n in spans:
         for i in range(n):
@@ -178,21 +92,21 @@ def test_equal_keys_and_alternating_values_cancel_exactly():
 def test_nan_in_unread_rows_does_not_reach_the_result():
     """The same spans on a cache whose unread rows are NaN and on one where they are random: every output finite and bit-identical."""
     spans = [(0, 0, 1), (2, 127, 130), (3, 200, 57), (1, 1000, 300)]
-    q, kc, vc = make_cache(5, 2, 1400, spans, seed=12, poison=True)
-    _, kc2, vc2 = make_cache(5, 2, 1400, spans, seed=12, poison=False)
+    q, kc, vc = make_kv_cache(5, 2, 1400, spans, seed=12, poison=True)
+    _, kc2, vc2 = make_kv_cache(5, 2, 1400, spans, seed=12, poison=False)
     for b, s, n in spans:  # the same rows that are read
         kc2[1, b, :, :s + n] = kc[1, b, :, :s + n]
         vc2[1, b, :, :s + n] = vc[1, b, :, :s + n]
-    a, c = run(q, kc, vc, spans), run(q, kc2, vc2, spans)
+    a, c = run_cached_attention(q, kc, vc, spans), run_cached_attention(q, kc2, vc2, spans)
     assert torch.isfinite(a).all() and torch.equal(a, c)
 
 
 def test_determinism_and_span_independence():
     from gptq_b200 import ops
     spans = [(0, 3, 200), (1, 500, 64), (2, 0, 1), (3, 127, 129)]
-    q, kc, vc = make_cache(4, 2, 1024, spans, seed=13)
-    a = run(q, kc, vc, spans)
-    assert torch.equal(a, run(q, kc, vc, spans)), 'two runs differ'
+    q, kc, vc = make_kv_cache(4, 2, 1024, spans, seed=13)
+    a = run_cached_attention(q, kc, vc, spans)
+    assert torch.equal(a, run_cached_attention(q, kc, vc, spans)), 'two runs differ'
     rows = [n for _, _, n in spans]
     parts = a.split(rows)
     qs = q.split(rows)
@@ -226,7 +140,7 @@ print(json.dumps(sorted(names)))
 
 def test_empty_call():
     from gptq_b200 import ops
-    q, kc, vc = make_cache(2, 2, 256, [(0, 10, 50)], seed=14)
+    q, kc, vc = make_kv_cache(2, 2, 256, [(0, 10, 50)], seed=14)
     assert ops.cached_attention(q[:0], kc[1], vc[1], [(1, 0, 0)]).shape == (0, 2 * HD)
 
 

@@ -43,12 +43,16 @@ import pytest  # noqa: E402
 import torch  # noqa: E402
 
 import exact_fixtures as X  # noqa: E402
-from gpu_util import check_fp64_bound, check_swiglu_fp64_bound, fp16_from_fp64, fp16_ulp_distance, launched_kernels, report  # noqa: E402
+from gpu_util import Layer, WorstRatios, assert_equal, check_fp64_bound, check_swiglu_fp64_bound, cyclic, fp16_from_fp64, fp16_ulp_distance, \
+    generic, generic_t, launched_kernels, ops, recorded_transposes  # noqa: E402
+from llama_oracle import END_TO_END_TOL, KV_ROW_TOL, MLP_HEAD_TOL, LlamaOracle, assert_no_failures, check, check_extend_against_stepping, \
+    check_scores  # noqa: E402
 from oracle import gptq_oracle as O  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-WORST = {}  # sweep -> worst |err| / bound
+WORST = WorstRatios()
+note = WORST.note
 
 
 @pytest.fixture(scope='module', autouse=True)
@@ -56,49 +60,13 @@ def worst_ratio_summary():
     yield
     layer.cache_clear()
     torch.cuda.empty_cache()
-    for sweep, r in WORST.items():
-        print(f'worst |err| / bound, {sweep}: {r:.3g}')
-
-
-def note(sweep, ratio):
-    WORST[sweep] = max(WORST.get(sweep, 0.0), ratio)
-    return ratio
-
-
-@pytest.fixture(scope='module')
-def ops():
-    from gptq_b200 import ops as _ops  # raises if libgptq_b200.so is missing: no fallback
-    return _ops
-
-
-def generic(bits, M, dual=False):
-    return f'qlinear_generic_kernel<{bits}, {M if M <= 2 else 4}, {str(dual).lower()}>'
-
-
-def generic_t(bits):
-    return f'qlinear_transpose_generic_kernel<{bits}, 2>'
+    WORST.summary()
 
 
 # ----------------------------------------------------------------------------- layers and inputs
-class Layer:
-    """A packed layer on the CPU and on the device, the oracle's fp16 weight W [K, N] (built on the CPU) on the device, and the groupsize
-    hint the kernels get: gs for a trivial g_idx, 0 (the g_idx gather) for act-order."""
-
-    def __init__(self, packed, bits, gs, act):
-        self.cpu = tuple(packed)
-        self.dev = tuple(t.cuda() for t in packed)
-        self.bits, self.gs, self.act = bits, gs, act
-        self.hint = 0 if act else gs
-        self.W = O.dequant(*packed, bits).cuda()
-
-    @property
-    def K(self):
-        return self.W.shape[0]
-
-
 @lru_cache(maxsize=1)
 def layer(K, N, bits, gs, act, seed=0):
-    return Layer(O.random_packed(K, N, bits, gs, act_order=act, seed=seed)[:4], bits, gs, act)
+    return Layer.random(K, N, bits, gs, act, seed=seed)
 
 
 def pow2_layer(K, N, bits, gs, act, seed=0):
@@ -172,22 +140,6 @@ def check_sliced(out, x, W, depth, what, cols=4096):
         worst = max(worst, check_fp64_bound(out[:, c0:c1], x, W[:, c0:c1], what=f'{what} cols {c0}:{c1}', depth=depth,
                                             locate=lambda m, n, c0=c0: f'm={m} n={c0 + n}'))
     return worst
-
-
-def assert_equal(out, exp, what, locate):
-    """torch.equal, naming the first mismatching element through locate(row, col)."""
-    assert out.shape == exp.shape, (what, out.shape, exp.shape)
-    if torch.equal(out, exp):
-        return
-    bad = out != exp
-    r, c = (int(i) for i in torch.nonzero(bad)[0])
-    raise AssertionError(f'{what}: {int(bad.sum())} / {bad.numel()} outputs differ; first at {locate(r, c)}: got {out[r, c].item()!r}, '
-                         f'want {exp[r, c].item()!r}')
-
-
-def cyclic(ks, M):
-    ks = list(ks)
-    return ks + ks[:(-len(ks)) % M]
 
 
 def forward_depth(K):
@@ -601,13 +553,11 @@ def test_engine_decode_on_the_generic_kernels(ops, name):
     """Batch 1 at positions {0, 255, 256, 2047} and batch 8 at those positions, on a random KV cache.  The layer-0 V rows equal the V columns
     of ops.matmul248(ops.rmsnorm(embedding rows), qkv) bit for bit (the same generic kernel instance at the same M), the K rows are within
     KV_ROW_TOL of a float64 RoPE of that product; the logits of the 1-layer model (input: the embedding row, known exactly) and of the
-    2-layer model are within the block and end-to-end bounds of tests/test_gpu_engine_fullsize.py against the oracle; next_tokens is the
+    2-layer model are within the block and end-to-end bounds of tests/llama_oracle.py against the oracle; next_tokens is the
     argmax."""
     from gptq_b200 import engine
-    from test_gpu_engine_fullsize import END_TO_END_TOL, FAILURES, KV_ROW_TOL, MLP_HEAD_TOL, _cpu_layers, check, oracle_attn_block, oracle_head, \
-        oracle_mlp_block
     base = _model(name)
-    layers = _cpu_layers(base)
+    oracle = LlamaOracle.from_decoder(base, eps=1e-6, base=10000.0)
     eps = base.model.rms_eps
     H, nh, hd = base.hidden, base.n_heads, base.head_dim
     for B, positions in ((1, [0, 255, 256, 2047]), (8, [0, 255, 256, 2047, 2047, 256, 255, 0])):
@@ -643,16 +593,15 @@ def test_engine_decode_on_the_generic_kernels(ops, name):
                 x = base.embed[toks[b]].cpu()[None, :].clone()
                 refs = []
                 for li in range(2):
-                    x = oracle_mlp_block(layers[li], oracle_attn_block(base, layers[li], x, p, kc[li][b:b + 1], vc[li][b:b + 1])[0])
-                    refs.append(oracle_head(base, x))
+                    x = oracle.mlp(li, oracle.attention(li, x, p, kc[li, b], vc[li, b])[0])
+                    refs.append(oracle.head(x)[0])
                 check(decs[1].logits[b], refs[0], MLP_HEAD_TOL, f'{what}: logits of sequence {b} after 1 layer')
                 check(decs[2].logits[b], refs[1], END_TO_END_TOL, f'{what}: logits of sequence {b} after 2 layers, end to end')
                 for n, dec in decs.items():
                     assert int(dec.next_tokens[b]) == int(dec.logits[b].float().argmax()), f'{what}: greedy token of sequence {b}, {n} layers'
         del decs
         torch.cuda.empty_cache()
-    failed, FAILURES[:] = list(FAILURES), []
-    assert not failed, '\n'.join(failed)
+    assert_no_failures()
 
 
 def test_extend_of_the_int8_model_matches_stepping():
@@ -661,65 +610,17 @@ def test_extend_of_the_int8_model_matches_stepping():
     the run-to-run spread bounds of tests/test_gpu_extend.py (max 1.5e-2, rms 3e-3 of the rms)."""
     dec = _model('7b-int8-g128')
     toks = torch.randint(0, VOCAB, (2048, ), generator=torch.Generator().manual_seed(3)).tolist()
-
-    def step_all(ts, start):
-        for i, t in enumerate(ts):
-            dec.set_input(t, start + i)
-            dec.step()
-        torch.cuda.synchronize()
-
-    step_all(toks[:1791], 0)
-    assert dec.extend([toks[1791:2047]]) == [2047]
-    dec.set_input(toks[2047], 2047)
-    dec.step()
-    torch.cuda.synchronize()
-    got = [dec.logits[0].float().clone(), dec.k_cache[:, 0, :, 1791:2047].float().clone(), dec.v_cache[:, 0, :, 1791:2047].float().clone()]
-    step_all(toks[1791:], 1791)
-    ref = [dec.logits[0].float(), dec.k_cache[:, 0, :, 1791:2047].float(), dec.v_cache[:, 0, :, 1791:2047].float()]
-    for what, a, b in zip(('logits', 'K rows', 'V rows'), got, ref):
-        rms = b.pow(2).mean().sqrt().item()
-        d = (a - b).abs()
-        print(f'  7b int8 extend vs stepping, {what}: max {d.max().item() / rms:.3g}, rms {d.pow(2).mean().sqrt().item() / rms:.3g} of the rms')
-        assert d.max().item() <= 1.5e-2 * rms and d.pow(2).mean().sqrt().item() <= 3e-3 * rms, what
-
-
-def _oracle_sequence_logits(dec, Ws, toks, eps=1e-6, base=10000.0):
-    """The oracle's per-position logits of one token list (the arithmetic of tests/test_gpu_engine.py _oracle_decode, all positions of the
-    list at once): fp32 products over the oracle's fp16 weights Ws (O.dequant, CPU) rounded to fp16, fp32 causal softmax."""
-    H, nh = dec.hidden, dec.n_heads
-    hd, n = H // nh, len(toks)
-    lin = lambda x, W: (x.float() @ W.float()).half()
-    x = dec.embed.cpu()[torch.tensor(toks)]
-    causal = torch.ones(n, n, dtype=torch.bool).tril()
-    for ly, W in zip(dec.layers, Ws):
-        qkv = lin(O.rmsnorm_fwd(x, ly['input_norm'].cpu(), eps), W['qkv']).view(1, n, 3, nh, hd).clone()
-        O.rope_inplace(qkv[:, :, :2], torch.arange(n)[None, :], base=base)
-        q, k, v = (qkv[0, :, i].transpose(0, 1).float() for i in range(3))  # [nh, n, hd]
-        s = (q @ k.transpose(1, 2) * hd**-0.5).masked_fill(~causal, float('-inf'))
-        att = (torch.softmax(s, -1) @ v).half().transpose(0, 1).reshape(n, H)
-        x = x + lin(att, W['o'])
-        xn = O.rmsnorm_fwd(x, ly['post_norm'].cpu(), eps).float()
-        a1, a2 = xn @ W['gate'].float(), xn @ W['up'].float()
-        x = x + lin((a1 * torch.sigmoid(a1) * a2).half(), W['down'])
-    xn = O.rmsnorm_fwd(x, dec.final_norm.cpu(), eps)
-    return (xn.float() @ dec.lm_head.cpu().float().t()).half()
+    check_extend_against_stepping(dec, toks, 1791, '7b int8 extend vs stepping')
 
 
 def test_score_of_the_int8_model_matches_the_oracle():
     """Three lists in one score() call against float64 log-softmaxes of the oracle's fp16 logits, at the bound of tests/test_gpu_score.py:
     2 x 2e-2 x max|ref logits| per element."""
     dec = _model('7b-int8-g128', max_seq=16)
-    Ws = [{k: O.dequant(*(t.cpu() for t in ly[k].parts()), ly[k].bits) for k in ('qkv', 'o', 'gate', 'up', 'down')} for ly in dec.layers]
     g = torch.Generator().manual_seed(8)
     seqs = [torch.randint(0, VOCAB, (n, ), generator=g).tolist() for n in (9, 2, 23)]
     out = dec.score(seqs)
-    for s, lp in zip(seqs, out):
-        logits = _oracle_sequence_logits(dec, Ws, s)[:-1].double()
-        ref = torch.log_softmax(logits, -1).gather(1, torch.tensor(s[1:])[:, None])[:, 0]
-        bound = 2 * 2e-2 * logits.abs().amax(-1)
-        ratio = ((lp.cpu().double() - ref).abs() / bound).max().item()
-        report(ratio, f'score 7b int8 n={len(s)}')
-        note('score 7b int8', ratio)
+    note('score 7b int8', check_scores(out, seqs, LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0), 'score 7b int8'))
 
 
 def _int8_down_proj(M=300):
@@ -735,7 +636,6 @@ def test_int8_quant_linear_backward_at_down_proj(ops, routes):
     """M = 300: the backward makes one 8-bit transposed request with the groupsize hint, which runs on qlinear_transpose_generic_kernel<8, 2>
     (routing probe), and x.grad is within the transposed bound of the fp64 product go . W^T, W = ops.dequant of the stored tensors (pinned
     to the oracle above)."""
-    from test_gpu_backward import recorded_transposes
     assert_route(routes, 'int8 backward', generic_t(8))
     ql, x, go = _int8_down_proj()
     N = ql.outfeatures

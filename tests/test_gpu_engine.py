@@ -1,52 +1,12 @@
-"""GPU: the decode engine (gptq_llama_decode_step through the C ABI, CUDA-graph replayed) against a
-token-by-token reference composed from the CPU oracle's ops."""
+"""GPU: the decode engine (gptq_llama_decode_step through the C ABI, CUDA-graph replayed) against the CPU reference decoder
+(tests/llama_oracle.py)."""
 import pytest
 import torch
 
-from oracle import gptq_oracle as O
-from gpu_util import assert_rel_close
-from test_gpu_modules import CODELLAMA, LLAMA1, scale_down_embedding_row
+from gpu_util import assert_rel_close, tiny_quant_llama
+from llama_oracle import CODELLAMA, LLAMA1, LlamaOracle, scale_down_embedding_row
 
 pytestmark = pytest.mark.gpu
-
-
-def _oracle_decode(dec, token_ids, eps=1e-6, base=10000.0):
-    """Reference: same math as the reference's decoder layer over its kernels, evaluated with the oracle on the CPU, at the RMSNorm epsilon
-    and RoPE base the caller chose (never the decoder's own settings: a decoder built with the wrong ones would agree with itself)."""
-    H, nh = dec.hidden, dec.n_heads
-    hd = H // nh
-    cpu = lambda t: t.detach().cpu()
-    layers = []
-    for ly in dec.layers:
-        layers.append({k: ((cpu(v.qweight), cpu(v.scales), cpu(v.qzeros), cpu(v.g_idx)), v.bits) for k, v in ly.items() if hasattr(v, 'qweight')} |
-                      {'input_norm': cpu(ly['input_norm']), 'post_norm': cpu(ly['post_norm'])})
-    embed, fnorm, head = cpu(dec.embed), cpu(dec.final_norm), cpu(dec.lm_head)
-    kc = [[] for _ in layers]
-    vc = [[] for _ in layers]
-    outs = []
-    for pos, tok in enumerate(token_ids):
-        x = embed[tok][None, :].clone()
-        for li, ly in enumerate(layers):
-            (w, bits) = ly['qkv']
-            qkv = O.qlinear_fwd(O.rmsnorm_fwd(x, ly['input_norm'], eps), *w, bits).view(1, 1, 3, nh, hd).clone()
-            O.rope_inplace(qkv[:, :, :2], torch.tensor([[pos]]), base=base)
-            q, k, v = qkv[0, 0, 0], qkv[0, 0, 1], qkv[0, 0, 2]
-            kc[li].append(k.clone())
-            vc[li].append(v.clone())
-            K = torch.stack(kc[li], 1).float()  # [nh, T, hd]
-            V = torch.stack(vc[li], 1).float()
-            s = torch.einsum('hd,htd->ht', q.float(), K) * hd**-0.5
-            p = torch.softmax(s, -1)
-            att = torch.einsum('ht,htd->hd', p, V).half().reshape(1, H)
-            (w, bits) = ly['o']
-            x = x + O.qlinear_fwd(att, *w, bits)
-            (wg, bits), (wu, _) = ly['gate'], ly['up']
-            hmid = O.fused_mlp_fwd(O.rmsnorm_fwd(x, ly['post_norm'], eps), wg, wu, bits)
-            (w, bits) = ly['down']
-            x = x + O.qlinear_fwd(hmid, *w, bits)
-        xn = O.rmsnorm_fwd(x, fnorm, eps)
-        outs.append((xn.float() @ head.float().t()).half()[0])
-    return torch.stack(outs)
 
 
 DECODE_CASES = [('tiny', 4, False, True), ('tiny', 4, False, False), ('tiny', 4, True, True), ('tiny', 8, False, True), ('tiny', 3, True, True),
@@ -75,7 +35,7 @@ def test_decode_steps_match_oracle(size, bits, act, use_graph, rope):
     toks = torch.randint(0, 512, (6, ), generator=gen).tolist()
     if rope != LLAMA1:
         scale_down_embedding_row(dec.embed, toks[0], 8)
-    ref = _oracle_decode(dec, toks, eps=eps, base=base)
+    ref = LlamaOracle.from_decoder(dec, eps=eps, base=base).logits(toks)
     for pos, tok in enumerate(toks):
         dec.tokens.fill_(tok)
         dec.positions.fill_(pos)
@@ -94,9 +54,8 @@ def test_hf_checkpoint_groupsizes_decode_on_the_persistent_kernel(gs, rope):
     embedding row is scaled to a mean square of about 1.6e-6 (HF's init has std 0.02) so that the epsilon shows in the output."""
     import quant
     from gptq_b200 import engine
-    from test_gpu_modules import _tiny_quant_llama
     base, eps = rope
-    model = _tiny_quant_llama(gs=gs, hidden=256, intermediate=768, heads=2, rope_theta=base, rms_norm_eps=eps)
+    model = tiny_quant_llama(gs=gs, hidden=256, intermediate=768, heads=2, rope_theta=base, rms_norm_eps=eps)
     toks = torch.randint(0, model.config.vocab_size, (6, ), generator=torch.Generator().manual_seed(gs + 2)).tolist()
     if rope != LLAMA1:
         scale_down_embedding_row(model.model.embed_tokens.weight, toks[0], 4)
@@ -110,7 +69,7 @@ def test_hf_checkpoint_groupsizes_decode_on_the_persistent_kernel(gs, rope):
         for name in ('qkv', 'o', 'gate', 'up', 'down'):
             K = kl[name].g_idx.numel()
             assert kl[name].hint == (K if gs == -1 else gs), f'{name}: groupsize hint {kl[name].hint}'
-    ref = _oracle_decode(dec, toks, eps=eps, base=base)
+    ref = LlamaOracle.from_decoder(dec, eps=eps, base=base).logits(toks)
     for pos, tok in enumerate(toks):
         dec.set_input(tok, pos)
         dec.step()
@@ -125,7 +84,7 @@ def test_long_context_attention_splits(size):
     from gptq_b200 import engine
     dec = engine.synthetic_llama(size, bits=4, groupsize=128, vocab=256, seed=1, max_seq=640)
     toks = torch.randint(0, 256, (530, ), generator=torch.Generator().manual_seed(1)).tolist()
-    ref = _oracle_decode(dec, toks)
+    ref = LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0).logits(toks)
     for pos, tok in enumerate(toks):
         dec.tokens.fill_(tok)
         dec.positions.fill_(pos)

@@ -3,7 +3,7 @@
 The small-model tests (test_gpu_engine.py) cannot reach the stream-K ranges, attention unit splits, ring wrap-arounds and
 staging sizes of the 7B / 13B configurations, so here the kernel runs LLaMA-7B-shaped (int4 g128, BASELINE config 2) and
 LLaMA-13B-shaped (int3 g128 act-order, config 4) layers -- two of them, which exercises every inter-layer hand-off -- on a
-randomly filled KV cache at the context positions {0, 255, 256, 2046, 2047}, against the oracle (oracle/gptq_oracle.py); and 7B at
+randomly filled KV cache at the context positions {0, 255, 256, 2046, 2047}, against the oracle (tests/llama_oracle.py); and 7B at
 the groupsizes 32, 1024 and -1 (one group per linear) at the positions {0, 2047}.  LLaMA-65B-shaped layers (int4 g128, bench.py
 --config 65b: hidden 8192, the kernel's limit) run at the same five positions, LLaMA-33B-shaped ones at gs 1024 (every linear ends in a
 partial group of 512) at {0, 2047}.
@@ -20,127 +20,17 @@ end-to-end bound on the logits against the oracle run from the embedding.
 import pytest
 import torch
 
-from oracle import cref
-from oracle import gptq_oracle as O
-from attn_probe import resid_buffers
-from gpu_util import assert_rel_close
+from llama_oracle import END_TO_END_TOL, LlamaOracle, assert_no_failures, check, check_last_layer_blocks, scale_down_embedding_row
 
 pytestmark = pytest.mark.gpu
-
-FAILURES = []
-
-
-def check(out, ref, rel, what):
-    """assert_rel_close, but every check of a test case is evaluated and reported (worst error / bound) before the case fails."""
-    try:
-        assert_rel_close(out, ref, rel=rel, what=what)
-    except AssertionError as e:
-        FAILURES.append(str(e))
-
-Q = cref if cref.available() else O  # same arithmetic; the C/OpenMP restatement is just faster at 7B shapes
-
-
-class Exact:
-    """QuantLinear with the weights dequantised exactly ((w - z) * s in fp32), fp32 accumulation, one fp16 rounding: the product the
-    persistent kernel computes (it applies scale and zero per group on the fp32 accumulator).  The attention block is checked against it
-    because a softmax over 2048 keys amplifies one-ulp changes in q: at context 2047 of the 7B case the reference's per-weight fp16
-    rounding of the qkv weights alone moves the block by twice ATTN_BLOCK_TOL.  Each QuantLinear is held to the reference's rounding
-    within 1e-3 by tests/test_gpu_parity.py and tests/test_gpu_modules.py, and the appended K / V rows below are held to it here (the K
-    rows of the groupsize -1 case excepted, see _run_case) as well as to Exact."""
-
-    @staticmethod
-    def qlinear_fwd(x, qweight, scales, qzeros, g_idx, bits):
-        w = torch.from_numpy(O.unpack_rows(qweight.numpy(), bits))
-        z = torch.from_numpy(O.unpack_cols(qzeros.numpy(), bits)) + 1
-        g = g_idx.long()
-        W = (w - z[g]).float() * scales[g].float()
-        return (x.reshape(-1, x.shape[-1]).float() @ W).half().reshape(x.shape[:-1] + (W.shape[1], ))
-
-# Every QuantLinear output alone is held to 1e-3 (tests/test_gpu_modules.py, test_gpu_parity.py).  A block chains 3-5 such
-# operations with an fp16 rounding after each (one fp16 ulp is up to 9.8e-4 relative), hence the 1e-3-class block bounds:
-ATTN_BLOCK_TOL = 4e-3     # qkv -> RoPE -> attention -> o_proj -> residual add
-KV_ROW_TOL = 2.5e-3       # qkv -> RoPE (one QuantLinear + one rotation, each rounded to fp16)
-MLP_HEAD_TOL = 5e-3       # gate/up -> SwiGLU -> down -> residual -> final norm -> lm_head
-END_TO_END_TOL = 1.5e-2   # whole step from the embedding: sanity only (see the module docstring)
-
-
-def _cpu_layer(ly):
-    cpu = lambda t: t.detach().cpu()
-    d = {k: ((cpu(v.qweight), cpu(v.scales), cpu(v.qzeros), cpu(v.g_idx)), v.bits) for k, v in ly.items() if hasattr(v, 'qweight')}
-    d['input_norm'], d['post_norm'] = cpu(ly['input_norm']), cpu(ly['post_norm'])
-    return d
-
-
-def _cpu_layers(dec):
-    return [_cpu_layer(ly) for ly in dec.layers]
-
-
-def oracle_attn_block(dec, ly, x, pos, kc_l, vc_l, Q=Q, eps=1e-6, base=10000.0):
-    """x [1, H] entering a layer -> (x after the attention block, new k rows [nh, hd], new v rows); cache rows [0, pos) of the layer."""
-    H, nh = dec.hidden, dec.n_heads
-    hd = H // nh
-    (w, bits) = ly['qkv']
-    qkv = Q.qlinear_fwd(O.rmsnorm_fwd(x, ly['input_norm'], eps), *w, bits).view(1, 1, 3, nh, hd).clone()
-    O.rope_inplace(qkv[:, :, :2], torch.tensor([[pos]]), base=base)
-    q, k, v = qkv[0, 0, 0], qkv[0, 0, 1], qkv[0, 0, 2]
-    K = torch.cat([kc_l[0, :, :pos], k[:, None, :]], 1).float()  # [nh, pos+1, hd]
-    V = torch.cat([vc_l[0, :, :pos], v[:, None, :]], 1).float()
-    s = torch.einsum('hd,htd->ht', q.float(), K) * hd**-0.5
-    att = torch.einsum('ht,htd->hd', torch.softmax(s, -1), V).half().reshape(1, H)
-    (w, bits) = ly['o']
-    return x + Q.qlinear_fwd(att, *w, bits), k.clone(), v.clone()
-
-
-def oracle_mlp_block(ly, x, eps=1e-6):
-    (wg, bits), (wu, _) = ly['gate'], ly['up']
-    hmid = Q.fused_mlp_fwd(O.rmsnorm_fwd(x, ly['post_norm'], eps), wg, wu, bits)
-    (w, bits) = ly['down']
-    return x + Q.qlinear_fwd(hmid, *w, bits)
-
-
-def oracle_head(dec, x, eps=1e-6):
-    xn = O.rmsnorm_fwd(x, dec.final_norm.detach().cpu(), eps)
-    return (xn.float() @ dec.lm_head.detach().cpu().float().t()).half()[0]
-
-
-def _resid_buffers(dec):
-    """Row 0 of the kernel's residual ping-pong (attn_probe.resid_buffers): [0] = x entering the last layer, [1] = x after its attention."""
-    return [r[0].cpu() for r in resid_buffers(dec)]
-
-
-def _check_last_layer_blocks(dec, layers, n_layers, tok, pos, kc, vc, what, k_row_vs_reference=True, eps=1e-6, base=10000.0):
-    """Run one step of `dec` (n_layers deep, RMSNorm epsilon eps, RoPE base `base`) and check its last layer block by block from the kernel's
-    own intermediate values.  The appended K / V rows are held to Exact and to the reference's per-weight fp16 rounding (the K row to the
-    latter only with k_row_vs_reference)."""
-    dec.tokens.fill_(tok)
-    dec.positions.fill_(pos)
-    dec.step()
-    torch.cuda.synchronize()
-    x_in, x_attn = _resid_buffers(dec)
-    li = n_layers - 1
-    if n_layers == 1:  # the input of layer 0 is the embedding row, exactly
-        assert torch.equal(x_in, dec.embed[tok].cpu()), f'{what}: residual entering layer 0 is not the embedding row'
-    _, k_new, v_new = oracle_attn_block(dec, layers[li], x_in[None, :], pos, kc[li], vc[li], eps=eps, base=base)
-    ref_attn, k_ex, v_ex = oracle_attn_block(dec, layers[li], x_in[None, :], pos, kc[li], vc[li], Q=Exact, eps=eps, base=base)
-    check(x_attn, ref_attn[0], rel=ATTN_BLOCK_TOL, what=f'{what}: attention block of layer {li}')
-    if k_row_vs_reference:
-        check(dec.k_cache[li, 0, :, pos], k_new, rel=KV_ROW_TOL, what=f'{what}: appended K row, layer {li}')
-    check(dec.v_cache[li, 0, :, pos], v_new, rel=KV_ROW_TOL, what=f'{what}: appended V row, layer {li}')
-    check(dec.k_cache[li, 0, :, pos], k_ex, rel=KV_ROW_TOL, what=f'{what}: appended K row vs Exact, layer {li}')
-    check(dec.v_cache[li, 0, :, pos], v_ex, rel=KV_ROW_TOL, what=f'{what}: appended V row vs Exact, layer {li}')
-    ref_logits = oracle_head(dec, oracle_mlp_block(layers[li], x_attn[None, :], eps), eps)
-    check(dec.logits[0], ref_logits, rel=MLP_HEAD_TOL, what=f'{what}: MLP block of layer {li} + lm_head')
-    assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
-    return dec.logits[0].float().cpu()
 
 
 def _run_case(size, bits, act, positions, vocab, seed, gs=128, max_seq=2048, rms_eps=1e-6, rope_base=10000.0, small_embedding=False,
               k_row_vs_reference=True):
     """Both decoders and every oracle call take max_seq, rms_eps and rope_base from the arguments.  small_embedding: the token of the first
     position has its embedding row scaled by 2^-8 (mean square about 4e-6, near the epsilon), so that the 1-layer checks see the epsilon.
-    k_row_vs_reference=False holds the appended K rows to Exact only (see the comment in the loop)."""
+    k_row_vs_reference=False holds the appended K rows to the exact linears only (see the comment in the loop)."""
     from gptq_b200 import engine
-    from test_gpu_modules import scale_down_embedding_row
     dec2 = engine.synthetic_llama(size, bits=bits, groupsize=gs, act_order=act, vocab=vocab, seed=seed, max_seq=max_seq, n_layers=2, rms_eps=rms_eps,
                                   rope_base=rope_base)
     assert dec2.launches_per_step() == 1, 'the persistent kernel must be the path under test'
@@ -155,7 +45,7 @@ def _run_case(size, bits, act, positions, vocab, seed, gs=128, max_seq=2048, rms
     dec2.k_cache.copy_((torch.randn(dec2.k_cache.shape, device=dec2.dev, generator=gen) * 0.5).half())
     dec2.v_cache.copy_((torch.randn(dec2.v_cache.shape, device=dec2.dev, generator=gen) * 0.5).half())
     kc, vc = dec2.k_cache.cpu(), dec2.v_cache.cpu()
-    layers = _cpu_layers(dec2)
+    oracle = LlamaOracle.from_decoder(dec2, eps=rms_eps, base=rope_base)
     for i, pos in enumerate(positions):
         tok = (17 * i + 3) % vocab
         what = f'{size} int{bits} g{gs} act={act} eps={rms_eps:g} base={rope_base:g} pos={pos}'
@@ -168,18 +58,17 @@ def _run_case(size, bits, act, positions, vocab, seed, gs=128, max_seq=2048, rms
         # 9.2890625, the nearest fp16; reference rounding 9.296875).  That case holds its K rows to Exact only, and so does the LLaMA-2-13B
         # case: at context 4095, layer 0, one K-row element is 1.05 of its bound from the reference rounding (|err| 2.93e-3, row rms 1.12)
         # while the whole row stays within 0.39 of its bound from Exact.
-        kw = dict(k_row_vs_reference=k_row_vs_reference and gs != -1, eps=rms_eps, base=rope_base)
-        _check_last_layer_blocks(dec1, layers, 1, tok, pos, kc, vc, what + ' (1 layer)', **kw)
-        logits2 = _check_last_layer_blocks(dec2, layers, 2, tok, pos, kc, vc, what + ' (2 layers)', **kw)
+        k_row = k_row_vs_reference and gs != -1
+        check_last_layer_blocks(dec1, oracle, tok, pos, kc, vc, what + ' (1 layer)', k_row)
+        logits2 = check_last_layer_blocks(dec2, oracle, tok, pos, kc, vc, what + ' (2 layers)', k_row)
         # end to end from the embedding
         x = dec2.embed[tok].cpu()[None, :].clone()
         for li in range(2):
-            x = oracle_mlp_block(layers[li], oracle_attn_block(dec2, layers[li], x, pos, kc[li], vc[li], eps=rms_eps, base=rope_base)[0], rms_eps)
-        check(logits2, oracle_head(dec2, x, rms_eps), rel=END_TO_END_TOL, what=what + ': logits after 2 layers, end to end')
+            x = oracle.mlp(li, oracle.attention(li, x, pos, kc[li, 0], vc[li, 0])[0])
+        check(logits2, oracle.head(x)[0], rel=END_TO_END_TOL, what=what + ': logits after 2 layers, end to end')
         dec2.k_cache.copy_(kc)  # every position starts from the same cache
         dec2.v_cache.copy_(vc)
-    failed, FAILURES[:] = list(FAILURES), []
-    assert not failed, '\n'.join(failed)
+    assert_no_failures()
 
 
 def test_mega_kernel_7b_int4_g128_matches_oracle():

@@ -14,60 +14,23 @@ import pytest
 import torch
 
 import exact_fixtures as X
-from gpu_util import fp16_from_fp64, fp16_ulp_distance, run_kernel
-from oracle import gptq_oracle as O
+from gpu_util import GEMM_1, GEMM_2, GEMM_DUAL, MATVEC, MATVEC_DUAL, Layer, assert_equal, cyclic, fp16_from_fp64, fp16_ulp_distance, generic, ops, \
+    run_kernel
 
 pytestmark = pytest.mark.gpu
-
-MATVEC, MATVEC_DUAL = 'qmatvec_int4_kernel<false>', 'qmatvec_int4_kernel<true>'
-GEMM_1, GEMM_2, GEMM_DUAL = 'qgemm_wgmma_kernel<false, 1, 6>', 'qgemm_wgmma_kernel<false, 2, 4>', 'qgemm_wgmma_kernel<true, 1, 4>'
-
-
-def generic(bits, M, dual=False):
-    return f'qlinear_generic_kernel<{bits}, {M if M <= 2 else 4}, {str(dual).lower()}>'
-
 
 def gemm_kernel(M):
     return GEMM_2 if M > 128 else GEMM_1
 
 
-@pytest.fixture(scope='module')
-def ops():
-    from gptq_b200 import ops as _ops  # raises if libgptq_b200.so is missing: no fallback
-    return _ops
-
-
-class Layer:
-    """A packed layer on the CPU and on the device, with the oracle's fp16 weight on the device."""
-
-    def __init__(self, packed, bits, bias=None):
-        self.cpu = tuple(packed)
-        self.dev = tuple(t.cuda() for t in packed)
-        self.bits = bits
-        self.W = O.dequant(*packed, bits).cuda()
-        self.bias = bias.cuda() if bias is not None else None
-
-
 @lru_cache(maxsize=None)
 def random_layer(K, N, bits, gs, act=False, bias=False, seed=0):
-    qw, s, qz, g, b = O.random_packed(K, N, bits, gs, act_order=act, seed=seed, bias=bias)
-    return Layer((qw, s, qz, g), bits, b)
+    return Layer.random(K, N, bits, gs, act, bias, seed)
 
 
 @lru_cache(maxsize=None)
 def pow2_layer(K, N, gs, jmin=6, seed=0):
     return Layer(X.pow2_packed(K, N, gs, jmin=jmin, seed=seed), 4)
-
-
-def assert_equal(out, exp, what, locate):
-    """torch.equal, naming the first mismatching element through locate(row, n)."""
-    assert out.shape == exp.shape, (what, out.shape, exp.shape)
-    if torch.equal(out, exp):
-        return
-    bad = out != exp
-    r, n = (int(i) for i in torch.nonzero(bad)[0])
-    raise AssertionError(f'{what}: {int(bad.sum())} / {bad.numel()} outputs differ; first at {locate(r, n)}: '
-                         f'got {out[r, n].item()!r}, want {exp[r, n].item()!r}')
 
 
 def assert_ulp1(out, ref_fp64, what, locate):
@@ -87,12 +50,6 @@ def batched_calls(fn, x, M, kernel, what):
         xc = x[c * M:(c + 1) * M]
         outs.append(run_kernel(lambda: fn(xc), kernel, what) if c == 0 else fn(xc))
     return torch.cat(outs)
-
-
-def cyclic(ks, M):
-    """ks padded (cyclically) to a multiple of M."""
-    ks = list(ks)
-    return ks + ks[:(-len(ks)) % M]
 
 
 # ============================================================================= one-hot rows: every path

@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from gpu_util import assert_rel_close, run_kernel
+from llama_oracle import check_extend_against_stepping, step_all
 
 pytestmark = pytest.mark.gpu
 
@@ -18,13 +19,6 @@ def _model(size, bits, act, seed, gs=64, **kw):
 
 def _ids(n, seed):
     return torch.randint(0, 300, (n, ), generator=torch.Generator().manual_seed(seed)).tolist()
-
-
-def _step_all(dec, toks, start):
-    for i, t in enumerate(toks):
-        dec.set_input(t, start + i)
-        dec.step()
-    torch.cuda.synchronize()
 
 
 @pytest.mark.parametrize('size, bits, act, rope_base, cached', [pytest.param(*m, 10000.0, 10, id='-'.join(map(str, m))) for m in MODELS] +
@@ -49,12 +43,12 @@ def test_extend_after_decode_at_groupsizes(gs, kernel):
 def _extend_after_decode(dec, kernel=None, what='', cached=10):
     c, e = cached, cached + 29
     prompt = _ids(e + 1, 2)
-    _step_all(dec, prompt, 0)
+    step_all(dec, prompt, 0)
     ref_logits, ref_k, ref_v = dec.logits[0].float().clone(), dec.k_cache[:, 0, :, :e + 1].float().clone(), dec.v_cache[:, 0, :, :e + 1].float().clone()
     dec.reset()
     dec.k_cache.zero_()
     dec.v_cache.zero_()
-    _step_all(dec, prompt[:c], 0)
+    step_all(dec, prompt[:c], 0)
     assert dec.lengths == [c] and dec.cached_tokens == [prompt[:c]]
 
     def extend():  # repeatable (run_kernel may trace it again): from the c cached positions each time
@@ -204,16 +198,4 @@ def test_llama_7b_shapes_extend_256_at_1791():
     dec = engine.synthetic_llama('7b', bits=4, groupsize=128, vocab=32000, seed=15, max_seq=2048, n_layers=2)
     assert dec.launches_per_step() == 1
     toks = torch.randint(0, 32000, (2048, ), generator=torch.Generator().manual_seed(5)).tolist()
-    _step_all(dec, toks[:1791], 0)
-    assert dec.extend([toks[1791:2047]]) == [2047]
-    dec.set_input(toks[2047], 2047)
-    dec.step()
-    torch.cuda.synchronize()
-    got = [dec.logits[0].float().clone(), dec.k_cache[:, 0, :, 1791:2047].float().clone(), dec.v_cache[:, 0, :, 1791:2047].float().clone()]
-    _step_all(dec, toks[1791:], 1791)
-    ref = [dec.logits[0].float(), dec.k_cache[:, 0, :, 1791:2047].float(), dec.v_cache[:, 0, :, 1791:2047].float()]
-    for what, g, r in zip(('logits', 'K rows', 'V rows'), got, ref):
-        rms = r.pow(2).mean().sqrt().item()
-        d = (g - r).abs()
-        print(f'  {what}: max |diff| / rms = {d.max().item() / rms:.3g}, rms diff / rms = {d.pow(2).mean().sqrt().item() / rms:.3g}')
-        assert d.max().item() <= 1.5e-2 * rms and d.pow(2).mean().sqrt().item() <= 3e-3 * rms, what
+    check_extend_against_stepping(dec, toks, 1791, '7b extend')

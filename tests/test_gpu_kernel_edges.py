@@ -20,53 +20,24 @@ import pytest
 import torch
 
 import exact_fixtures as X
-from gpu_util import check_fp64_bound, check_swiglu_fp64_bound, run_kernel
-from oracle import gptq_oracle as O
+from gpu_util import GEMM_1, GEMM_2, GEMM_DUAL, GENERIC_4, MATVEC, MATVEC_DUAL, Layer, WorstRatios, check_fp64_bound, check_swiglu_fp64_bound, ops, randn_x, \
+    run_kernel
 
 pytestmark = pytest.mark.gpu
 
-MATVEC, MATVEC_DUAL = 'qmatvec_int4_kernel<false>', 'qmatvec_int4_kernel<true>'
-GEMM_1, GEMM_2, GEMM_DUAL = 'qgemm_wgmma_kernel<false, 1, 6>', 'qgemm_wgmma_kernel<false, 2, 4>', 'qgemm_wgmma_kernel<true, 1, 4>'
-GENERIC_4 = 'qlinear_generic_kernel<4, 4, false>'
-
-WORST = {}  # sweep -> worst |err| / bound, printed at the end of the module (pytest -s)
+WORST = WorstRatios()
+note = WORST.note
 
 
 @pytest.fixture(scope='module', autouse=True)
 def worst_ratio_summary():
     yield
-    for sweep, r in WORST.items():
-        print(f'worst |err| / bound, {sweep}: {r:.3g}')
-
-
-def note(sweep, ratio):
-    WORST[sweep] = max(WORST.get(sweep, 0.0), ratio)
-
-
-@pytest.fixture(scope='module')
-def ops():
-    from gptq_b200 import ops as _ops  # raises if libgptq_b200.so is missing: no fallback
-    return _ops
-
-
-class Layer:
-
-    def __init__(self, K, N, gs, bias, seed):
-        qw, s, qz, g, b = O.random_packed(K, N, 4, gs, seed=seed, bias=bias)
-        self.dev = tuple(t.cuda() for t in (qw, s, qz, g))
-        self.W = O.dequant(qw, s, qz, g, 4).cuda()  # the oracle's fp16 weight, built on the CPU once per shape
-        self.bias = b.cuda() if b is not None else None
+    WORST.summary()
 
 
 @lru_cache(maxsize=None)
 def layer(K, N, gs, bias=False, seed=0):
-    return Layer(K, N, gs, bias, seed)
-
-
-def randn_x(M, K, seed, ld=None):
-    """fp16 [M, K] ~ N(0, 1) on the device; with ld, a column slice of an [M, ld] buffer (row stride ld)."""
-    buf = torch.randn(M, ld or K, generator=torch.Generator().manual_seed(seed)).half().cuda()
-    return buf[:, :K]
+    return Layer.random(K, N, 4, gs, bias=bias, seed=seed)
 
 
 def workspace_counters(ops, dev, N):

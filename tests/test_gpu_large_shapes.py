@@ -14,34 +14,25 @@ reference weight is formed from the same integers in torch as the reference's ma
 fp16, times the fp16 scale, one rounding).  Every kernel case asserts which kernel served it.  The two engine cases take no trace: a
 torch.profiler session around a 65B extend or score left later sessions of the test process with kernel records missing
 (tests/test_gpu_launches.py); the kernel cases above cover their batched linears at the same shapes."""
-import math
 from functools import lru_cache
 
 import pytest
 import torch
 
-from gpu_util import check_fp64_bound, check_swiglu_fp64_bound, report, run_kernel
-from test_gpu_cached_attention import check as check_attention
-from test_gpu_cached_attention import make_cache
-from test_gpu_cached_attention import run as run_attention
-from test_gpu_extend import _step_all
-from test_gpu_kernel_edges import GEMM_1, GEMM_2, GEMM_DUAL, GENERIC_4, MATVEC, MATVEC_DUAL, randn_x
-from test_gpu_score import _random, check_logprob
+from gpu_util import GEMM_1, GEMM_2, GEMM_DUAL, GENERIC_4, MATVEC, MATVEC_DUAL, WorstRatios, check_cached_attention, check_fp64_bound, check_logprob, \
+    check_swiglu_fp64_bound, make_kv_cache, random_logprob_inputs, randn_x, report, run_cached_attention, run_kernel
+from llama_oracle import LlamaOracle, check_extend_against_stepping, check_scores
 
 pytestmark = pytest.mark.gpu
 
-WORST = {}
+WORST = WorstRatios()
+note = WORST.note
 
 
 @pytest.fixture(scope='module', autouse=True)
 def worst_ratio_summary():
     yield
-    for sweep, r in WORST.items():
-        print(f'worst |err| / bound, {sweep}: {r:.3g}')
-
-
-def note(sweep, ratio):
-    WORST[sweep] = max(WORST.get(sweep, 0.0), ratio)
+    WORST.summary()
 
 
 class Layer:
@@ -153,7 +144,7 @@ def test_matvec_partials_do_not_leak_into_the_next_call():
         torch.cuda.synchronize()
         assert workspace_is_zero(ops, x.device), f'{what}: workspace left non-zero'
         note('matvec', check_fp64_bound(out, x, L.W, what=what))
-    xl, W, t = _random(300, 1000, 8192, seed=3)
+    xl, W, t = random_logprob_inputs(300, 1000, 8192, seed=3)
     check_logprob(ops.lm_head_logprob(xl, W, t), xl, W, t, 'lm_head_logprob after the matvecs')
 
 
@@ -161,7 +152,7 @@ def test_matvec_partials_do_not_leak_into_the_next_call():
 @pytest.mark.parametrize('K', [8192, 6656])
 def test_lm_head_logprob(K):
     from gptq_b200 import ops
-    x, W, t = _random(2048, 32000, K, seed=K)
+    x, W, t = random_logprob_inputs(2048, 32000, K, seed=K)
     lp = ops.lm_head_logprob(x, W, t)
     check_logprob(lp, x, W, t, f'lm_head_logprob M=2048 V=32000 K={K}')
 
@@ -171,9 +162,9 @@ def test_lm_head_logprob(K):
 def test_cached_attention(nh):
     """128 rows at start 1920 (the span ends at the last cache row) next to a ragged second sequence, then a ragged call of four spans."""
     for spans in ([(0, 1920, 128), (1, 700, 77)], [(0, 0, 300), (1, 1000, 129), (2, 63, 1), (3, 1919, 129)]):
-        q, kc, vc = make_cache(len(spans), nh, 2048, spans, seed=nh + len(spans), layers=2, layer=1)
-        out = run_attention(q, kc, vc, spans)
-        note(f'cached attention, {nh} heads', check_attention(out, q, kc[1], vc[1], spans, f'{nh} heads {spans}'))
+        q, kc, vc = make_kv_cache(len(spans), nh, 2048, spans, seed=nh + len(spans), layers=2, layer=1)
+        out = run_cached_attention(q, kc, vc, spans)
+        note(f'cached attention, {nh} heads', check_cached_attention(out, q, kc[1], vc[1], spans, f'{nh} heads {spans}'))
         del q, kc, vc
     report(WORST[f'cached attention, {nh} heads'], f'cached attention, {nh} heads')
 
@@ -186,45 +177,7 @@ def test_extend_65b_against_stepping():
     dec = engine.synthetic_llama('65b', bits=4, groupsize=128, vocab=32000, seed=15, max_seq=2048, n_layers=2)
     assert dec.launches_per_step() == 1
     toks = torch.randint(0, 32000, (2048, ), generator=torch.Generator().manual_seed(5)).tolist()
-    _step_all(dec, toks[:1791], 0)
-    assert dec.extend([toks[1791:2047]]) == [2047]
-    dec.set_input(toks[2047], 2047)
-    dec.step()
-    torch.cuda.synchronize()
-    got = [dec.logits[0].float().clone(), dec.k_cache[:, 0, :, 1791:2047].float().clone(), dec.v_cache[:, 0, :, 1791:2047].float().clone()]
-    _step_all(dec, toks[1791:], 1791)
-    ref = [dec.logits[0].float(), dec.k_cache[:, 0, :, 1791:2047].float(), dec.v_cache[:, 0, :, 1791:2047].float()]
-    for what, g, r in zip(('logits', 'K rows', 'V rows'), got, ref):
-        rms = r.pow(2).mean().sqrt().item()
-        d = (g - r).abs()
-        print(f'  65b extend {what}: max |diff| / rms = {d.max().item() / rms:.3g}, rms diff / rms = {d.pow(2).mean().sqrt().item() / rms:.3g}')
-        assert d.max().item() <= 1.5e-2 * rms and d.pow(2).mean().sqrt().item() <= 3e-3 * rms, what
-
-
-def _oracle_logits(dec, seqs):
-    """The oracle's fp16 logits at every position of each sequence: test_gpu_engine._oracle_decode's arithmetic (the oracle's fp16 weights,
-    fp32 accumulation, the same fp16 rounding points), with every position of a sequence in one pass and each layer dequantised once."""
-    from oracle import gptq_oracle as O
-    H, nh = dec.hidden, dec.n_heads
-    hd = H // nh
-    cpu = lambda t: t.detach().cpu()
-    lin = lambda x, W: (x.float() @ W.float()).half()
-    xs = [cpu(dec.embed)[torch.tensor(s)] for s in seqs]
-    for ly in dec.layers:
-        W = {k: O.dequant(cpu(ly[k].qweight), cpu(ly[k].scales), cpu(ly[k].qzeros), cpu(ly[k].g_idx), ly[k].bits) for k in ('qkv', 'o', 'gate', 'up', 'down')}
-        for i, x in enumerate(xs):
-            T = x.shape[0]
-            qkv = lin(O.rmsnorm_fwd(x, cpu(ly['input_norm']), 1e-6), W['qkv']).view(1, T, 3, nh, hd).clone()
-            O.rope_inplace(qkv[:, :, :2], torch.arange(T)[None, :])
-            q, k, v = (qkv[0, :, j].transpose(0, 1).float() for j in range(3))  # [nh, T, hd]
-            sc = (q @ k.transpose(1, 2)) * hd**-0.5
-            sc = sc.masked_fill(torch.ones(T, T, dtype=torch.bool).triu(1), -math.inf)
-            att = (torch.softmax(sc, -1) @ v).half().transpose(0, 1).reshape(T, H)
-            x = x + lin(att, W['o'])
-            xn = O.rmsnorm_fwd(x, cpu(ly['post_norm']), 1e-6).float()
-            a1, a2 = xn @ W['gate'].float(), xn @ W['up'].float()
-            xs[i] = x + lin((a1 * torch.sigmoid(a1) * a2).half(), W['down'])
-    return [lin(O.rmsnorm_fwd(x, cpu(dec.final_norm), 1e-6), cpu(dec.lm_head).t()) for x in xs]
+    check_extend_against_stepping(dec, toks, 1791, '65b extend')
 
 
 def test_score_65b_against_the_oracle():
@@ -236,8 +189,4 @@ def test_score_65b_against_the_oracle():
     seqs = [torch.randint(0, 300, (n, ), generator=g).tolist() for n in (9, 2, 23)]
     out = dec.score(seqs)
     assert [o.shape[0] for o in out] == [8, 1, 22]
-    for s, lp, logits in zip(seqs, out, _oracle_logits(dec, seqs)):
-        logits = logits[:-1].double()
-        ref = torch.log_softmax(logits, -1).gather(1, torch.tensor(s[1:])[:, None])[:, 0]
-        bound = 2 * 2e-2 * logits.abs().amax(-1)
-        report(((lp.cpu().double() - ref).abs() / bound).max().item(), f'65b score n={len(s)}')
+    check_scores(out, seqs, LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0), '65b score')

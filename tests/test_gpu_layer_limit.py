@@ -7,15 +7,14 @@ A LLaMA-65B-shaped stack (hidden 8192, 64 heads) that needs the memory of about 
 Inputs are the probe's embedding rows with rms_eps = 0 and unit norms, at position 0.  Then x entering the last layer is the embedding row
 bit for bit, and every aliased layer appends the probe's exact K / V rows (gs_probe.Expect.k / .v) to its own cache slice: the probe's sums
 are exact in fp32, so these rows do not depend on the order in which the split-K atomics add.  The last layer is checked block by block
-(test_gpu_engine_fullsize._check_last_layer_blocks) on the persistent kernel; on the chain, which keeps no x after attention, its logits are
+(llama_oracle.check_last_layer_blocks) on the persistent kernel; on the chain, which keeps no x after attention, its logits are
 held to the oracle run from the (exact) embedding row at the MLP block's bound."""
 import pytest
 import torch
 
 import gs_probe as P
 from attn_probe import resid_buffers
-from test_gpu_engine_fullsize import (FAILURES, MLP_HEAD_TOL, Exact, _check_last_layer_blocks, _cpu_layer, check, oracle_attn_block, oracle_head,
-                                      oracle_mlp_block)
+from llama_oracle import MLP_HEAD_TOL, LlamaOracle, assert_no_failures, check, check_last_layer_blocks
 
 pytestmark = pytest.mark.gpu
 
@@ -61,12 +60,12 @@ def test_persistent_kernel_at_80_layers_and_chain_at_81():
     L, ly, last, final_norm, lm_head = _stack()
     dev = torch.device('cuda:0')
     E = P.Expect(L, P.embed_rows(P.VOCAB, L.H)[torch.tensor([TOK])], device=dev)
-    layers = [None] * (MAX_LAYERS - 1) + [_cpu_layer(last)]
 
     dec = _decoder(ly, last, final_norm, lm_head, MAX_LAYERS)
     assert dec.launches_per_step() == 1, f'{MAX_LAYERS} layers: {dec.launches_per_step()} launches'
+    oracle = LlamaOracle.from_decoder(dec, eps=0.0, base=10000.0)  # only the last layer's blocks run on it
     kc, vc = dec.k_cache.cpu(), dec.v_cache.cpu()
-    _check_last_layer_blocks(dec, layers, MAX_LAYERS, TOK, 0, kc, vc, f'65b {MAX_LAYERS} layers', eps=0.0)
+    check_last_layer_blocks(dec, oracle, TOK, 0, kc, vc, f'65b {MAX_LAYERS} layers')
     x_in = resid_buffers(dec)[0][0]
     assert torch.equal(x_in, dec.embed[TOK]), 'x entering layer 79 is not the embedding row'
     _check_aliased_kv(dec, E, MAX_LAYERS - 1, f'65b {MAX_LAYERS} layers (persistent)')
@@ -79,10 +78,8 @@ def test_persistent_kernel_at_80_layers_and_chain_at_81():
     dec.step()
     torch.cuda.synchronize()
     _check_aliased_kv(dec, E, n - 1, f'65b {n} layers (kernel chain)')
-    layers81 = [None] * (n - 1) + layers[-1:]
     x = dec.embed[TOK].cpu()[None, :].clone()
-    x_attn, _, _ = oracle_attn_block(dec, layers81[-1], x, 0, kc[0], vc[0], Q=Exact, eps=0.0)
-    check(dec.logits[0], oracle_head(dec, oracle_mlp_block(layers81[-1], x_attn, 0.0), 0.0), rel=MLP_HEAD_TOL,
+    x_attn, _, _ = oracle.attention(MAX_LAYERS - 1, x, 0, exact=True)  # the last layer: the same tensors at 80 and 81 layers
+    check(dec.logits[0], oracle.head(oracle.mlp(MAX_LAYERS - 1, x_attn))[0], rel=MLP_HEAD_TOL,
           what=f'65b {n} layers (kernel chain): last layer + lm_head from the embedding row')
-    failed, FAILURES[:] = list(FAILURES), []
-    assert not failed, '\n'.join(failed)
+    assert_no_failures()

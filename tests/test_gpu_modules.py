@@ -5,23 +5,17 @@ import pytest
 import torch
 
 from oracle import gptq_oracle as O
-from gpu_util import assert_rel_close, cuda
+from gpu_util import assert_rel_close, cuda, fill_quant_linear, tiny_quant_llama
+from llama_oracle import CODELLAMA, LLAMA1, scale_down_embedding_row
 
 pytestmark = pytest.mark.gpu
-
-
-def _fill(ql, bits, seed, act=False):
-    qw, s, qz, g, b = O.random_packed(ql.infeatures, ql.outfeatures, bits, ql.groupsize, act_order=act, seed=seed, bias=ql.bias is not None)
-    ql.qweight, ql.scales, ql.qzeros, ql.g_idx = qw, s, qz, g
-    if b is not None:
-        ql.bias = b
 
 
 @pytest.mark.parametrize('bits,act', [(4, False), (4, True), (3, True), (8, False), (2, False)])
 def test_quantlinear_module_forward_and_backward(bits, act):
     import quant
     ql = quant.QuantLinear(bits, 64, 256, 128, True)
-    _fill(ql, bits, seed=bits, act=act)
+    fill_quant_linear(ql, bits, seed=bits, act=act)
     x = torch.randn(2, 3, 256, generator=torch.Generator().manual_seed(0)).half()
     ref = O.qlinear_fwd(x, ql.qweight, ql.scales, ql.qzeros, ql.g_idx, bits, ql.bias)
     ql = ql.cuda()
@@ -34,29 +28,6 @@ def test_quantlinear_module_forward_and_backward(bits, act):
     out.backward(go.cuda())
     gref = O.qlinear_transpose_fwd(go, *(t.cpu() for t in (ql.qweight, ql.scales, ql.qzeros, ql.g_idx)), bits)
     assert_rel_close(xd.grad, gref, what='module bwd')
-
-
-def _tiny_quant_llama(bits=4, gs=32, act=False, hidden=128, intermediate=352, heads=4, rope_theta=10000.0, rms_norm_eps=1e-6):
-    import quant
-    import utils
-    from transformers import LlamaConfig, LlamaForCausalLM
-    cfg = LlamaConfig(hidden_size=hidden, intermediate_size=intermediate, num_hidden_layers=2, num_attention_heads=heads, num_key_value_heads=heads,
-                      vocab_size=256, max_position_embeddings=128, rope_theta=rope_theta, rms_norm_eps=rms_norm_eps)
-    torch.manual_seed(0)
-    model = LlamaForCausalLM(cfg).half().eval()
-    layers = utils.find_layers(model)
-    layers.pop('lm_head')
-    quant.make_quant_linear(model, layers, bits, gs)
-    seed = 0
-    for name, m in model.named_modules():
-        if isinstance(m, quant.QuantLinear):
-            seed += 1
-            # q/k/v of one block share their input, hence their act-order
-            _fill(m, bits, seed, act=False)
-            if act:
-                blk = name.split('.')[2]
-                m.g_idx = O.make_g_idx(m.infeatures, gs, True, torch.Generator().manual_seed(int(blk) + m.infeatures))
-    return model
 
 
 def _ref_forward(model, ids, base, eps):
@@ -88,17 +59,6 @@ def _ref_forward(model, ids, base, eps):
     return (h.float() @ model.lm_head.weight.data.float().t())
 
 
-def scale_down_embedding_row(embed, tok, shift):
-    """Multiply embedding row `tok` by 2^-shift in place, so that its mean square comes near the RMSNorm epsilon: only then does the
-    epsilon move the first norm by more than an fp16 ulp, and a norm that used another epsilon shows in the output."""
-    with torch.no_grad():
-        embed[tok] *= 2.0**-shift
-
-
-# LLaMA-1 (RoPE base 10000, RMSNorm epsilon 1e-6) and CodeLlama (base 1e6, epsilon 1e-5)
-LLAMA1, CODELLAMA = (10000.0, 1e-6), (1e6, 1e-5)
-
-
 @pytest.mark.parametrize('bits,act,rope', [pytest.param(4, False, LLAMA1, id='4-False'), pytest.param(4, True, LLAMA1, id='4-True'),
                                            pytest.param(3, True, LLAMA1, id='3-True'), pytest.param(4, False, CODELLAMA, id='4-False-codellama')])
 def test_load_quant_pipeline_on_tiny_llama(bits, act, rope):
@@ -108,7 +68,7 @@ def test_load_quant_pipeline_on_tiny_llama(bits, act, rope):
     where epsilon 1e-5 and 1e-6 give norms a factor 2 apart."""
     import quant
     base, eps = rope
-    model = _tiny_quant_llama(bits=bits, act=act, rope_theta=base, rms_norm_eps=eps)
+    model = tiny_quant_llama(bits=bits, act=act, rope_theta=base, rms_norm_eps=eps)
     ids = torch.randint(0, 256, (1, 9), generator=torch.Generator().manual_seed(0))
     if rope != LLAMA1:
         scale_down_embedding_row(model.model.embed_tokens.weight, int(ids[0, 0]), 4)
@@ -136,7 +96,7 @@ def test_engine_and_modules_derive_the_same_kernel_form(bits):
     import quant
     from gptq_b200 import engine, ops
     gs = 32
-    model = _tiny_quant_llama(bits=bits, gs=gs, act=True, hidden=256, intermediate=768, heads=2)
+    model = tiny_quant_llama(bits=bits, gs=gs, act=True, hidden=256, intermediate=768, heads=2)
     quant.make_quant_attn(model)
     quant.make_quant_norm(model)
     quant.make_fused_mlp(model)
@@ -207,7 +167,7 @@ def test_act_order_plan_uses_tuned_kernels_and_matches_gather_path():
     import quant
     from gptq_b200 import ops
     ql = quant.QuantLinear(4, 128, 1024, 512, False)
-    _fill(ql, 4, seed=11, act=True)
+    fill_quant_linear(ql, 4, seed=11, act=True)
     x = torch.randn(3, 1024, generator=torch.Generator().manual_seed(2)).half()
     ref = O.qlinear_fwd(x, ql.qweight, ql.scales, ql.qzeros, ql.g_idx, 4)
     ql = ql.cuda()
@@ -230,7 +190,7 @@ def test_narrow_bits_are_served_by_the_int4_kernels_through_the_widened_plan(bit
     import quant
     from gptq_b200 import ops
     ql = quant.QuantLinear(bits, 128, 1024, 512, False)
-    _fill(ql, bits, seed=20 + bits, act=act)
+    fill_quant_linear(ql, bits, seed=20 + bits, act=act)
     cpu = [t.clone() for t in (ql.qweight, ql.scales, ql.qzeros, ql.g_idx)]
     ql = ql.cuda()
     plan = ql.kernel_plan()

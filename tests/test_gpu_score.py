@@ -6,58 +6,10 @@ import math
 import pytest
 import torch
 
-from gpu_util import launched_kernels, report, run_kernel, ulp16
-from test_gpu_engine import _oracle_decode
-from test_gpu_modules import CODELLAMA, LLAMA1, scale_down_embedding_row
+from gpu_util import check_logprob, launched_kernels, lse_tol, random_logprob_inputs, report, run_kernel, tiny_quant_llama
+from llama_oracle import CODELLAMA, LLAMA1, LlamaOracle, check_scores, scale_down_embedding_row
 
 pytestmark = pytest.mark.gpu
-
-U = 2.0**-24
-# fp32 part of the bound (everything after the fp16 logits).  The row's sum s = sum exp(l - max) is formed by 31 sequential adds per
-# thread, 2 quad shuffles, at most 8 per-lane merges (ceil(251 / 32) vocabulary tiles) and 5 butterfly merges, each merge 2 expf (2 ulp),
-# 2 multiplies and 1 add; with 2 ulp for the terms' expf that is <= 31 + 2 + 13 * 6 + 2 = 113 roundings of relative size 2^-24, so
-# |log s' - log s| <= 128 * 2^-24 = 7.6e-6.  The exp arguments l - max are rounded relative to their size; weighted by exp(-a) that adds at
-# most (log V + 1) 2^-24, and logf, max + log s and l_t - (...) round relative to their magnitudes: 2^-23 (|max l| + log V + |logprob|).
-LSE_EPS = 128 * U
-
-
-def lse_tol(lmax, V, ref):
-    return LSE_EPS + 2 * U * (lmax + math.log(V) + ref.abs())
-
-
-def ref_logprob(x, W, targets):
-    """float64 log-softmax of the fp16 logits fp16(x . W^T), on the GPU.  (CUDA's float64 -> fp16 cast goes through fp32, which can move a
-    logit by one fp16 ulp at a tie: the per-logit ulp terms of the bound cover it; on the integer grid every logit is exact.)"""
-    l = (x.double() @ W.double().t()).half().double()
-    lt = l.gather(1, targets.long()[:, None])[:, 0]
-    return lt - torch.logsumexp(l, -1), lt, l.abs().amax(-1)
-
-
-def check_logprob(lp, x, W, targets, what, exact=False):
-    """|logprob - ref| <= ulp16(|l_t|) + ulp16(max |l|) + lse_tol: logsumexp is 1-Lipschitz in the max-norm, so a one-ulp flip of any fp16
-    logit (fp32 summation order) moves the result by at most ulp16(max |l|), and the target's own flip by ulp16(|l_t|).  exact: the logits
-    are exact, only the fp32 log-softmax part remains."""
-    ref, lt, lmax = ref_logprob(x, W, targets)
-    tol = lse_tol(lmax, W.shape[0], ref)
-    if not exact:
-        tol = tol + ulp16(lt) + ulp16(lmax)
-    assert torch.isfinite(lp).all(), f'{what}: non-finite output'
-    ratio_t = (lp.double() - ref).abs() / tol
-    ratio = ratio_t.max().item()
-    if ratio > 1:
-        what = f'{what}: first bad row {int(torch.nonzero(ratio_t > 1)[0])}'
-    report(ratio, what)
-    return ref
-
-
-def _random(M, V, K, ldx=None, ldw=None, seed=0):
-    g = torch.Generator(device='cuda').manual_seed(seed)
-    x = torch.randn(M, ldx or K, device='cuda', generator=g).half()[:, :K]
-    W = (torch.randn(V, ldw or K, device='cuda', generator=g) * (2.5 / math.sqrt(K))).half()[:, :K]  # logits of std ~2.5
-    t = torch.randint(0, V, (M, ), device='cuda', generator=g, dtype=torch.int32)
-    t[:4] = torch.tensor([0, V - 1, min(127, V - 1), min(128, V - 1)], dtype=torch.int32)[:M]
-    return x, W, t
-
 
 # ----------------------------------------------------------------------------- the kernel
 def test_exact_anchors_on_an_integer_grid():
@@ -91,14 +43,14 @@ EDGES = ([(M, 32001, 256, None, None) for M in (1, 2, 127, 128, 129, 255, 256, 2
 @pytest.mark.parametrize('M,V,K,ldx,ldw', EDGES)
 def test_tile_edges_against_fp64(M, V, K, ldx, ldw):
     from gptq_b200 import ops
-    x, W, t = _random(M, V, K, ldx, ldw, seed=M + V + K)
+    x, W, t = random_logprob_inputs(M, V, K, ldx, ldw, seed=M + V + K)
     assert (ldx is None or x.stride(0) == ldx) and (ldw is None or W.stride(0) == ldw)
     check_logprob(ops.lm_head_logprob(x, W, t), x, W, t, f'M={M} V={V} K={K} ldx={ldx} ldw={ldw}')
 
 
 def test_deterministic_and_independent_of_the_other_rows():
     from gptq_b200 import ops
-    x, W, t = _random(4099, 32000, 4096, seed=7)
+    x, W, t = random_logprob_inputs(4099, 32000, 4096, seed=7)
     a = ops.lm_head_logprob(x, W, t)
     b = ops.lm_head_logprob(x, W, t)
     assert torch.equal(a, b)
@@ -108,7 +60,7 @@ def test_deterministic_and_independent_of_the_other_rows():
 
 def test_workspace_is_left_zeroed_and_bad_targets_are_rejected():
     from gptq_b200 import ops
-    x, W, t = _random(300, 1000, 256, seed=3)
+    x, W, t = random_logprob_inputs(300, 1000, 256, seed=3)
     ops.lm_head_logprob(x, W, t)
     torch.cuda.synchronize()
     for ws in ops._workspaces.values():
@@ -174,11 +126,7 @@ def _score_against_oracle(dec, seed, what, kernel=None, rope=LLAMA1):
         scale_down_embedding_row(dec.embed, seqs[0][0], 8)
     out = dec.score(seqs) if kernel is None else run_kernel(lambda: dec.score(seqs), kernel, f'{what}: score')
     assert [o.shape[0] for o in out] == [8, 1, 22] and all(o.dtype == torch.float32 for o in out)
-    for s, lp in zip(seqs, out):
-        logits = _oracle_decode(dec, s, eps=eps, base=base)[:-1].double()
-        ref = torch.log_softmax(logits, -1).gather(1, torch.tensor(s[1:])[:, None])[:, 0]
-        bound = 2 * 2e-2 * logits.abs().amax(-1)
-        report(((lp.cpu().double() - ref).abs() / bound).max().item(), f'{what} n={len(s)}')
+    check_scores(out, seqs, LlamaOracle.from_decoder(dec, eps=eps, base=base), what)
 
 
 def test_perplexity_matches_the_reference_formula_on_the_hf_modules():
@@ -189,8 +137,7 @@ def test_perplexity_matches_the_reference_formula_on_the_hf_modules():
     log-softmax outputs and the mean loss (|loss| < 8: half an ulp, 2^-9, each).  The mean NLL differs by at most the sum of the two."""
     import quant
     from gptq_b200 import engine
-    from test_gpu_modules import _tiny_quant_llama
-    model = _tiny_quant_llama(hidden=256, intermediate=768, heads=2)
+    model = tiny_quant_llama(hidden=256, intermediate=768, heads=2)
     quant.make_quant_attn(model)
     quant.make_quant_norm(model)
     quant.make_fused_mlp(model)
