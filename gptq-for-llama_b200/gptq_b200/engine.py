@@ -147,7 +147,7 @@ class LlamaDecoder:
         self.sample_graph = None  # the decode step followed by gptq_sample_tokens, captured on first sampled use
         self._stream = torch.cuda.Stream(self.dev)
         if use_graph:
-            self._capture()
+            self.graph = self._capture(self._enqueue, self._enqueue)
 
     def _setup_tp(self, scratch_bytes):
         """Scratch and logits in IPC-shareable device memory; every rank maps every other rank's buffers (gptq_llama_tp)."""
@@ -198,20 +198,29 @@ class LlamaDecoder:
             self._layer_arr[i].mlp_perm = pm['gate'].data_ptr() if pm['gate'] is not None else None
 
     # ------------------------------------------------------------------------------------------
-    def _enqueue(self, stream):
+    def _enqueue(self, stream, sample=False):
+        """One decode step on `stream`; with `sample`, followed by gptq_sample_tokens under set_sampling's parameters."""
         check(lib.gptq_llama_decode_step(ctypes.byref(self.model), ctypes.byref(self.state), ctypes.c_void_p(stream.cuda_stream)))
+        if sample:
+            self._enqueue_sample(stream)
 
-    def _capture(self):
+    def _enqueue_sample(self, stream):
+        check(lib.gptq_sample_tokens(self.logits.data_ptr(), self.vocab, self.batch, self.vocab, self.positions.data_ptr(), ctypes.byref(self._sampling),
+                                     self.next_tokens.data_ptr(), ctypes.c_void_p(stream.cuda_stream)))
+
+    def _capture(self, enqueue, warm_up):
+        """A CUDA graph of enqueue(stream), captured on the decoder's stream after warm_up(stream) has run once outside the capture (lazy module
+        loading, func attributes)."""
         with torch.cuda.device(self.dev):
             torch.cuda.synchronize()
             with torch.cuda.stream(self._stream):
-                self._enqueue(self._stream)  # warm-up outside capture (lazy module loading, func attributes)
+                warm_up(self._stream)
                 self._stream.synchronize()
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g, stream=self._stream):
-                    self._enqueue(self._stream)
-            self.graph = g
+                    enqueue(self._stream)
             torch.cuda.synchronize()
+        return g
 
     def launches_per_step(self) -> int:
         """Kernels of ours launched per decoded token (1 on the persistent single-kernel path)."""
@@ -224,71 +233,49 @@ class LlamaDecoder:
     def step(self, stream=None):
         """Run one decode step on the tokens/positions currently in device memory.  With set_sampling in force, next_tokens is then drawn
         from the step's logits by gptq_sample_tokens (one more launch, in a second captured graph)."""
-        if self._sampling is not None:
-            if self.graph is None:
-                s = stream or torch.cuda.current_stream(self.dev)
-                self._enqueue(s)
-                self._enqueue_sample(s)
-                return
-            if self.sample_graph is None:
-                self._capture_sampled()
-            self.sample_graph.replay()
-        elif self.graph is not None:
+        sample = self._sampling is not None
+        if self.graph is None:
+            self._enqueue(stream or torch.cuda.current_stream(self.dev), sample)
+        elif not sample:
             self.graph.replay()
         else:
-            self._enqueue(stream or torch.cuda.current_stream(self.dev))
+            if self.sample_graph is None:  # warm-up: the sampling kernel alone, which reads the current logits and writes next_tokens only
+                self.sample_graph = self._capture(lambda s: self._enqueue(s, sample=True), self._enqueue_sample)
+            self.sample_graph.replay()
+
+    def _refuse_tp(self, feature):
+        """The ranks of a tensor-parallel decoder run the decode step only: anything else is refused before it touches the device."""
+        if self.tp is not None:
+            raise ValueError(f'{feature}: not supported under tensor parallelism')
+
+    def _sampling_args(self, temperature, top_k, top_p, seed, eos_token_id, min_length):
+        """set_sampling's arguments checked and as host tensors of one value per sequence, named after the gptq_sampling fields."""
+        self._refuse_tp('sampling and eos stopping')
+        t, k, p = sampling_lists(self.batch, temperature, top_k, top_p)
+        eos = [-1 if v is None else int(v) for v in _per_seq(self.batch, eos_token_id, 'eos_token_id')]
+        if any(not -1 <= e < self.vocab for e in eos):
+            raise ValueError(f'eos_token_id outside the vocabulary (0..{self.vocab - 1})')
+        return dict(temperature=torch.tensor(t, dtype=torch.float32), top_k=torch.tensor(k, dtype=torch.int32), top_p=torch.tensor(p, dtype=torch.float32),
+                    seed=torch.tensor([(int(v) + 2**63) % 2**64 - 2**63 for v in _per_seq(self.batch, seed, 'seed')]),  # the uint64 seed's bits as int64
+                    eos_token=torch.tensor(eos, dtype=torch.int32),
+                    min_length=torch.tensor([int(v) for v in _per_seq(self.batch, min_length, 'min_length')], dtype=torch.int32))
 
     def set_sampling(self, temperature, top_k, top_p, seed, eos_token_id=None, min_length=0):
         """Draw next_tokens from each step's logits from now on (gptq_sample_tokens; clear_sampling ends it).  Every argument is one value for
         all sequences or a list of `batch`: temperature (0: greedy), top_k (0: off), top_p (1: off), seed (64-bit), eos_token_id (None: no eos)
         and min_length (eos is suppressed while position + 1 < min_length)."""
-        if self.tp is not None:
-            raise ValueError('sampling and eos stopping are not supported under tensor parallelism')
-        t, k, p = sampling_lists(self.batch, temperature, top_k, top_p)
-        seeds = [int(v) % 2**64 for v in _per_seq(self.batch, seed, 'seed')]
-        eos = [-1 if v is None else int(v) for v in _per_seq(self.batch, eos_token_id, 'eos_token_id')]
-        if any(not -1 <= e < self.vocab for e in eos):
-            raise ValueError(f'eos_token_id outside the vocabulary (0..{self.vocab - 1})')
-        ml = [int(v) for v in _per_seq(self.batch, min_length, 'min_length')]
-        if self._sampling_struct is None:
+        args = self._sampling_args(temperature, top_k, top_p, seed, eos_token_id, min_length)
+        if self._sampling_arrays is None:  # allocated once: the sampled graph reads them in place
             with torch.cuda.device(self.dev):
-                arrs = dict(temperature=torch.zeros(self.batch, dtype=torch.float32, device=self.dev),
-                            top_k=torch.zeros(self.batch, dtype=torch.int32, device=self.dev),
-                            top_p=torch.zeros(self.batch, dtype=torch.float32, device=self.dev),
-                            seed=torch.zeros(self.batch, dtype=torch.int64, device=self.dev),
-                            eos_token=torch.zeros(self.batch, dtype=torch.int32, device=self.dev),
-                            min_length=torch.zeros(self.batch, dtype=torch.int32, device=self.dev))
-            st = Sampling(**{f: a.data_ptr() for f, a in arrs.items()})
-            self._sampling_arrays, self._sampling_struct = arrs, st
-        a = self._sampling_arrays
-        a['temperature'].copy_(torch.tensor(t, dtype=torch.float32))
-        a['top_k'].copy_(torch.tensor(k, dtype=torch.int32))
-        a['top_p'].copy_(torch.tensor(p, dtype=torch.float32))
-        a['seed'].copy_(torch.tensor([v - 2**64 if v >= 2**63 else v for v in seeds], dtype=torch.int64))  # uint64 bits
-        a['eos_token'].copy_(torch.tensor(eos, dtype=torch.int32))
-        a['min_length'].copy_(torch.tensor(ml, dtype=torch.int32))
+                self._sampling_arrays = {f: torch.zeros_like(v, device=self.dev) for f, v in args.items()}
+            self._sampling_struct = Sampling(**{f: a.data_ptr() for f, a in self._sampling_arrays.items()})
+        for f, v in args.items():
+            self._sampling_arrays[f].copy_(v)
         self._sampling = self._sampling_struct
 
     def clear_sampling(self):
         """step() takes the argmax again (the decode step's own next_tokens)."""
         self._sampling = None
-
-    def _enqueue_sample(self, stream):
-        check(lib.gptq_sample_tokens(self.logits.data_ptr(), self.vocab, self.batch, self.vocab, self.positions.data_ptr(), ctypes.byref(self._sampling),
-                                     self.next_tokens.data_ptr(), ctypes.c_void_p(stream.cuda_stream)))
-
-    def _capture_sampled(self):
-        with torch.cuda.device(self.dev):
-            torch.cuda.synchronize()
-            with torch.cuda.stream(self._stream):
-                self._enqueue_sample(self._stream)  # warm-up outside capture: reads the current logits, writes next_tokens only
-                self._stream.synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g, stream=self._stream):
-                    self._enqueue(self._stream)
-                    self._enqueue_sample(self._stream)
-            self.sample_graph = g
-            torch.cuda.synchronize()
 
     def reset(self):
         self.positions.zero_()
@@ -302,12 +289,20 @@ class LlamaDecoder:
         known = self.cached_tokens[b]
         self.cached_tokens[b] = known[:pos] + list(toks) if len(known) >= pos else known
 
+    def _token_ids(self, tokens, what='token id', check=True):
+        """Token ids given as a tensor (of any shape) or a sequence, as a list, each checked against the vocabulary (ValueError) unless `check`
+        is False."""
+        ids = tokens.reshape(-1).tolist() if isinstance(tokens, torch.Tensor) else [int(t) for t in tokens]
+        if check and any(not 0 <= t < self.vocab for t in ids):
+            raise ValueError(f'{what} outside the vocabulary (0..{self.vocab - 1})')
+        return ids
+
     def set_input(self, tokens, positions):
         """Token ids (int or sequence of `batch` ints) and the cache position of this step (int: every sequence, or sequence of `batch` ints: one
         per sequence); validated on the host: the kernels only clamp (a position beyond the cache or a token outside the vocabulary must never
         reach them).  The step that follows caches row p of each sequence, so `lengths` becomes p + 1 (writing self.positions directly bypasses
         this record, and generate(..., reuse_cache=True) then reuses less or nothing)."""
-        toks = [int(tokens)] * self.batch if isinstance(tokens, int) else [int(t) for t in tokens]
+        toks = self._token_ids([tokens] * self.batch if isinstance(tokens, int) else tokens)
         if len(toks) != self.batch:
             raise ValueError(f'expected {self.batch} token ids, got {len(toks)}')
         pos = [int(positions)] * self.batch if isinstance(positions, int) else [int(p) for p in positions]
@@ -315,8 +310,6 @@ class LlamaDecoder:
             raise ValueError(f'expected {self.batch} positions, got {len(pos)}')
         if any(not 0 <= p < self.max_seq for p in pos):
             raise ValueError(f'position {positions} outside the KV cache (max_seq = {self.max_seq})')
-        if any(t < 0 or t >= self.vocab for t in toks):
-            raise ValueError(f'token id outside the vocabulary (0..{self.vocab - 1})')
         self.tokens.copy_(torch.tensor(toks, dtype=torch.int32))
         self.positions.copy_(torch.tensor(pos, dtype=torch.int32))
         for b, (t, p) in enumerate(zip(toks, pos)):
@@ -378,7 +371,7 @@ class LlamaDecoder:
         """Ragged pass (_forward_rows) over the first len(prompt) - 1 tokens of each of the `batch` prompts that fills sequence b's slot of the
         static KV cache.  The LAST token of each prompt then goes through the decode step like every generated one (it produces the first
         logits).  Returns the number of cached positions per prompt (0 for a prompt of length 1)."""
-        assert self.tp is None
+        self._refuse_tp('prefill_batch()')
         if len(prompts) != self.batch:
             raise ValueError(f'expected {self.batch} prompts, got {len(prompts)}')
         ns = [max(len(p) - 1, 0) for p in prompts]
@@ -398,14 +391,11 @@ class LlamaDecoder:
         gptq_cached_attention, and their keys and values are written to cache rows lengths[b] .. lengths[b] + len - 1.  An empty chunk leaves its
         sequence untouched.  The decode buffers and the captured graph are not touched; the next step(s) continue at the new lengths.
         Everything is validated before anything is written.  Returns the new lengths."""
-        if self.tp is not None:
-            raise ValueError('extend() is not supported under tensor parallelism')
+        self._refuse_tp('extend()')
         if len(chunks) != self.batch:
             raise ValueError(f'expected {self.batch} chunks, got {len(chunks)}')
-        seqs = [c.reshape(-1).tolist() if isinstance(c, torch.Tensor) else [int(t) for t in c] for c in chunks]
+        seqs = [self._token_ids(c) for c in chunks]
         for b, s in enumerate(seqs):
-            if any(t < 0 or t >= self.vocab for t in s):
-                raise ValueError(f'token id outside the vocabulary (0..{self.vocab - 1})')
             if self.lengths[b] + len(s) > self.max_seq:
                 raise ValueError(f'sequence {b}: {self.lengths[b]} cached + {len(s)} new positions do not fit the KV cache (max_seq = {self.max_seq})')
         if any(seqs):
@@ -422,14 +412,10 @@ class LlamaDecoder:
         lm_head + log-softmax kernel (gptq_lm_head_logprob).  Lists are grouped into passes of at most SCORE_ROWS rows (a longer list is scored
         alone), so activation memory stays bounded.  Independent of `batch` and `max_seq`; the KV cache, the decode buffers and the captured
         graph are not touched."""
-        if self.tp is not None:
-            raise ValueError('score() is not supported under tensor parallelism')
-        seqs = [s.reshape(-1).tolist() if isinstance(s, torch.Tensor) else [int(t) for t in s] for s in sequences]
-        for s in seqs:
-            if len(s) < 2:
-                raise ValueError('every scored sequence needs at least 2 tokens')
-            if any(t < 0 or t >= self.vocab for t in s):
-                raise ValueError(f'token id outside the vocabulary (0..{self.vocab - 1})')
+        self._refuse_tp('score()')
+        seqs = [self._token_ids(s) for s in sequences]
+        if any(len(s) < 2 for s in seqs):
+            raise ValueError('every scored sequence needs at least 2 tokens')
         out = []
         i = 0
         while i < len(seqs):
@@ -454,7 +440,7 @@ class LlamaDecoder:
     def perplexity(self, token_ids, seqlen=2048):
         """Perplexity of a token stream as the reference's llama_eval computes it (llama.py:174-259): nsamples = len // seqlen chunks (the tail is
         dropped), each scored from position 0, ppl = exp(sum of the chunks' NLL / (nsamples * (seqlen - 1))), the NLL summed in fp64."""
-        ids = token_ids.reshape(-1).tolist() if isinstance(token_ids, torch.Tensor) else [int(t) for t in token_ids]
+        ids = self._token_ids(token_ids, check=False)  # score() checks the chunks; the dropped tail is never read
         if seqlen < 2:
             raise ValueError('seqlen must be at least 2')
         nsamples = len(ids) // seqlen
@@ -464,20 +450,11 @@ class LlamaDecoder:
         nll = -float(torch.cat(lps).double().sum())
         return math.exp(nll / (nsamples * (seqlen - 1)))
 
-    def _check_prompts(self, prompts, max_new_tokens):
-        if len(prompts) != self.batch:
-            raise ValueError(f'expected {self.batch} prompts, got {len(prompts)}')
-        for p in prompts:
-            if len(p) < 1 or len(p) + max_new_tokens > self.max_seq + 1:
-                raise ValueError(f'prompt ({len(p)}) + max_new_tokens ({max_new_tokens}) does not fit the KV cache (max_seq = {self.max_seq})')
-            if any(int(t) < 0 or int(t) >= self.vocab for t in p):
-                raise ValueError(f'prompt token id outside the vocabulary (0..{self.vocab - 1})')
-
     def _decode(self, prompts, max_new_tokens, starts, eos=None):
         """Lock-step decode: sequence b is stepped from position starts[b] (its cache holds the positions before it) until it has
-        max_new_tokens new tokens or has emitted eos[b]; the prompts' remaining tokens are fed first.  The steps end when every sequence is
-        done; a finished sequence is stepped along meanwhile, and the cache rows it writes then are dropped from its record."""
-        out = [[int(t) for t in p] for p in prompts]
+        max_new_tokens new tokens or has emitted eos[b] (None: no eos); the prompts' remaining tokens are fed first.  The steps end when every
+        sequence is done; a finished sequence is stepped along meanwhile, and the cache rows it writes then are dropped from its record."""
+        out = [list(p) for p in prompts]
         steps = len(prompts[0]) + max_new_tokens - 1 - starts[0]
         assert all(len(p) + max_new_tokens - 1 - s == steps for p, s in zip(prompts, starts))
         stopped = [False] * len(prompts)
@@ -498,28 +475,9 @@ class LlamaDecoder:
                 self.cached_tokens[b] = self.cached_tokens[b][:len(o) - 1]
         return out
 
-    def _sampled_decode(self, prompts, max_new_tokens, starts, do_sample, temperature, top_k, top_p, seed, eos_token_id, min_new_tokens):
-        """_decode with gptq_sample_tokens after every step when sampling or an eos token is asked for (else exactly the greedy decode).
-        Sequence b draws with seed + b (seed None: a random 64-bit seed from torch's host RNG) and cannot emit eos before
-        min_new_tokens new tokens (min_length = len(prompt) + min_new_tokens)."""
-        if not do_sample and eos_token_id is None:
-            return self._decode(prompts, max_new_tokens, starts)
-        if seed is None:
-            seed = int(torch.randint(-2**63, 2**63 - 1, (1, ), dtype=torch.int64)) % 2**64
-        eos = [None if v is None else int(v) for v in _per_seq(self.batch, eos_token_id, 'eos_token_id')]
-        self.set_sampling(temperature if do_sample else 0.0, top_k if do_sample else 0, top_p if do_sample else 1.0,
-                          [int(seed) + b for b in range(self.batch)], eos, [len(p) + int(min_new_tokens) for p in prompts])
-        try:
-            return self._decode(prompts, max_new_tokens, starts, [-1 if e is None else e for e in eos])
-        finally:
-            self.clear_sampling()
-
     def _reuse(self, prompts, extend=True):
         """Keep what each sequence's cache shares with its prompt (reusable_prefix) and drop the rest of the record; with `extend`, append the
         uncached prompt tokens but the last in one extend() pass.  Returns the positions the decode steps start from."""
-        if self.tp is not None:
-            raise ValueError('reuse_cache is not supported under tensor parallelism')
-        prompts = [[int(t) for t in p] for p in prompts]
         keep = [reusable_prefix(p, self.cached_tokens[b][:self.lengths[b]]) for b, p in enumerate(prompts)]
         for b, c in enumerate(keep):
             self.lengths[b] = c
@@ -529,16 +487,41 @@ class LlamaDecoder:
         self.extend([p[c:len(p) - 1] for p, c in zip(prompts, keep)])
         return [len(p) - 1 for p in prompts]
 
-    def _check_sampling_args(self, do_sample, temperature, top_k, top_p, eos_token_id, min_new_tokens):
-        """Everything generate / generate_batch are given is validated before the cache or the record is touched."""
-        if (do_sample or eos_token_id is not None) and self.tp is not None:
-            raise ValueError('sampling and eos stopping are not supported under tensor parallelism')
-        if do_sample:
-            sampling_lists(self.batch, temperature, top_k, top_p)
-        if any(v is not None and not 0 <= int(v) < self.vocab for v in _per_seq(self.batch, eos_token_id, 'eos_token_id')):
-            raise ValueError(f'eos_token_id outside the vocabulary (0..{self.vocab - 1})')
+    def _generate(self, prompts, max_new_tokens, prefill, reuse_cache, do_sample, temperature, top_k, top_p, seed, eos_token_id, min_new_tokens):
+        """generate and generate_batch.  Every argument is checked before the cache or its record is touched.  When sampling or an eos token is
+        asked for, gptq_sample_tokens runs after every step (else exactly the greedy decode): sequence b draws with seed + b (seed None: a random
+        64-bit seed from torch's host RNG) and cannot emit eos before min_new_tokens new tokens (min_length = len(prompt) + min_new_tokens)."""
+        if len(prompts) != self.batch:
+            raise ValueError(f'expected {self.batch} prompts, got {len(prompts)}')
+        prompts = [self._token_ids(p, 'prompt token id') for p in prompts]
+        for p in prompts:
+            if len(p) < 1 or len(p) + max_new_tokens > self.max_seq + 1:
+                raise ValueError(f'prompt ({len(p)}) + max_new_tokens ({max_new_tokens}) does not fit the KV cache (max_seq = {self.max_seq})')
+        sampling = None
+        if do_sample or eos_token_id is not None:
+            eos = [None if v is None else int(v) for v in _per_seq(self.batch, eos_token_id, 'eos_token_id')]
+            sampling = dict(temperature=temperature if do_sample else 0.0, top_k=top_k if do_sample else 0, top_p=top_p if do_sample else 1.0,
+                            eos_token_id=eos, min_length=[len(p) + int(min_new_tokens) for p in prompts])
+            self._sampling_args(seed=0, **sampling)  # the seed is drawn once everything has passed
+            self._token_ids([e for e in eos if e is not None], 'eos_token_id')  # None is "no eos" here: unlike set_sampling, -1 is refused
         if int(min_new_tokens) < 0:
             raise ValueError('min_new_tokens must be >= 0')
+        if reuse_cache or prefill:
+            self._refuse_tp('reuse_cache' if reuse_cache else 'prefill')
+        if reuse_cache:
+            starts = self._reuse(prompts, extend=prefill)
+        else:
+            self.reset()
+            starts = self.prefill_batch(prompts) if prefill else [0] * self.batch
+        if sampling is None:
+            return self._decode(prompts, max_new_tokens, starts)
+        if seed is None:
+            seed = int(torch.randint(-2**63, 2**63 - 1, (1, ), dtype=torch.int64)) % 2**64
+        self.set_sampling(seed=[int(seed) + b for b in range(self.batch)], **sampling)
+        try:
+            return self._decode(prompts, max_new_tokens, starts, eos)
+        finally:
+            self.clear_sampling()
 
     @torch.no_grad()
     def generate(self, prompt_ids, max_new_tokens, prefill=True, reuse_cache=False, do_sample=False, temperature=1.0, top_k=50, top_p=1.0, seed=None,
@@ -547,18 +530,12 @@ class LlamaDecoder:
         top-k, top-p and one draw per token on the device (gptq_sample_tokens; the defaults are HF's).  seed None draws a random one; the same
         seed gives the same tokens.  With eos_token_id, generation stops after that token (greedy or sampled; it ends the returned list), but
         not before min_new_tokens new tokens.  One engine, two phases: the prompt is prefilled in one batched pass (wgmma GEMM path) into the static KV
-        cache, then the persistent decode kernel takes over token by token; prefill=False feeds the prompt through the decode step instead.
-        reuse_cache=True keeps the cached positions the prompt starts with (e.g. the conversation so far, when the prompt is that conversation
-        plus a new turn) and computes only the rest (with extend(), or through the decode step with prefill=False)."""
+        cache, then the persistent decode kernel takes over token by token; prefill=False, and tensor parallelism, feed the prompt through the
+        decode step instead.  reuse_cache=True keeps the cached positions the prompt starts with (e.g. the conversation so far, when the prompt is
+        that conversation plus a new turn) and computes only the rest (with extend(), or through the decode step with prefill=False)."""
         assert self.batch == 1
-        self._check_prompts([prompt_ids], max_new_tokens)
-        self._check_sampling_args(do_sample, temperature, top_k, top_p, eos_token_id, min_new_tokens)
-        samp = (do_sample, temperature, top_k, top_p, seed, eos_token_id, min_new_tokens)
-        if reuse_cache:
-            return self._sampled_decode([prompt_ids], max_new_tokens, self._reuse([prompt_ids], extend=prefill), *samp)[0]
-        self.reset()
-        start = self.prefill(prompt_ids) if (prefill and self.tp is None) else 0
-        return self._sampled_decode([prompt_ids], max_new_tokens, [start], *samp)[0]
+        return self._generate([prompt_ids], max_new_tokens, prefill and self.tp is None, reuse_cache, do_sample, temperature, top_k, top_p, seed,
+                              eos_token_id, min_new_tokens)[0]
 
     @torch.no_grad()
     def generate_batch(self, prompts, max_new_tokens, reuse_cache=False, do_sample=False, temperature=1.0, top_k=50, top_p=1.0, seed=None,
@@ -573,14 +550,7 @@ class LlamaDecoder:
         value per sequence, and sequence b draws with seed + b, so row b is comparable with a batch-1 run seeded seed + b.  A sequence that
         emits eos stops (its list ends with it) while the others go on; afterwards each sequence's record (lengths, cached_tokens) covers its
         returned tokens but the last, so a following reuse_cache=True turn extends from there."""
-        self._check_prompts(prompts, max_new_tokens)
-        self._check_sampling_args(do_sample, temperature, top_k, top_p, eos_token_id, min_new_tokens)
-        samp = (do_sample, temperature, top_k, top_p, seed, eos_token_id, min_new_tokens)
-        if reuse_cache:
-            return self._sampled_decode(prompts, max_new_tokens, self._reuse(prompts), *samp)
-        self.reset()
-        starts = self.prefill_batch(prompts)
-        return self._sampled_decode(prompts, max_new_tokens, starts, *samp)
+        return self._generate(prompts, max_new_tokens, True, reuse_cache, do_sample, temperature, top_k, top_p, seed, eos_token_id, min_new_tokens)
 
 
 def _per_seq(batch, v, name):
@@ -616,31 +586,34 @@ def reusable_prefix(prompt, cached):
     return c
 
 
-def synthetic_llama(size='7b', bits=4, groupsize=128, act_order=False, vocab=32000, device='cuda:0', seed=0, n_layers=None, **kw):
-    """Random-init GPTQ LLaMA of the named size (no checkpoints are reachable offline): every layer has its
-    own distinct packed tensors so that a decode step streams the full model from HBM.  groupsize -1: one group per linear (the
+def _synthetic_draws(size, bits, groupsize, act_order, vocab, device, seed, n_layers):
+    """The weights of the random-init model, drawn one at a time from one generator seeded with `seed`: each layer's dict, then the
+    embedding, the lm_head and the final norm.  synthetic_llama and synthetic_llama_tp both build their model from these draws, so a
+    tensor-parallel rank holds a shard of the very model synthetic_llama builds from the same seed.  groupsize -1: one group per linear (the
     reference's --groupsize -1, where QuantLinear takes groupsize = infeatures): hidden for qkv / o / gate / up, intermediate for down."""
-    hidden, inter, layers, heads = LLAMA_SHAPES[size]
-    layers = n_layers or layers
+    hidden, inter, layers, _ = LLAMA_SHAPES[size]
     gs_h, gs_i = (hidden, inter) if groupsize == -1 else (groupsize, groupsize)
     dev = torch.device(device)
     gen = torch.Generator(device=dev).manual_seed(seed)
-    L = []
-    for _ in range(layers):
-        gate = random_qlayer(hidden, inter, bits, gs_h, dev, gen, act_order)
-        up = random_qlayer(hidden, inter, bits, gs_h, dev, gen, act_order)
+    qlayer = lambda K, N, gs: random_qlayer(K, N, bits, gs, dev, gen, act_order)
+    norm = lambda: (torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half()
+    for _ in range(n_layers or layers):
+        gate, up = qlayer(hidden, inter, gs_h), qlayer(hidden, inter, gs_h)
         if act_order:  # gate and up see the same input, hence the same Hessian diagonal and the same act-order map (gptq.py:210-216)
             up = QLayerWeights(up.qweight, up.scales, up.qzeros, gate.g_idx.clone(), bits, gs_h)
-        L.append(
-            dict(qkv=random_qlayer(hidden, 3 * hidden, bits, gs_h, dev, gen, act_order), o=random_qlayer(hidden, hidden, bits, gs_h, dev, gen, act_order),
-                 gate=gate, up=up, down=random_qlayer(inter, hidden, bits, gs_i, dev, gen, act_order),
-                 input_norm=(torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half(),
-                 post_norm=(torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half()))
-    # q/k/v share their input, hence their act-order map (quant/fused_attn.py:180): nothing to do, qkv is one layer here
-    embed = (torch.randn(vocab, hidden, device=dev, generator=gen) * 0.5).half()
-    lm_head = (torch.randn(vocab, hidden, device=dev, generator=gen) * 0.02).half()
-    final_norm = (torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half()
-    return LlamaDecoder(L, embed, final_norm, lm_head, heads, **kw)
+        # q/k/v share their input, hence their act-order map (quant/fused_attn.py:180): nothing to do, qkv is one layer here
+        yield dict(qkv=qlayer(hidden, 3 * hidden, gs_h), o=qlayer(hidden, hidden, gs_h), gate=gate, up=up, down=qlayer(inter, hidden, gs_i),
+                   input_norm=norm(), post_norm=norm())
+    yield (torch.randn(vocab, hidden, device=dev, generator=gen) * 0.5).half()
+    yield (torch.randn(vocab, hidden, device=dev, generator=gen) * 0.02).half()
+    yield norm()
+
+
+def synthetic_llama(size='7b', bits=4, groupsize=128, act_order=False, vocab=32000, device='cuda:0', seed=0, n_layers=None, **kw):
+    """Random-init GPTQ LLaMA of the named size (no checkpoints are reachable offline): every layer has its
+    own distinct packed tensors so that a decode step streams the full model from HBM.  groupsize -1 as in _synthetic_draws."""
+    *L, embed, lm_head, final_norm = _synthetic_draws(size, bits, groupsize, act_order, vocab, device, seed, n_layers)
+    return LlamaDecoder(L, embed, final_norm, lm_head, LLAMA_SHAPES[size][3], **kw)
 
 
 def shard_for_rank(layers, lm_head, n_heads, head_dim, rank, size):
@@ -667,30 +640,17 @@ def shard_for_rank(layers, lm_head, n_heads, head_dim, rank, size):
 
 
 def synthetic_llama_tp(size_name, rank, world, bits=4, groupsize=128, vocab=32000, device='cuda:0', seed=0, n_layers=None, full=None, reduce_mode=0, **kw):
-    """One tensor-parallel rank of the random-init model `synthetic_llama(size_name, seed=seed)` (every rank generates the same full model from the same
+    """One tensor-parallel rank of the random-init model `synthetic_llama(size_name, seed=seed)` (every rank draws the same full model from the same
     seed layer by layer and keeps its shard), or of the given `full` decoder's weights.  groupsize -1 as in synthetic_llama."""
-    hidden, inter, layers, heads = LLAMA_SHAPES[size_name]
-    gs_h, gs_i = (hidden, inter) if groupsize == -1 else (groupsize, groupsize)
-    layers = n_layers or layers
-    dev = torch.device(device)
+    hidden, _, _, heads = LLAMA_SHAPES[size_name]
     hd = hidden // heads
     if full is not None:
         L, lm_head, hl, (v0, v1) = shard_for_rank(full.layers, full.lm_head, heads, hd, rank, world)
         return LlamaDecoder(L, full.embed, full.final_norm, lm_head, hl, head_dim=hd, tp=(rank, world, v0, v1, reduce_mode), **kw)
-    gen = torch.Generator(device=dev).manual_seed(seed)
-    L = []
-    fake_head = torch.empty(0, hidden, device=dev)
-    for _ in range(layers):  # shard as we go: a 65B model never exists whole on one GPU
-        gate = random_qlayer(hidden, inter, bits, gs_h, dev, gen)
-        up = random_qlayer(hidden, inter, bits, gs_h, dev, gen)
-        ly = dict(qkv=random_qlayer(hidden, 3 * hidden, bits, gs_h, dev, gen), o=random_qlayer(hidden, hidden, bits, gs_h, dev, gen), gate=gate, up=up,
-                  down=random_qlayer(inter, hidden, bits, gs_i, dev, gen), input_norm=(torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half(),
-                  post_norm=(torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half())
-        L.append(shard_for_rank([ly], fake_head, heads, hd, rank, world)[0][0])
-        del ly, gate, up
-    embed = (torch.randn(vocab, hidden, device=dev, generator=gen) * 0.5).half()
-    lm_head = (torch.randn(vocab, hidden, device=dev, generator=gen) * 0.02).half()
-    final_norm = (torch.rand(hidden, device=dev, generator=gen) * 0.2 + 0.9).half()
+    fake_head = torch.empty(0, hidden, device=device)
+    shard = lambda w: shard_for_rank([w], fake_head, heads, hd, rank, world)[0][0] if isinstance(w, dict) else w
+    # each layer is sharded as soon as it is drawn: a 65B model never exists whole on one GPU
+    *L, embed, lm_head, final_norm = map(shard, _synthetic_draws(size_name, bits, groupsize, False, vocab, device, seed, n_layers))
     v0, v1 = rank * vocab // world, (rank + 1) * vocab // world
     return LlamaDecoder(L, embed, final_norm, lm_head[v0:v1].contiguous(), heads // world, head_dim=hd, tp=(rank, world, v0, v1, reduce_mode), **kw)
 

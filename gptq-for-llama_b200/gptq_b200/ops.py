@@ -32,6 +32,14 @@ def _stream(t: torch.Tensor):
     return ctypes.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
 
 
+def _rows(t: torch.Tensor):
+    """A 2-D operand as the kernels take it: (t with a unit stride along its last dimension, copied only when it has none, and its leading
+    dimension).  The leading dimension is the row stride, or the row width for a single row, whose row stride may be anything."""
+    if t.stride(1) != 1:
+        t = t.contiguous()
+    return t, t.stride(0) if t.shape[0] > 1 else t.shape[1]
+
+
 _workspaces = {}
 
 
@@ -85,8 +93,7 @@ def matmul248(input, qweight, scales, qzeros, g_idx, bits, maxq=None, bias=None,
         raise ValueError('matmul248 expects a 2-D input')
     if input.dtype != torch.float16:
         input = input.half()
-    if input.stride(1) != 1:
-        input = input.contiguous()
+    input, ld = _rows(input)
     w = make_qweight(qweight, scales, qzeros, g_idx, bits, groupsize)
     if input.shape[1] != w.K:
         raise ValueError(f'input has {input.shape[1]} features, weight expects {w.K}')
@@ -97,8 +104,8 @@ def matmul248(input, qweight, scales, qzeros, g_idx, bits, maxq=None, bias=None,
         out = torch.empty((M, w.N), device=input.device, dtype=torch.float16)
         ws, ws_bytes = _workspace(input.device, lib.gptq_qlinear_workspace_bytes(M, w.K, w.N, bits))
         check(
-            lib.gptq_qlinear_fwd(input.data_ptr(), input.stride(0) if M > 1 else w.K, ctypes.byref(w), bias.data_ptr() if bias is not None else None,
-                                 out.data_ptr(), w.N, M, ws.data_ptr() if ws is not None else None, ws_bytes, _stream(input)))
+            lib.gptq_qlinear_fwd(input.data_ptr(), ld, ctypes.byref(w), bias.data_ptr() if bias is not None else None, out.data_ptr(), w.N, M,
+                                 ws.data_ptr() if ws is not None else None, ws_bytes, _stream(input)))
     return out
 
 
@@ -107,15 +114,14 @@ def transpose_matmul248(input, qweight, scales, qzeros, g_idx, bits, maxq=None, 
     _require_cuda(input)
     if input.dtype != torch.float16:
         input = input.half()
-    if input.stride(1) != 1:
-        input = input.contiguous()
+    input, ld = _rows(input)
     w = make_qweight(qweight, scales, qzeros, g_idx, bits, groupsize)
     M = input.shape[0]
     if M == 0:
         return torch.empty((0, w.K), device=input.device, dtype=torch.float16)
     with torch.cuda.device(input.device):
         out = torch.empty((M, w.K), device=input.device, dtype=torch.float16)
-        check(lib.gptq_qlinear_transpose_fwd(input.data_ptr(), input.stride(0) if M > 1 else w.N, ctypes.byref(w), out.data_ptr(), w.K, M, _stream(input)))
+        check(lib.gptq_qlinear_transpose_fwd(input.data_ptr(), ld, ctypes.byref(w), out.data_ptr(), w.K, M, _stream(input)))
     return out
 
 
@@ -124,8 +130,7 @@ def fused_mlp(x, gate, up, bits, groupsize: int = 0):
     _require_cuda(x)
     if x.dtype != torch.float16:
         x = x.half()
-    if x.stride(1) != 1:
-        x = x.contiguous()
+    x, ld = _rows(x)
     wg = make_qweight(*gate, bits, groupsize)
     wu = make_qweight(*up, bits, groupsize)
     M = x.shape[0]
@@ -135,8 +140,8 @@ def fused_mlp(x, gate, up, bits, groupsize: int = 0):
         out = torch.empty((M, wg.N), device=x.device, dtype=torch.float16)
         ws, ws_bytes = _workspace(x.device, lib.gptq_fused_mlp_workspace_bytes(M, wg.K, wg.N, bits))
         check(
-            lib.gptq_fused_mlp_fwd(x.data_ptr(), x.stride(0) if M > 1 else wg.K, ctypes.byref(wg), ctypes.byref(wu), out.data_ptr(), wg.N, M,
-                                   ws.data_ptr() if ws is not None else None, ws_bytes, _stream(x)))
+            lib.gptq_fused_mlp_fwd(x.data_ptr(), ld, ctypes.byref(wg), ctypes.byref(wu), out.data_ptr(), wg.N, M, ws.data_ptr() if ws is not None else None,
+                                   ws_bytes, _stream(x)))
     return out
 
 
@@ -162,15 +167,13 @@ def rotate_half_(qk, position_ids, config=None, base: float = 10000.0):
 
 def rmsnorm(x, weight, eps: float):
     _require_cuda(x, weight)
-    x_arg = x.reshape(-1, x.shape[-1])
-    if x_arg.stride(1) != 1:
-        x_arg = x_arg.contiguous()
+    x_arg, ld = _rows(x.reshape(-1, x.shape[-1]))
     if x_arg.dtype != torch.float16 or weight.dtype != torch.float16:
         raise ValueError('rmsnorm expects float16 activations and weight')
     M, N = x_arg.shape
     with torch.cuda.device(x.device):
         y = torch.empty((M, N), device=x.device, dtype=torch.float16)
-        check(lib.gptq_rmsnorm_fwd(x_arg.data_ptr(), x_arg.stride(0) if M > 1 else N, weight.data_ptr(), y.data_ptr(), N, M, N, float(eps), _stream(x)))
+        check(lib.gptq_rmsnorm_fwd(x_arg.data_ptr(), ld, weight.data_ptr(), y.data_ptr(), N, M, N, float(eps), _stream(x)))
     return y.reshape(x.shape)
 
 
@@ -192,16 +195,14 @@ def lm_head_logprob(x, weight, targets):
     if int(targets.min()) < 0 or int(targets.max()) >= V:
         raise ValueError(f'target id outside the vocabulary (0..{V - 1})')
     targets = targets.to(torch.int32).contiguous()
-    if x.stride(1) != 1:
-        x = x.contiguous()
-    if weight.stride(1) != 1:
-        weight = weight.contiguous()
+    x, ldx = _rows(x)
+    weight, ldw = _rows(weight)
     with torch.cuda.device(x.device):
         out = torch.empty(M, device=x.device, dtype=torch.float32)
         ws, ws_bytes = _workspace(x.device, lib.gptq_lm_head_logprob_workspace_bytes(M, V))
         check(
-            lib.gptq_lm_head_logprob(x.data_ptr(), x.stride(0) if M > 1 else K, weight.data_ptr(), weight.stride(0) if V > 1 else K, M, K, V,
-                                     targets.data_ptr(), out.data_ptr(), ws.data_ptr(), ws_bytes, _stream(x)))
+            lib.gptq_lm_head_logprob(x.data_ptr(), ldx, weight.data_ptr(), ldw, M, K, V, targets.data_ptr(), out.data_ptr(), ws.data_ptr(), ws_bytes,
+                                     _stream(x)))
     return out
 
 
@@ -226,13 +227,12 @@ def cached_attention(q, k_cache, v_cache, spans):
     out = torch.empty((M, nh * hd), device=q.device, dtype=torch.float16)
     if M == 0:
         return out
-    if q.stride(1) != 1:
-        q = q.contiguous()
+    q, ld = _rows(q)
     arr = lambda i: (ctypes.c_int32 * len(spans))(*[sp[i] for sp in spans])
     with torch.cuda.device(q.device):
         check(
-            lib.gptq_cached_attention(q.data_ptr(), q.stride(0) if M > 1 else nh * hd, k_cache.data_ptr(), v_cache.data_ptr(), B, nh, hd, S, len(spans), arr(0),
-                                      arr(1), arr(2), out.data_ptr(), nh * hd, _stream(q)))
+            lib.gptq_cached_attention(q.data_ptr(), ld, k_cache.data_ptr(), v_cache.data_ptr(), B, nh, hd, S, len(spans), arr(0), arr(1), arr(2), out.data_ptr(),
+                                      nh * hd, _stream(q)))
     return out
 
 
@@ -258,8 +258,7 @@ def sample_tokens(logits, positions, temperature, top_k, top_p, seed, eos_token=
     prm = _lib.Sampling(temperature=temperature.data_ptr(), top_k=top_k.data_ptr(), top_p=top_p.data_ptr(), seed=seed.data_ptr(),
                         eos_token=eos_token.data_ptr(), min_length=min_length.data_ptr())
     with torch.cuda.device(dev):
-        check(lib.gptq_sample_tokens(logits.data_ptr(), logits.stride(0) if B > 1 else V, B, V, positions.data_ptr(), ctypes.byref(prm), out.data_ptr(),
-                                     _stream(logits)))
+        check(lib.gptq_sample_tokens(logits.data_ptr(), _rows(logits)[1], B, V, positions.data_ptr(), ctypes.byref(prm), out.data_ptr(), _stream(logits)))
     return out
 
 
@@ -272,48 +271,39 @@ def dequant(qweight, scales, qzeros, g_idx, bits, groupsize: int = 0):
     return out
 
 
-def pack_qweight(intweight, bits):
-    """int32 [K, N] in [0, 2^bits) -> qweight int32 [K/32*bits, N], on the device."""
-    _require_cuda(intweight)
-    intweight = intweight.to(torch.int32).contiguous()
-    K, N = intweight.shape
+def _pack_call(fn, src, bits, fields, out_shape):
+    """int32 out_shape = fn(src) for one of the pack / unpack kernels (csrc/pack.cu), which take the [rows, cols] shape `fields` of the
+    unpacked side."""
+    _require_cuda(src)
     if bits not in SUPPORTED_BITS:
         raise NotImplementedError('Only 2,3,4,8 bits are supported.')
-    with torch.cuda.device(intweight.device):
-        out = torch.empty((K // 32 * bits, N), device=intweight.device, dtype=torch.int32)
-        check(lib.gptq_pack_qweight(intweight.data_ptr(), out.data_ptr(), K, N, bits, _stream(intweight)))
+    src = src.to(torch.int32).contiguous()
+    with torch.cuda.device(src.device):
+        out = torch.empty(out_shape, device=src.device, dtype=torch.int32)
+        check(fn(src.data_ptr(), out.data_ptr(), *fields, bits, _stream(src)))
     return out
+
+
+def pack_qweight(intweight, bits):
+    """int32 [K, N] in [0, 2^bits) -> qweight int32 [K/32*bits, N], on the device."""
+    K, N = intweight.shape
+    return _pack_call(lib.gptq_pack_qweight, intweight, bits, (K, N), (K // 32 * bits, N))
 
 
 def pack_qzeros(zeros_m1, bits):
     """int32 [G, N] (already minus one) -> qzeros int32 [G, N/32*bits]."""
-    _require_cuda(zeros_m1)
-    zeros_m1 = zeros_m1.to(torch.int32).contiguous()
     G, N = zeros_m1.shape
-    if bits not in SUPPORTED_BITS:
-        raise NotImplementedError('Only 2,3,4,8 bits are supported.')
-    with torch.cuda.device(zeros_m1.device):
-        out = torch.empty((G, N // 32 * bits), device=zeros_m1.device, dtype=torch.int32)
-        check(lib.gptq_pack_qzeros(zeros_m1.data_ptr(), out.data_ptr(), G, N, bits, _stream(zeros_m1)))
-    return out
+    return _pack_call(lib.gptq_pack_qzeros, zeros_m1, bits, (G, N), (G, N // 32 * bits))
 
 
 def unpack_qweight(qweight, bits):
-    _require_cuda(qweight)
     K, N = qweight.shape[0] * 32 // bits, qweight.shape[1]
-    with torch.cuda.device(qweight.device):
-        out = torch.empty((K, N), device=qweight.device, dtype=torch.int32)
-        check(lib.gptq_unpack_qweight(qweight.contiguous().data_ptr(), out.data_ptr(), K, N, bits, _stream(qweight)))
-    return out
+    return _pack_call(lib.gptq_unpack_qweight, qweight, bits, (K, N), (K, N))
 
 
 def unpack_qzeros(qzeros, bits):
-    _require_cuda(qzeros)
     G, N = qzeros.shape[0], qzeros.shape[1] * 32 // bits
-    with torch.cuda.device(qzeros.device):
-        out = torch.empty((G, N), device=qzeros.device, dtype=torch.int32)
-        check(lib.gptq_unpack_qzeros(qzeros.contiguous().data_ptr(), out.data_ptr(), G, N, bits, _stream(qzeros)))
-    return out
+    return _pack_call(lib.gptq_unpack_qzeros, qzeros, bits, (G, N), (G, N))
 
 
 class QLayerWeights:
@@ -326,10 +316,6 @@ class QLayerWeights:
         self.qweight, self.scales, self.qzeros = qweight.contiguous(), scales.contiguous(), qzeros.contiguous()
         self.g_idx = g_idx[:K].contiguous()  # the fused qkv g_idx of the reference is 3K long; only the first K entries are read
         self.bits, self.groupsize, self.perm = bits, groupsize, perm
-
-    def __getitem__(self, name):
-        """Field access by key (plan['qweight'], plan['perm'], ...), as callers of kernel_form and QuantLinear.kernel_plan read their result."""
-        return getattr(self, name)
 
     @functools.cached_property
     def hint(self) -> int:
@@ -402,13 +388,6 @@ class QLayerWeights:
             raise ValueError(f'row shard [{k0}, {k1}) does not keep whole groups of {gs} and whole packed words')
         g = (torch.arange(k1 - k0, device=self.g_idx.device) // gs).to(torch.int32)
         return QLayerWeights(self.qweight[k0 * bits // 32:k1 * bits // 32], self.scales[k0 // gs:k1 // gs], self.qzeros[k0 // gs:k1 // gs], g, bits, gs)
-
-
-def kernel_form(qweight, scales, qzeros, g_idx, bits, groupsize, allow_perm=True):
-    """QLayerWeights.kernel_form of a stored layer, or None when the layer is already in that form or does not qualify."""
-    stored = QLayerWeights(qweight, scales, qzeros, g_idx, bits, groupsize)
-    kf = stored.kernel_form(allow_perm)
-    return None if kf is stored else kf
 
 
 def mlp_kernel_form(gate, up, allow_perm=True):

@@ -7,7 +7,7 @@ autotune_warmup_fused :256-288); the gate/up contraction + SwiGLU epilogue is on
 import torch.nn as nn
 
 from gptq_b200 import ops
-from .quant_linear import QuantLinear
+from .quant_linear import QuantLinear, _PackedView
 
 try:  # only needed by make_fused_mlp's isinstance test
     from transformers.models.llama.modeling_llama import LlamaMLP
@@ -17,7 +17,7 @@ except Exception:  # pragma: no cover - transformers is optional for the kernels
 _PARTS = ('qweight', 'scales', 'qzeros', 'g_idx')
 
 
-class QuantLlamaMLP(nn.Module):
+class QuantLlamaMLP(_PackedView, nn.Module):
 
     def __init__(self, gate_proj, down_proj, up_proj):
         super().__init__()
@@ -34,30 +34,26 @@ class QuantLlamaMLP(nn.Module):
         self.maxq = gate_proj.maxq
         self.groupsize = gate_proj.groupsize
         self.down_proj = down_proj
-        self._view = None  # {'key', 'weights': (gate, up) as ops.QLayerWeights, 'plan': their kernel form once asked for}
 
-    def _cached_view(self):
-        # like QuantLinear's: keyed on the buffers, which fused2cuda / fused2cpu and .cuda() replace
-        bufs = [getattr(self, f'{proj}_{part}') for proj in ('gate_proj', 'up_proj') for part in _PARTS]
-        key = [(t.device, t.data_ptr(), t._version) for t in bufs]
-        if self._view is None or self._view['key'] != key:
-            self._view = dict(key=key, weights=(ops.QLayerWeights(*bufs[:4], self.bits, self.groupsize), ops.QLayerWeights(*bufs[4:], self.bits, self.groupsize)))
-        return self._view
+    def _packed(self):
+        return [getattr(self, f'{proj}_{part}') for proj in ('gate_proj', 'up_proj') for part in _PARTS]
 
     def weights(self):
         """(gate, up) as gptq_b200.ops.QLayerWeights (cached until a buffer is replaced or modified)."""
-        return self._cached_view()['weights']
+        def pair():
+            bufs = self._packed()
+            return ops.QLayerWeights(*bufs[:4], self.bits, self.groupsize), ops.QLayerWeights(*bufs[4:], self.bits, self.groupsize)
+        return self._derived('weights', pair)
 
     def kernel_plan(self):
         """(gate, up) in the layout of the tuned int4 kernels (ops.mlp_kernel_form: act-order rows regrouped, 2/3-bit fields widened;
         their shared input gather in `perm`) when both need it and share their input gather; None otherwise."""
-        view = self._cached_view()
-        if 'plan' not in view:
-            gate, up = view['weights']
+        def plan():
+            gate, up = self.weights()
             plan = ops.mlp_kernel_form(gate, up)
             # the fused kernel takes one bit width: a pair with a layer left as stored runs as stored
-            view['plan'] = None if plan is None or plan[0] is gate or plan[1] is up else plan
-        return view['plan']
+            return None if plan is None or plan[0] is gate or plan[1] is up else plan
+        return self._derived('plan', plan)
 
     def forward(self, x):
         return self.down_proj(self.triton_llama_mlp(x))

@@ -49,7 +49,21 @@ class QuantLinearFunction(torch.autograd.Function):
         return grad_input, None, None, None, None, None, None, None, None
 
 
-class QuantLinear(nn.Module):
+class _PackedView:
+    """What a module over packed buffers (the tensors _packed() returns) derives from them -- weights() and kernel_plan() -- each computed
+    once and kept until a buffer is replaced or modified: pack(), load_state_dict, .cuda() and fused2cuda / fused2cpu do."""
+    _view = None  # {'key': the buffers' identity and versions, name: what _derived(name, ...) computed for them}
+
+    def _derived(self, name, derive):
+        key = [(t.device, t.data_ptr(), t._version) for t in self._packed()]
+        if self._view is None or self._view['key'] != key:
+            self._view = dict(key=key)
+        if name not in self._view:
+            self._view[name] = derive()
+        return self._view[name]
+
+
+class QuantLinear(_PackedView, nn.Module):
 
     def __init__(self, bits, groupsize, infeatures, outfeatures, bias):
         super().__init__()
@@ -70,7 +84,6 @@ class QuantLinear(nn.Module):
             self.register_buffer('bias', torch.zeros((outfeatures), dtype=torch.float16))
         else:
             self.bias = None
-        self._view = None  # {'key', 'weights': ops.QLayerWeights of the buffers, 'plan': its kernel form once asked for}
 
     # ------------------------------------------------------------------ packing (offline)
     def pack(self, linear, scales, zeros, g_idx=None):
@@ -102,16 +115,12 @@ class QuantLinear(nn.Module):
             self.bias = linear.bias.detach().clone().half().to(home)
 
     # ------------------------------------------------------------------ forward
-    def _cached_view(self):
-        # pack(), load_state_dict and .cuda() replace or modify the buffers: the view, and what is derived from it, is rebuilt then
-        key = [(t.device, t.data_ptr(), t._version) for t in (self.qweight, self.scales, self.qzeros, self.g_idx)]
-        if self._view is None or self._view['key'] != key:
-            self._view = dict(key=key, weights=ops.QLayerWeights(self.qweight, self.scales, self.qzeros, self.g_idx, self.bits, self.groupsize))
-        return self._view
+    def _packed(self):
+        return self.qweight, self.scales, self.qzeros, self.g_idx
 
     def weights(self):
         """The buffers as one gptq_b200.ops.QLayerWeights (cached until a buffer is replaced or modified)."""
-        return self._cached_view()['weights']
+        return self._derived('weights', lambda: ops.QLayerWeights(*self._packed(), self.bits, self.groupsize))
 
     def groupsize_hint(self):
         """groupsize if g_idx is the trivial k // groupsize map (lets the kernels skip the gather), else 0.
@@ -121,11 +130,11 @@ class QuantLinear(nn.Module):
     def kernel_plan(self):
         """The derived layer (ops.QLayerWeights.kernel_form, with its input gather in `perm`) that routes an act-order and/or 2/3-bit layer to
         the tuned int4 kernels without touching the stored tensors; None when the layer needs none or does not qualify."""
-        view = self._cached_view()
-        if 'plan' not in view:
-            form = view['weights'].kernel_form()
-            view['plan'] = None if form is view['weights'] else form
-        return view['plan']
+        def plan():
+            stored = self.weights()
+            form = stored.kernel_form()
+            return None if form is stored else form
+        return self._derived('plan', plan)
 
     def forward(self, x):
         out_shape = x.shape[:-1] + (self.outfeatures, )

@@ -135,17 +135,18 @@ def test_transpose_onehot_returns_columns(ops, bits):
 
 
 @pytest.mark.parametrize('bits,act', [(4, True), (3, True), (3, False), (2, False)])
-def test_kernel_form_onehot(ops, bits, act):
-    """Layers served through ops.kernel_form (act-order rows regrouped, 2/3-bit fields widened to int4): a one-hot at k' of the
+def test_qlayer_kernel_form_onehot(ops, bits, act):
+    """Layers served through ops.QLayerWeights.kernel_form (act-order rows regrouped, 2/3-bit fields widened to int4): a one-hot at k' of the
     permuted basis must return the stored layer's row perm[k'], through the matvec (M = 8) and the wgmma GEMM (M = K)."""
     K, N, gs = 256, 256, 64
     L = random_layer(K, N, bits, gs, act=act, seed=20 + bits + act)
     qw, s, qz, g = L.dev
-    kf = ops.kernel_form(qw, s, qz, g, bits, gs)
-    assert kf is not None and kf['bits'] == 4
-    perm = kf['perm'].cpu() if kf['perm'] is not None else torch.arange(K)
+    stored = ops.QLayerWeights(qw, s, qz, g, bits, gs)
+    kf = stored.kernel_form()
+    assert kf is not stored and kf.bits == 4
+    perm = kf.perm.cpu() if kf.perm is not None else torch.arange(K)
     assert not act or not torch.equal(perm, torch.arange(K))
-    layer = (kf['qweight'], s, kf['qzeros'], kf['g_idx'])
+    layer = (kf.qweight, s, kf.qzeros, kf.g_idx)
     for M, kernel in ((8, MATVEC), (K, gemm_kernel(K))):
         ks = cyclic(range(K), M)
         x, mult = X.onehot_rows(ks, K, salt=M)

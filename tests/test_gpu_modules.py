@@ -162,7 +162,7 @@ def test_column_slices_are_independent():
         assert_rel_close(part, full[:, n0:n1], what=f'cols {n0}:{n1}')
 
 
-def test_act_order_plan_uses_tuned_kernels_and_matches_gather_path():
+def test_act_order_kernel_plan_uses_tuned_kernels_and_matches_gather_path():
     """Act-order int4: the load-time row regrouping (derived buffer + x gather) gives the same result as the g_idx-gather kernel."""
     import quant
     from gptq_b200 import ops
@@ -173,8 +173,8 @@ def test_act_order_plan_uses_tuned_kernels_and_matches_gather_path():
     ql = ql.cuda()
     assert quant.autotune_warmup_linear(ql) == 1 and ql.kernel_plan() is not None
     plan = ql.kernel_plan()
-    perm, qw_sorted, g_triv = plan['perm'], plan['qweight'], plan['g_idx']
-    assert plan['bits'] == 4 and plan['qzeros'] is ql.qzeros
+    perm, qw_sorted, g_triv = plan.perm, plan.qweight, plan.g_idx
+    assert plan.bits == 4 and plan.qzeros is ql.qzeros
     W_gather = ops.dequant(ql.qweight, ql.scales, ql.qzeros, ql.g_idx, 4, 0)
     W_sorted = ops.dequant(qw_sorted, ql.scales, ql.qzeros, g_triv, 4, 128)
     assert torch.equal(W_sorted, W_gather.index_select(0, perm))  # the same fp16 weights, rows regrouped
@@ -184,7 +184,7 @@ def test_act_order_plan_uses_tuned_kernels_and_matches_gather_path():
 
 
 @pytest.mark.parametrize('bits,act', [(3, False), (3, True), (2, True)])
-def test_narrow_bits_are_served_by_the_int4_kernels_through_the_widened_plan(bits, act):
+def test_narrow_bits_are_served_by_the_int4_kernels_through_the_widened_kernel_plan(bits, act):
     """2/3-bit layers (config 4: int3 act-order): fields widened to nibbles at load time -> identical dequantised weights,
     outputs within tolerance of the oracle on the ORIGINAL packed tensors, for the matvec (M=1) and the GEMM (M=40)."""
     import quant
@@ -194,10 +194,10 @@ def test_narrow_bits_are_served_by_the_int4_kernels_through_the_widened_plan(bit
     cpu = [t.clone() for t in (ql.qweight, ql.scales, ql.qzeros, ql.g_idx)]
     ql = ql.cuda()
     plan = ql.kernel_plan()
-    assert plan is not None and plan['bits'] == 4 and (plan['perm'] is not None) == act
+    assert plan is not None and plan.bits == 4 and (plan.perm is not None) == act
     W_orig = ops.dequant(ql.qweight, ql.scales, ql.qzeros, ql.g_idx, bits, 0)
-    W_plan = ops.dequant(plan['qweight'], ql.scales, plan['qzeros'], plan['g_idx'], 4, 128)
-    assert torch.equal(W_plan, W_orig if plan['perm'] is None else W_orig.index_select(0, plan['perm']))
+    W_plan = ops.dequant(plan.qweight, ql.scales, plan.qzeros, plan.g_idx, 4, 128)
+    assert torch.equal(W_plan, W_orig if plan.perm is None else W_orig.index_select(0, plan.perm))
     for M, rel in ((1, 1e-3), (40, 2e-3)):
         x = torch.randn(M, 1024, generator=torch.Generator().manual_seed(M)).half()
         assert_rel_close(ql(x.cuda()), O.qlinear_fwd(x, *cpu, bits), rel=rel, what=f'bits={bits} act={act} M={M}')

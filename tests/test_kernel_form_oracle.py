@@ -1,4 +1,4 @@
-"""CPU: the algebra behind gptq_b200.ops.kernel_form (load-time derived buffers), restated with the oracle's pack/unpack.
+"""CPU: the algebra behind gptq_b200.ops.QLayerWeights.kernel_form (load-time derived buffers), restated with the oracle's pack/unpack.
 
 Regrouping act-order rows by a stable sort on the group and widening 2/3-bit fields to nibbles must leave every
 dequantised weight bit-identical (rows permuted), so the only difference between the derived form and the stored

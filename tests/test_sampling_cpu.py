@@ -169,3 +169,64 @@ def test_tensor_parallel_decoder_refuses_sampling_and_eos():
         dec.generate([1, 2], 4, eos_token_id=3)
     with pytest.raises(ValueError, match='tensor parallelism'):
         dec.set_sampling(1.0, 50, 1.0, 0)
+
+
+TP = (0, 2, 0, 256)  # rank 0 of 2, holding vocabulary rows 0..255
+OOV = 512  # the shell's vocabulary is 0..511
+
+
+def _decoder_shell(tp, batch):
+    """A decoder without weights, cache or device buffers: a call that got past its argument checks fails on a missing attribute instead."""
+    from gptq_b200.engine import LlamaDecoder
+    dec = LlamaDecoder.__new__(LlamaDecoder)
+    dec.tp, dec.batch, dec.max_seq, dec.vocab = tp, batch, 64, 512
+    dec.lengths, dec.cached_tokens = [0] * batch, [[] for _ in range(batch)]
+    return dec
+
+
+@pytest.mark.parametrize('tp, batch, call', [
+    pytest.param(None, 1, lambda d: d.set_input(OOV, 0), id='set_input-oov'),
+    pytest.param(None, 2, lambda d: d.set_input(torch.tensor([3, -1]), [0, 1]), id='set_input-negative-tensor'),
+    pytest.param(None, 1, lambda d: d.extend([[1, OOV]]), id='extend-oov'),
+    pytest.param(None, 2, lambda d: d.extend([[], torch.tensor([[3], [OOV]])]), id='extend-oov-tensor'),
+    pytest.param(TP, 1, lambda d: d.extend([[1, 2]]), id='extend-tp'),
+    pytest.param(None, 1, lambda d: d.score([[1, 2], [3, OOV]]), id='score-oov'),
+    pytest.param(TP, 1, lambda d: d.score([[1, 2]]), id='score-tp'),
+    pytest.param(None, 1, lambda d: d.perplexity(torch.tensor([[1, 2, OOV, 3]]), seqlen=2), id='perplexity-oov'),
+    pytest.param(TP, 1, lambda d: d.perplexity([1, 2, 3, 4], seqlen=2), id='perplexity-tp'),
+    pytest.param(None, 1, lambda d: d.generate([1, OOV], 4), id='generate-oov'),
+    pytest.param(None, 1, lambda d: d.generate([1, 2], 4, eos_token_id=OOV), id='generate-eos-oov'),
+    pytest.param(None, 1, lambda d: d.generate([1, 2], 4, eos_token_id=-1), id='generate-eos-negative'),
+    pytest.param(TP, 1, lambda d: d.generate([1, 2], 4, do_sample=True), id='generate-tp-sample'),
+    pytest.param(TP, 1, lambda d: d.generate([1, 2], 4, eos_token_id=3), id='generate-tp-eos'),
+    pytest.param(TP, 1, lambda d: d.generate([1, 2], 4, reuse_cache=True), id='generate-tp-reuse'),
+    pytest.param(None, 1, lambda d: d.generate([1, 2], 4, do_sample=True, top_p=1.5), id='generate-top_p'),
+    pytest.param(None, 1, lambda d: d.generate([1, 2], 4, do_sample=True, temperature=-1.0), id='generate-temperature'),
+    pytest.param(None, 1, lambda d: d.generate([1, 2], 4, min_new_tokens=-1), id='generate-min_new_tokens'),
+    pytest.param(None, 2, lambda d: d.generate_batch([[1, 2], [3, OOV]], 4), id='generate_batch-oov'),
+    pytest.param(None, 2, lambda d: d.generate_batch([[1, 2], [3]], 4, eos_token_id=[5, OOV]), id='generate_batch-eos-oov'),
+    pytest.param(TP, 1, lambda d: d.generate_batch([[1, 2]], 4, reuse_cache=True), id='generate_batch-tp-reuse'),
+    pytest.param(TP, 1, lambda d: d.generate_batch([[1, 2]], 4, do_sample=True), id='generate_batch-tp-sample'),
+    pytest.param(None, 2, lambda d: d.generate_batch([[1, 2], [3]], 4, do_sample=True, temperature=[1.0]), id='generate_batch-temperature-list'),
+    pytest.param(None, 2, lambda d: d.generate_batch([[1, 2], [3]], 4, do_sample=True, top_k=[5, -1]), id='generate_batch-top_k'),
+    pytest.param(None, 1, lambda d: d.set_sampling(1.0, 50, 1.0, 0, eos_token_id=OOV), id='set_sampling-eos-oov'),
+    pytest.param(TP, 1, lambda d: d.set_sampling(1.0, 50, 1.0, 0), id='set_sampling-tp'),
+    pytest.param(None, 1, lambda d: d.set_sampling(1.0, 50, 0.0, 0), id='set_sampling-top_p'),
+    pytest.param(None, 2, lambda d: d.set_sampling(1.0, 50, 1.0, 0, min_length=[1, 2, 3]), id='set_sampling-min_length-list'),
+])
+def test_decoder_entry_points_refuse_bad_arguments_before_any_device_work(tp, batch, call):
+    """Out-of-vocabulary token ids, features a tensor-parallel rank does not run, and bad sampling arguments raise ValueError from every
+    public entry point of the decoder while its checks run, before anything is written to the device, the cache or its record."""
+    dec = _decoder_shell(tp, batch)
+    with pytest.raises(ValueError, match='tensor parallelism' if tp else None):
+        call(dec)
+    assert dec.lengths == [0] * batch and dec.cached_tokens == [[]] * batch
+
+
+def test_tensor_parallel_generate_batch_is_refused_before_the_cache_is_reset():
+    """A tensor-parallel rank cannot prefill, so generate_batch refuses outright rather than feed the prompts through the decode step."""
+    dec = _decoder_shell(TP, 1)
+    with pytest.raises(ValueError, match='tensor parallelism'):
+        dec.generate_batch([[1, 2, 3]], 4)
+    with pytest.raises(ValueError, match='tensor parallelism'):
+        dec.prefill_batch([[1, 2, 3]])
