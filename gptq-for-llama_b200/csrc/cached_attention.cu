@@ -225,10 +225,7 @@ cudaError_t launch_cached_attention(const void* q, int64_t ldq, const void* k_ca
     if (!make_kmajor_tensor_map(&tmQ, q, M, n_heads * kHeadDim, ldq) || !make_kmajor_tensor_map(&tmK, k_cache, kv_rows, kHeadDim, kHeadDim) ||
         !make_kmajor_tensor_map(&tmV, v_cache, kv_rows, kHeadDim, kHeadDim))
         return cudaErrorNotSupported;
-    cudaError_t e = cudaFuncSetAttribute(cached_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e != cudaSuccess) return e;
-    cached_attention_kernel<<<dim3(tiles, n_heads), kThreads, kSmemBytes, stream>>>(tmQ, tmK, tmV, p);
-    return cudaGetLastError();
+    return launch_kernel(cached_attention_kernel, dim3(tiles, n_heads), dim3(kThreads), kSmemBytes, stream, false, tmQ, tmK, tmV, p);
 }
 
 }  // namespace gptq

@@ -10,7 +10,6 @@ using namespace gptq;
 namespace {
 
 inline bool bits_ok(int bits) { return bits == 2 || bits == 3 || bits == 4 || bits == 8; }
-inline bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
 int check_weight(const gptq_qweight* w) {
     if (w == nullptr) return GPTQ_ERR_NULL;
@@ -63,7 +62,7 @@ static int run_qlinear(const QLinearArgs& a) {
     if (skinny_supported(a)) {
         const size_t need = skinny_workspace_bytes(a.M, a.w.K, a.w.N, a.dual);
         if (a.workspace == nullptr || a.ws_bytes < need) return GPTQ_ERR_WORKSPACE;
-        if ((reinterpret_cast<uintptr_t>(a.workspace) & 255) != 0) return GPTQ_ERR_ALIGN;
+        if (!aligned(a.workspace, 256)) return GPTQ_ERR_ALIGN;
         return cuda_status(launch_qlinear_skinny(a, false));
     }
     if (gemm_tc_supported(a)) return cuda_status(launch_qlinear_gemm_tc(a));

@@ -18,30 +18,12 @@ constexpr int kAttnChunk = 256;    // keys per attention CTA
 constexpr int kAttnThreads = 128;  // 16 groups of 8 lanes; a group owns one key at a time
 constexpr int kHeadDim = 128;
 
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-// Launch with the programmatic-dependent-launch attribute: the kernel may start while its predecessor drains; every
-// kernel calls pdl_wait() before it touches anything another kernel produces or still reads.
-template <typename... KArgs, typename... Args>
-cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
+// Every kernel of the chain is launched with programmatic dependent launch (launch_kernel's pdl).
 
 __global__ void embed_kernel(const __half* __restrict__ embed, const int32_t* __restrict__ tokens, __half* __restrict__ x, int hidden, int vocab) {
     const int b = blockIdx.x;
-    pdl_trigger();
-    pdl_wait();
+    grid_launch_dependents();
+    grid_dependency_wait();
     const uint4* src = reinterpret_cast<const uint4*>(embed + (size_t)min(max(tokens[b], 0), vocab - 1) * hidden);
     uint4* dst = reinterpret_cast<uint4*>(x + (size_t)b * hidden);
     for (int i = threadIdx.x; i < hidden / 8; i += blockDim.x) dst[i] = __ldg(src + i);
@@ -49,8 +31,8 @@ __global__ void embed_kernel(const __half* __restrict__ embed, const int32_t* __
 
 __global__ void residual_add_kernel(__half* __restrict__ x, const __half* __restrict__ y, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    pdl_trigger();
-    pdl_wait();
+    grid_launch_dependents();
+    grid_dependency_wait();
     if (i < n) x[i] = __hadd(x[i], y[i]);
 }
 
@@ -62,8 +44,8 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half*
                                                                    __half* __restrict__ v_cache, const int32_t* __restrict__ positions, int n_heads, int max_seq,
                                                                    int batch, float inv_base, float scale, float* __restrict__ part, int nsplit) {
     const int head = blockIdx.x, split = blockIdx.y, b = blockIdx.z;
-    pdl_trigger();
-    pdl_wait();
+    grid_launch_dependents();
+    grid_dependency_wait();
     const int pos = min(max(positions[b], 0), max_seq - 1);  // the host rejects positions outside the cache; never write past it
     const int T = pos + 1;
     const int c0 = split * kAttnChunk;
@@ -83,7 +65,7 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half*
     __half* vc = v_cache + ((size_t)(b * n_heads + head) * max_seq) * kHeadDim;
 
     if (tid < 64) {
-        const float f = expf((float)tid * inv_base) * (float)pos;
+        const float f = rope_inv_freq(tid, inv_base) * (float)pos;
         cs_s[tid] = cosf(f);
         cs_s[64 + tid] = sinf(f);
     }
@@ -93,11 +75,11 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half*
         const float c = cs_s[i], s = cs_s[64 + i];
         const bool hi = tid >= 64;  // element i (x part) or i + 64 (y part)
         const float qx = __half2float(q[i]), qy = __half2float(q[i + 64]);
-        const float qr = hi ? __fadd_rn(__fmul_rn(qx, s), __fmul_rn(qy, c)) : __fsub_rn(__fmul_rn(qx, c), __fmul_rn(qy, s));
+        const float qr = hi ? rope_y(qx, qy, c, s) : rope_x(qx, qy, c, s);
         q_s[tid] = __half2float(__float2half_rn(qr));  // the reference stores the rotated q as fp16
         if (pos >= c0 && pos < c1) {                   // this CTA owns the new key/value: append them
             const float kx = __half2float(k[i]), ky = __half2float(k[i + 64]);
-            const float kr = hi ? __fadd_rn(__fmul_rn(kx, s), __fmul_rn(ky, c)) : __fsub_rn(__fmul_rn(kx, c), __fmul_rn(ky, s));
+            const float kr = hi ? rope_y(kx, ky, c, s) : rope_x(kx, ky, c, s);
             kc[(size_t)pos * kHeadDim + tid] = __float2half_rn(kr);
             vc[(size_t)pos * kHeadDim + tid] = v[tid];
         }
@@ -185,8 +167,8 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half*
 __global__ void __launch_bounds__(kHeadDim) attn_combine_kernel(const float* __restrict__ part, const int32_t* __restrict__ positions, __half* __restrict__ out,
                                                                 int hidden, int n_heads, int nsplit) {
     const int head = blockIdx.x, b = blockIdx.y, d = threadIdx.x;
-    pdl_trigger();
-    pdl_wait();
+    grid_launch_dependents();
+    grid_dependency_wait();
     const int nvalid = min(nsplit, max(positions[b], 0) / kAttnChunk + 1);
     const float* src = part + ((size_t)(b * n_heads + head) * nsplit) * (kHeadDim + 2);
     float M = -INFINITY;
@@ -210,8 +192,8 @@ __global__ void __launch_bounds__(256) lm_head_kernel(const __half* __restrict__
     __half* xs = reinterpret_cast<__half*>(smem_raw);  // [batch][hidden] normalised
     __shared__ float red[8];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    pdl_trigger();
-    pdl_wait();
+    grid_launch_dependents();
+    grid_dependency_wait();
     for (int b = 0; b < batch; ++b) {
         const __half2* xr = reinterpret_cast<const __half2*>(x + (size_t)b * hidden);
         float ss = 0.f;
@@ -226,11 +208,10 @@ __global__ void __launch_bounds__(256) lm_head_kernel(const __half* __restrict__
         float tot = 0.f;
 #pragma unroll
         for (int w = 0; w < 8; ++w) tot += red[w];
-        const float rstd = 1.0f / sqrtf(tot / (float)hidden + eps);
+        const float rstd = rms_rstd(tot, hidden, eps);
         for (int i = tid; i < hidden / 2; i += 256) {
-            const float2 f = __half22float2(xr[i]);
-            const float2 g = __half22float2(reinterpret_cast<const __half2*>(norm_w)[i]);
-            reinterpret_cast<__half2*>(xs + (size_t)b * hidden)[i] = __floats2half2_rn(__fmul_rn(__fmul_rn(f.x, rstd), g.x), __fmul_rn(__fmul_rn(f.y, rstd), g.y));
+            reinterpret_cast<__half2*>(xs + (size_t)b * hidden)[i] =
+                rms_apply2(__half22float2(xr[i]), rstd, __half22float2(reinterpret_cast<const __half2*>(norm_w)[i]));
         }
         __syncthreads();
     }
@@ -271,29 +252,21 @@ __global__ void __launch_bounds__(256) lm_head_kernel(const __half* __restrict__
 
 __global__ void __launch_bounds__(1024) argmax_kernel(const __half* __restrict__ logits, int vocab, int32_t* __restrict__ out) {
     const int b = blockIdx.x;
-    pdl_trigger();
-    pdl_wait();
+    grid_launch_dependents();
+    grid_dependency_wait();
     const __half* row = logits + (size_t)b * vocab;
     float best = -INFINITY;
     int idx = 0x7fffffff;
     for (int i = threadIdx.x; i < vocab; i += 1024) {
         const float v = __half2float(row[i]);
-        if (v > best || (v == best && i < idx)) {
+        if (GPTQ_ARGMAX_BEATS(v, i, best, idx)) {
             best = v;
             idx = i;
         }
     }
     __shared__ float sv[32];
     __shared__ int si[32];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-        if (ov > best || (ov == best && oi < idx)) {
-            best = ov;
-            idx = oi;
-        }
-    }
+    GPTQ_WARP_ARGMAX(best, idx);
     if ((threadIdx.x & 31) == 0) {
         sv[threadIdx.x >> 5] = best;
         si[threadIdx.x >> 5] = idx;
@@ -302,20 +275,10 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const __half* __restrict__
     if (threadIdx.x < 32) {
         best = sv[threadIdx.x];
         idx = si[threadIdx.x];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-            if (ov > best || (ov == best && oi < idx)) {
-                best = ov;
-                idx = oi;
-            }
-        }
+        GPTQ_WARP_ARGMAX(best, idx);
         if (threadIdx.x == 0) out[b] = idx;
     }
 }
-
-inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 struct ScratchLayout {
     size_t x, qkv, attn, h, xn, tmp, part, ws, mega, total;
@@ -326,29 +289,22 @@ struct ScratchLayout {
 ScratchLayout scratch_layout(const gptq_llama_model& m, int batch, int max_seq) {
     ScratchLayout L{};
     const size_t wide = (size_t)max(m.intermediate, 3 * m.hidden);
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        const size_t o = off;
-        off += align256(bytes);
-        return o;
-    };
     L.nsplit = ceil_div(max_seq, kAttnChunk);
-    L.x = take((size_t)batch * m.hidden * 2);
-    L.qkv = take((size_t)batch * 3 * m.hidden * 2);
-    L.attn = take((size_t)batch * m.hidden * 2);
-    L.h = take((size_t)batch * m.intermediate * 2);
-    L.xn = take((size_t)batch * wide * 2);
-    L.tmp = take((size_t)batch * wide * 2);
-    L.part = take((size_t)batch * m.n_heads * L.nsplit * (kHeadDim + 2) * sizeof(float));
+    L.x = carve(L.total, (size_t)batch * m.hidden * 2);
+    L.qkv = carve(L.total, (size_t)batch * 3 * m.hidden * 2);
+    L.attn = carve(L.total, (size_t)batch * m.hidden * 2);
+    L.h = carve(L.total, (size_t)batch * m.intermediate * 2);
+    L.xn = carve(L.total, (size_t)batch * wide * 2);
+    L.tmp = carve(L.total, (size_t)batch * wide * 2);
+    L.part = carve(L.total, (size_t)batch * m.n_heads * L.nsplit * (kHeadDim + 2) * sizeof(float));
     size_t ws = 0;
     ws = max(ws, skinny_workspace_bytes(batch, m.hidden, 3 * m.hidden, false));
     ws = max(ws, skinny_workspace_bytes(batch, m.hidden, m.hidden, false));
     ws = max(ws, skinny_workspace_bytes(batch, m.hidden, m.intermediate, true));
     ws = max(ws, skinny_workspace_bytes(batch, m.intermediate, m.hidden, false));
     L.ws_bytes = ws;
-    L.ws = take(ws);
-    L.mega = take(mega_scratch_bytes(m, batch));
-    L.total = off;
+    L.ws = carve(L.total, ws);
+    L.mega = carve(L.total, mega_scratch_bytes(m, batch));
     return L;
 }
 
@@ -403,8 +359,8 @@ cudaError_t engine_linear(const ChainLinear& c, uint8_t* scratch, const ScratchL
     if (a.residual != nullptr) {
         // residual and out are the same buffer in the engine (in-place x += f(x))
         const int n = a.M * a.w.N;
-        return launch_pdl(residual_add_kernel, dim3(ceil_div(n, 256)), dim3(256), 0, a.stream, reinterpret_cast<__half*>(a.out),
-                          reinterpret_cast<const __half*>(scratch + L.tmp), n);
+        return launch_kernel(residual_add_kernel, dim3(ceil_div(n, 256)), dim3(256), 0, a.stream, true, reinterpret_cast<__half*>(a.out),
+                             reinterpret_cast<const __half*>(scratch + L.tmp), n);
     }
     return cudaSuccess;
 }
@@ -451,7 +407,7 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
     if (st->batch < 1 || st->batch > 8 || st->max_seq < 1) return GPTQ_ERR_SHAPE;
     const ScratchLayout L = scratch_layout(m, st->batch, st->max_seq);
     if (st->scratch_bytes < L.total) return GPTQ_ERR_WORKSPACE;
-    if ((reinterpret_cast<uintptr_t>(st->scratch) & 255) != 0) return GPTQ_ERR_ALIGN;
+    if (!aligned(st->scratch, 256)) return GPTQ_ERR_ALIGN;
     for (int l = 0; l < m.n_layers; ++l) {
         const gptq_llama_layer& ly = m.layers[l];
         if (ly.qkv.K != m.hidden || ly.qkv.N != 3 * Hq || ly.o.K != Hq || ly.o.N != m.hidden || ly.gate.K != m.hidden ||
@@ -473,8 +429,8 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
     __half* attn = reinterpret_cast<__half*>(sc + L.attn);
     float* part = reinterpret_cast<float*>(sc + L.part);
     const int B = st->batch, H = m.hidden;
-    const float inv_base = (float)(-2.0 * log((double)m.rope_base) / (double)m.head_dim);
-    const float scale = 1.0f / sqrtf((float)m.head_dim);
+    const float inv_base = rope_inv_base(m.rope_base, m.head_dim);
+    const float scale = attn_scale(m.head_dim);
     const size_t layer_stride = (size_t)B * m.n_heads * st->max_seq * m.head_dim;
 
 #define GPTQ_TRY(expr)                                   \
@@ -482,31 +438,22 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
         if ((expr) != cudaSuccess) return GPTQ_ERR_CUDA; \
     } while (0)
 
-    GPTQ_TRY(launch_pdl(embed_kernel, dim3(B), dim3(256), 0, stream, reinterpret_cast<const __half*>(m.embed), st->tokens, x, H, m.vocab));
+    GPTQ_TRY(launch_kernel(embed_kernel, dim3(B), dim3(256), 0, stream, true, reinterpret_cast<const __half*>(m.embed), st->tokens, x, H, m.vocab));
     for (int l = 0; l < m.n_layers; ++l) {
         ChainLinear c[4];
         chain_linears(m, m.layers[l], *st, L, stream, c);
         GPTQ_TRY(engine_linear(c[0], sc, L));
-        GPTQ_TRY(launch_pdl(attn_decode_kernel, dim3(m.n_heads, L.nsplit, B), dim3(kAttnThreads), 0, stream, qkv, H,
-                            reinterpret_cast<__half*>(st->k_cache) + l * layer_stride, reinterpret_cast<__half*>(st->v_cache) + l * layer_stride, st->positions,
-                            m.n_heads, st->max_seq, B, inv_base, scale, part, L.nsplit));
-        GPTQ_TRY(launch_pdl(attn_combine_kernel, dim3(m.n_heads, B), dim3(kHeadDim), 0, stream, part, st->positions, attn, H, m.n_heads, L.nsplit));
+        GPTQ_TRY(launch_kernel(attn_decode_kernel, dim3(m.n_heads, L.nsplit, B), dim3(kAttnThreads), 0, stream, true, qkv, H,
+                               reinterpret_cast<__half*>(st->k_cache) + l * layer_stride, reinterpret_cast<__half*>(st->v_cache) + l * layer_stride,
+                               st->positions, m.n_heads, st->max_seq, B, inv_base, scale, part, L.nsplit));
+        GPTQ_TRY(launch_kernel(attn_combine_kernel, dim3(m.n_heads, B), dim3(kHeadDim), 0, stream, true, part, st->positions, attn, H, m.n_heads, L.nsplit));
         for (int i = 1; i < 4; ++i) GPTQ_TRY(engine_linear(c[i], sc, L));
     }
-    {
-        const size_t smem = (size_t)B * H * sizeof(__half);
-        const int grid = min(ceil_div(m.vocab, 8), kNumSMs * 8);
-        if (smem > 48 * 1024) GPTQ_TRY(cudaFuncSetAttribute(lm_head_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const __half* fn = reinterpret_cast<const __half*>(m.final_norm);
-        const __half* lw = reinterpret_cast<const __half*>(m.lm_head);
-        __half* lg = reinterpret_cast<__half*>(st->logits);
-        if (B == 1)
-            GPTQ_TRY(launch_pdl(lm_head_kernel<1>, dim3(grid), dim3(256), smem, stream, (const __half*)x, fn, m.rms_eps, lw, lg, H, m.vocab, B));
-        else
-            GPTQ_TRY(launch_pdl(lm_head_kernel<8>, dim3(grid), dim3(256), smem, stream, (const __half*)x, fn, m.rms_eps, lw, lg, H, m.vocab, B));
-    }
+    GPTQ_TRY(launch_kernel(B == 1 ? lm_head_kernel<1> : lm_head_kernel<8>, dim3(min(ceil_div(m.vocab, 8), kNumSMs * 8)), dim3(256),
+                           (size_t)B * H * sizeof(__half), stream, true, (const __half*)x, reinterpret_cast<const __half*>(m.final_norm), m.rms_eps,
+                           reinterpret_cast<const __half*>(m.lm_head), reinterpret_cast<__half*>(st->logits), H, m.vocab, B));
     if (st->next_tokens != nullptr) {
-        GPTQ_TRY(launch_pdl(argmax_kernel, dim3(B), dim3(1024), 0, stream, reinterpret_cast<const __half*>(st->logits), m.vocab, st->next_tokens));
+        GPTQ_TRY(launch_kernel(argmax_kernel, dim3(B), dim3(1024), 0, stream, true, reinterpret_cast<const __half*>(st->logits), m.vocab, st->next_tokens));
     }
 #undef GPTQ_TRY
     return GPTQ_OK;

@@ -38,12 +38,10 @@
 // per-sequence vector (residual stream, accumulators, staged x and its step sums, RoPE angles, logits) gets a [B] dimension; the
 // attention teams are dealt to (sequence, head) pairs in proportion to each sequence's context (seq_teams).  Batch 1 is the
 // !BATCH instantiation: its loops over the sequences have the compile-time count 1.
-#include <cuda.h>
-#include <cudaTypedefs.h>
-
 #include "common.cuh"
 #include "int4_core.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace gptq {
 namespace {
@@ -632,7 +630,7 @@ __device__ void stage_norm(const MegaParams& p, const __half* src, const float* 
     }
     uint32_t m = max(xm & 0xffffu, xm >> 16) | (max(wm & 0xffffu, wm >> 16) << 16);
     const float tot = block_sum(ss, m, red_s);  // its barriers also publish tmp
-    const float rstd = 1.0f / sqrtf(tot / (float)H + p.eps);
+    const float rstd = rms_rstd(tot, H, p.eps);
     XScale sc{1.f, 1.f, 1.f};
     if constexpr (!PLAIN) {
         sc = x_scale(__half2float(__ushort_as_half((unsigned short)(m & 0xffffu))) * rstd * __half2float(__ushort_as_half((unsigned short)(m >> 16))) * 1.001f);
@@ -671,9 +669,9 @@ __device__ void stage_norm(const MegaParams& p, const __half* src, const float* 
             const uint32_t wv[4] = {nwv[i].x, nwv[i].y, nwv[i].z, nwv[i].w};
             uint32_t o[4];
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {  // fp32 normalise, fp32 weight multiply, one rounding to fp16 (quant/triton_norm.py:30-38)
+            for (int j = 0; j < 4; ++j) {
                 const float2 wf = __half22float2(u32_as_h2(wv[j]));
-                o[j] = h2_as_u32(__floats2half2_rn(__fmul_rn(__fmul_rn(xf[2 * j], rstd), wf.x), __fmul_rn(__fmul_rn(xf[2 * j + 1], rstd), wf.y)));
+                o[j] = h2_as_u32(rms_apply2(make_float2(xf[2 * j], xf[2 * j + 1]), rstd, wf));
             }
             if constexpr (PLAIN) {
                 *reinterpret_cast<uint4*>(xs + c * 8) = make_uint4(o[0], o[1], o[2], o[3]);
@@ -1100,13 +1098,13 @@ __device__ void run_attention(const MegaParams& p, ConsRing& ring, const TeamCtx
             const float c = ld_cg(p.rope_cs + seq * kHD + i), s = ld_cg(p.rope_cs + seq * kHD + 64 + i);
             const float* aq = p.acc_qkv + (size_t)seq * 3 * p.Hq + head * kHD;
             const float qx = __half2float(__float2half_rn(ld_cg(aq + i))), qy = __half2float(__float2half_rn(ld_cg(aq + i + 64)));  // the qkv projection output is fp16
-            const float qr = hi ? __fadd_rn(__fmul_rn(qx, s), __fmul_rn(qy, c)) : __fsub_rn(__fmul_rn(qx, c), __fmul_rn(qy, s));
+            const float qr = hi ? rope_y(qx, qy, c, s) : rope_x(qx, qy, c, s);
             q_s[ttid] = __half2float(__float2half_rn(qr));
             if (owns_new) {  // this segment owns the new key/value: RoPE(k), append both to the cache
                 const float* ak = aq + p.Hq;
                 const float* av = aq + 2 * p.Hq;
                 const float kx = __half2float(__float2half_rn(ld_cg(ak + i))), ky = __half2float(__float2half_rn(ld_cg(ak + i + 64)));
-                const float kr = hi ? __fadd_rn(__fmul_rn(kx, s), __fmul_rn(ky, c)) : __fsub_rn(__fmul_rn(kx, c), __fmul_rn(ky, s));
+                const float kr = hi ? rope_y(kx, ky, c, s) : rope_x(kx, ky, c, s);
                 const __half kh = __float2half_rn(kr), vh = __float2half_rn(ld_cg(av + ttid));
                 knew[ttid] = kh;
                 vnew[ttid] = vh;
@@ -1354,22 +1352,14 @@ __device__ __forceinline__ void argmax_row(const __half* row, int V, int32_t* ou
     int idx = 0x7fffffff;
     for (int i = tid; i < V; i += kConsumers) {
         const float v = __half2float(ld_cg_h(row + i));  // written by other CTAs
-        if (v > best || (v == best && i < idx)) {
+        if (GPTQ_ARGMAX_BEATS(v, i, best, idx)) {
             best = v;
             idx = i;
         }
     }
     __shared__ float sv[kConsumerWarps];
     __shared__ int si[kConsumerWarps];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-        if (ov > best || (ov == best && oi < idx)) {
-            best = ov;
-            idx = oi;
-        }
-    }
+    GPTQ_WARP_ARGMAX(best, idx);
     if (lane == 0) {
         sv[warp] = best;
         si[warp] = idx;
@@ -1377,7 +1367,7 @@ __device__ __forceinline__ void argmax_row(const __half* row, int V, int32_t* ou
     cta_sync();
     if (tid == 0) {
         for (int w = 1; w < kConsumerWarps; ++w)
-            if (sv[w] > best || (sv[w] == best && si[w] < idx)) {
+            if (GPTQ_ARGMAX_BEATS(sv[w], si[w], best, idx)) {
                 best = sv[w];
                 idx = si[w];
             }
@@ -1483,7 +1473,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
     // this step's RoPE angles, one row per sequence (quant/fused_attn.py:43,91): freq_i = exp(i * inv_base) * pos
     if (blockIdx.x == 0 && tid < 64 * nbat) {
         const int s = tid >> 6, i = tid & 63;
-        const float f = expf((float)i * p.inv_base) * (float)step_pos(p, s);
+        const float f = rope_inv_freq(i, p.inv_base) * (float)step_pos(p, s);
         p.rope_cs[s * kHD + i] = cosf(f);
         p.rope_cs[s * kHD + 64 + i] = sinf(f);
     }
@@ -1591,22 +1581,13 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
     if ((int)blockIdx.x < nbat && p.next_token != nullptr) argmax_row(p.logits + (size_t)blockIdx.x * p.V, p.V, p.next_token + blockIdx.x);  // CTA s: sequence s
 }
 
-inline size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 // 3-D view of packed matrices with row stride N * 4 bytes: {32 words (128 B), packed rows, 128-byte chunks}, box 32 x box_rows x 8
-// (= box_rows rows of a 256-column slab), 128-byte swizzle.  cuTensorMapEncodeTiled comes through the runtime's driver entry
-// point (libcuda is not linked: the library must load without a driver).
+// (= box_rows rows of a 256-column slab), 128-byte swizzle
 bool encode_weight_map(CUtensorMap* tm, const void* base, int rows, uint64_t chunks, int N, int box_rows) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess || fn == nullptr) return false;
-    const auto encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled>(fn);
     const cuuint64_t dims[3] = {32, (cuuint64_t)rows, (cuuint64_t)chunks};  // innermost first
     const cuuint64_t strides[2] = {(cuuint64_t)N * 4, 128};                 // bytes: packed row, chunk
     const cuuint32_t box[3] = {32, (cuuint32_t)box_rows, (cuuint32_t)(kSlabCols / 32)};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    return encode(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    return encode_tensor_map(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, base, dims, strides, box);
 }
 
 // device properties that shape the launch (queried per call: no cached global state)
@@ -1663,24 +1644,19 @@ struct MegaScratch {
 MegaScratch mega_scratch(const gptq_llama_model& m, int batch) {
     const size_t B = (size_t)batch, H = (size_t)m.hidden, I = (size_t)m.intermediate;
     MegaScratch s{};
-    auto take = [&](size_t bytes) {
-        const size_t o = s.total;
-        s.total += al256(bytes);
-        return o;
-    };
-    s.resid[0] = take(B * H * 2);
-    s.resid[1] = take(B * H * 2);
-    s.acc_o = take(B * H * 4);
-    s.acc_d = take(B * H * 4);
-    s.xbar = take((kMaxTP + 1) * 256);
-    s.acc_o_loc = take(H * 4);
-    s.acc_d_loc = take(H * 4);
-    s.acc_qkv = take(B * 3 * H * 4);
-    s.acc_g = take(B * I * 4);
-    s.acc_u = take(B * I * 4);
-    s.part = take((size_t)kMaxTeams * kRec * 4);
-    s.rope_cs = take(B * 128 * 4);
-    s.bar = take(256);
+    s.resid[0] = carve(s.total, B * H * 2);
+    s.resid[1] = carve(s.total, B * H * 2);
+    s.acc_o = carve(s.total, B * H * 4);
+    s.acc_d = carve(s.total, B * H * 4);
+    s.xbar = carve(s.total, (kMaxTP + 1) * 256);
+    s.acc_o_loc = carve(s.total, H * 4);
+    s.acc_d_loc = carve(s.total, H * 4);
+    s.acc_qkv = carve(s.total, B * 3 * H * 4);
+    s.acc_g = carve(s.total, B * I * 4);
+    s.acc_u = carve(s.total, B * I * 4);
+    s.part = carve(s.total, (size_t)kMaxTeams * kRec * 4);
+    s.rope_cs = carve(s.total, B * 128 * 4);
+    s.bar = carve(s.total, 256);
     return s;
 }
 
@@ -1714,12 +1690,11 @@ cudaError_t mega_step_plan(const gptq_llama_model& m, const gptq_llama_state& st
         const gptq_qweight* ws[5] = {&ly.qkv, &ly.o, &ly.gate, &ly.up, &ly.down};
         for (const gptq_qweight* w : ws) {
             if (w->bits != 4 || w->groupsize <= 0 || w->groupsize % 32) return kNo;
-            if ((reinterpret_cast<uintptr_t>(w->qweight) & 15) || (reinterpret_cast<uintptr_t>(w->scales) & 15) || (reinterpret_cast<uintptr_t>(w->qzeros) & 15))
-                return kNo;
+            if (!aligned(w->qweight, 16) || !aligned(w->scales, 16) || !aligned(w->qzeros, 16)) return kNo;
         }
         if (ly.gate.groupsize != ly.up.groupsize) return kNo;
     }
-    if ((reinterpret_cast<uintptr_t>(m.lm_head) & 15) || (reinterpret_cast<uintptr_t>(st.k_cache) & 15) || (reinterpret_cast<uintptr_t>(st.v_cache) & 15)) return kNo;
+    if (!aligned(m.lm_head, 16) || !aligned(st.k_cache, 16) || !aligned(st.v_cache, 16)) return kNo;
     // the staging buffers of this batch must fit the current device
     int dev = 0, sms = 0, smem_optin = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
@@ -1757,8 +1732,8 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     p.n_stages = pl.n_stages;
     p.lm_rows = pl.lm_rows;
     p.eps = m.rms_eps;
-    p.inv_base = (float)(-2.0 * log((double)m.rope_base) / (double)m.head_dim);
-    p.scale = 1.0f / sqrtf((float)m.head_dim);
+    p.inv_base = rope_inv_base(m.rope_base, m.head_dim);
+    p.scale = attn_scale(m.head_dim);
     p.embed = reinterpret_cast<const __half*>(m.embed);
     p.final_norm = reinterpret_cast<const __half*>(m.final_norm);
     p.lm_head = reinterpret_cast<const __half*>(m.lm_head);
@@ -1812,7 +1787,7 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
         visit(ly.qkv, 0); visit(ly.o, 1); visit(ly.down, 1); visit(ly.gate, 2); visit(ly.up, 2);
     }
     for (int c = 0; c < 3; ++c) {
-        if ((base[c] & 127) != 0) return cudaErrorInvalidConfiguration;
+        if (!aligned(reinterpret_cast<const void*>(base[c]), 128)) return cudaErrorInvalidConfiguration;
         const uint64_t chunks = (uint64_t)(top[c] - base[c]) / 128 + (uint64_t)classN[c] / 32;
         if (chunks >= (1ull << 31)) return cudaErrorInvalidConfiguration;
         for (int v = 0; v < 2; ++v)
@@ -1821,7 +1796,7 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     }
     for (int l = 0; l < m.n_layers; ++l) {
         const gptq_llama_layer& ly = m.layers[l];
-        bool aligned = true;
+        bool whole_chunks = true;
         auto md = [&](const gptq_qweight& w, int c) {
             MatDesc d;
             d.sc = reinterpret_cast<const __half*>(w.scales);
@@ -1829,7 +1804,7 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
             d.gs_steps = w.groupsize / 32;
             d.tmap = c;
             const uintptr_t delta = reinterpret_cast<uintptr_t>(w.qweight) - base[c];
-            aligned = aligned && (delta % 128 == 0);
+            whole_chunks = whole_chunks && (delta % 128 == 0);
             d.chunk0 = (int)(delta / 128);
             return d;
         };
@@ -1838,7 +1813,7 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
         p.layers[l].gate = md(ly.gate, 2);
         p.layers[l].up = md(ly.up, 2);
         p.layers[l].down = md(ly.down, 1);
-        if (!aligned) return cudaErrorInvalidConfiguration;
+        if (!whole_chunks) return cudaErrorInvalidConfiguration;
         p.layers[l].input_norm = reinterpret_cast<const __half*>(ly.input_norm);
         p.layers[l].post_norm = reinterpret_cast<const __half*>(ly.post_norm);
         p.layers[l].qkv_perm = ly.qkv_perm;

@@ -5,9 +5,7 @@
 namespace gptq {
 namespace {
 
-// rotate_half_kernel (quant/fused_attn.py:8-58): one block per token, threads over (row, i).
-//   freq_i = exp(i * inv_base) * pos  (fp32, accurate exp: the reference insists on libdevice exp, :42-43)
-//   x' = x cos - y sin ; y' = x sin + y cos, y at +head_dim/2 (:52-57); fp32 math, fp16 store.
+// rotate_half_kernel (quant/fused_attn.py:8-58): one block per token, threads over (row, i); fp32 math (common.cuh), fp16 store.
 __global__ void rope_kernel(__half* __restrict__ qk, int64_t token_stride, const int64_t* __restrict__ position_ids, int64_t pos_batch_stride, int seq,
                             int rows, int head_dim, float inv_base) {
     const int token = blockIdx.x;
@@ -20,24 +18,19 @@ __global__ void rope_kernel(__half* __restrict__ qk, int64_t token_stride, const
     for (int idx = threadIdx.x; idx < rows * pairs_per_row; idx += blockDim.x) {
         const int row = idx / pairs_per_row;
         const int i = (idx - row * pairs_per_row) * 2;
-        const float f0 = expf((float)i * inv_base) * pos;
-        const float f1 = expf((float)(i + 1) * inv_base) * pos;
+        const float f0 = rope_inv_freq(i, inv_base) * pos, f1 = rope_inv_freq(i + 1, inv_base) * pos;
         const float c0 = cosf(f0), s0 = sinf(f0), c1 = cosf(f1), s1 = sinf(f1);
         __half2* px = reinterpret_cast<__half2*>(base + (size_t)row * head_dim + i);
         __half2* py = reinterpret_cast<__half2*>(base + (size_t)row * head_dim + half_dim + i);
         const float2 xv = __half22float2(*px), yv = __half22float2(*py);
-        // keep the reference's operation order; contraction into FMA is prevented to stay at 2 roundings per term
-        const float ox0 = __fsub_rn(__fmul_rn(xv.x, c0), __fmul_rn(yv.x, s0));
-        const float ox1 = __fsub_rn(__fmul_rn(xv.y, c1), __fmul_rn(yv.y, s1));
-        const float oy0 = __fadd_rn(__fmul_rn(xv.x, s0), __fmul_rn(yv.x, c0));
-        const float oy1 = __fadd_rn(__fmul_rn(xv.y, s1), __fmul_rn(yv.y, c1));
+        const float ox0 = rope_x(xv.x, yv.x, c0, s0), ox1 = rope_x(xv.y, yv.y, c1, s1);
+        const float oy0 = rope_y(xv.x, yv.x, c0, s0), oy1 = rope_y(xv.y, yv.y, c1, s1);
         *px = __floats2half2_rn(ox0, ox1);
         *py = __floats2half2_rn(oy0, oy1);
     }
 }
 
-// rms_norm_fwd_fused (quant/triton_norm.py:7-39): one block per row; variance in fp32,
-// y = (x * rstd) * w in fp32 (two roundings, like the reference), fp16 store.
+// rms_norm_fwd_fused (quant/triton_norm.py:7-39): one block per row; variance in fp32, y = fp16((x * rstd) * w) (common.cuh).
 template <int THREADS>
 __global__ void __launch_bounds__(THREADS) rmsnorm_kernel(const __half* __restrict__ x, int64_t ldx, const __half* __restrict__ w, __half* __restrict__ y,
                                                           int64_t ldy, int N, float eps) {
@@ -60,14 +53,12 @@ __global__ void __launch_bounds__(THREADS) rmsnorm_kernel(const __half* __restri
     if (threadIdx.x < 32) {
         float t = threadIdx.x < THREADS / 32 ? part[threadIdx.x] : 0.f;
         t = warp_sum(t);
-        if (threadIdx.x == 0) rstd_s = 1.0f / sqrtf(t / (float)N + eps);
+        if (threadIdx.x == 0) rstd_s = rms_rstd(t, N, eps);
     }
     __syncthreads();
     const float rstd = rstd_s;
     for (int i = threadIdx.x; i < n2; i += THREADS) {
-        const float2 v = __half22float2(xr[i]);
-        const float2 g = __half22float2(__ldg(wr + i));
-        yr[i] = __floats2half2_rn(__fmul_rn(__fmul_rn(v.x, rstd), g.x), __fmul_rn(__fmul_rn(v.y, rstd), g.y));
+        yr[i] = rms_apply2(__half22float2(xr[i]), rstd, __half22float2(__ldg(wr + i)));
     }
 }
 
@@ -75,11 +66,10 @@ __global__ void __launch_bounds__(THREADS) rmsnorm_kernel(const __half* __restri
 
 cudaError_t launch_rope(void* qk, int64_t token_stride, const int64_t* position_ids, int64_t pos_batch_stride, int bsz, int seq, int rows, int head_dim,
                         float base, cudaStream_t stream) {
-    const float inv_base = (float)(-2.0 * log((double)base) / (double)head_dim);  // quant/fused_attn.py:91
     const int work = rows * (head_dim / 4);
     const int threads = work >= 256 ? 256 : ((work + 31) / 32) * 32;
     rope_kernel<<<bsz * seq, threads, 0, stream>>>(reinterpret_cast<__half*>(qk), token_stride, position_ids, pos_batch_stride, seq, rows, head_dim,
-                                                    inv_base);
+                                                    rope_inv_base(base, head_dim));
     return cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-// Device helpers shared by the int4 decode kernels (qmatvec.cu, decode_mega.cu): asynchronous staging,
+// Device helpers shared by the int4 kernels (qmatvec.cu, decode_mega.cu, qgemm_wgmma.cu, qgemm_wgmma_t.cu): asynchronous staging,
 // reference-exact int4 -> fp16 dequantisation, and the swapped-operand m16n8k16 tensor-core dot.
 #pragma once
 #include "common.cuh"
@@ -89,8 +89,6 @@ __device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
-__device__ __forceinline__ void grid_dependency_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void grid_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 __device__ __forceinline__ uint32_t h2_as_u32(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
 __device__ __forceinline__ __half2 u32_as_h2(uint32_t u) { return *reinterpret_cast<__half2*>(&u); }
@@ -165,6 +163,24 @@ __device__ __forceinline__ void dequant8(uint32_t q, __half2 za_pair, __half2 zb
     w[3] = h2_as_u32(__hmul2(__hfma2(h1, sixteenth, zb), s));
 }
 
+// dequant8's zero constants of one column from its qzeros word: za = 1024 + z, zb = -(64 + z)
+__device__ __forceinline__ void zero_consts(uint32_t zw, int zshift, __half2& za, __half2& zb) {
+    const float z = (float)(((zw >> zshift) & 0xfu) + 1u);  // stored minus one, +1 unmasked (quant_linear.py:120-121)
+    za = __float2half2_rn(1024.f + z);
+    zb = __float2half2_rn(-(64.f + z));
+}
+
+// one packed word (8 consecutive k of one column) dequantised into a 16-byte chunk of halves in natural k order (a wgmma B-tile chunk)
+__device__ __forceinline__ uint4 dequant_chunk(uint32_t q, __half2 za, __half2 zb, __half2 s) {
+    uint32_t v[4];  // (k0,k4) (k1,k5) (k2,k6) (k3,k7)
+    dequant8<0>(q, za, zb, s, v);
+    uint4 o;
+    o.x = __byte_perm(v[0], v[1], 0x5410);  // (k0,k1)
+    o.y = __byte_perm(v[2], v[3], 0x5410);  // (k2,k3)
+    o.z = __byte_perm(v[0], v[1], 0x7632);  // (k4,k5)
+    o.w = __byte_perm(v[2], v[3], 0x7632);  // (k6,k7)
+    return o;
+}
 
 }  // namespace int4
 }  // namespace gptq

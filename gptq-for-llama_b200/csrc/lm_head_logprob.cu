@@ -185,7 +185,7 @@ __global__ void __launch_bounds__(32 * kCombineWarps) lm_head_logprob_combine_ke
 size_t lm_head_logprob_workspace_bytes(int M, int V) {
     if (M <= 0 || V <= 0) return 0;
     const size_t part = (size_t)M * ceil_div(V, BN) * sizeof(float2);
-    return (part + (size_t)M * sizeof(float) + 255) & ~(size_t)255;
+    return align256(part + (size_t)M * sizeof(float));
 }
 
 cudaError_t launch_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int K, int V, const int32_t* targets, float* logprob,
@@ -199,10 +199,8 @@ cudaError_t launch_lm_head_logprob(const void* x, int64_t ldx, const void* w, in
     p.tlogit = reinterpret_cast<float*>(p.part + (size_t)M * p.ntiles);
     p.mtiles = ceil_div(M, BM);
     p.M = M, p.K = K, p.V = V;
-    cudaError_t e = cudaFuncSetAttribute(lm_head_logprob_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    const cudaError_t e = launch_kernel(lm_head_logprob_kernel, dim3(p.mtiles * p.ntiles), dim3(kThreads), kSmemBytes, stream, false, tmX, tmW, p);
     if (e != cudaSuccess) return e;
-    lm_head_logprob_kernel<<<p.mtiles * p.ntiles, kThreads, kSmemBytes, stream>>>(tmX, tmW, p);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
     lm_head_logprob_combine_kernel<<<ceil_div(M, kCombineWarps), 32 * kCombineWarps, 0, stream>>>(p, logprob);
     return cudaGetLastError();
 }

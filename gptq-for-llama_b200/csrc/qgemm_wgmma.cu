@@ -102,10 +102,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) qgemm_wgmma_kernel(const __gr
 #pragma unroll
             for (int w = 0; w < NW; ++w) {
                 const __half sv = __ldg(p.sc[w] + (size_t)grp * p.N + col);
-                const uint32_t zw = __ldg(p.qz[w] + (size_t)grp * (p.N >> 3) + (col >> 3));
-                const float z = (float)(((zw >> zshift) & 0xfu) + 1u);  // stored minus one, +1 unmasked (quant_linear.py:120-121)
-                za[w] = __float2half2_rn(1024.f + z);
-                zb[w] = __float2half2_rn(-(64.f + z));
+                zero_consts(__ldg(p.qz[w] + (size_t)grp * (p.N >> 3) + (col >> 3)), zshift, za[w], zb[w]);
                 sc2[w] = __half2half2(sv);
             }
         }
@@ -113,15 +110,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1) qgemm_wgmma_kernel(const __gr
         for (int w = 0; w < NW; ++w) {
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                uint32_t v[4];  // (k0,k4) (k1,k5) (k2,k6) (k3,k7)
-                dequant8<0>(bq[0][w][i], za[w], zb[w], sc2[w], v);
-                uint4 o;
-                o.x = __byte_perm(v[0], v[1], 0x5410);  // (k0,k1)
-                o.y = __byte_perm(v[2], v[3], 0x5410);  // (k2,k3)
-                o.z = __byte_perm(v[0], v[1], 0x7632);  // (k4,k5)
-                o.w = __byte_perm(v[2], v[3], 0x7632);  // (k6,k7)
                 const int c = bc0 + 2 * i;
-                *reinterpret_cast<uint4*>(b_ptr + (s * NW + w) * kTileBytes + bn * 128 + ((c ^ (bn & 7)) << 4)) = o;
+                *reinterpret_cast<uint4*>(b_ptr + (s * NW + w) * kTileBytes + bn * 128 + ((c ^ (bn & 7)) << 4)) =
+                    dequant_chunk(bq[0][w][i], za[w], zb[w], sc2[w]);
             }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to wgmma (async proxy)
@@ -206,17 +197,15 @@ __global__ void __launch_bounds__(kGemmThreads, 1) qgemm_wgmma_kernel(const __gr
     }
 }
 
-inline bool al(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
-
 }  // namespace
 
 bool gemm_tc_supported(const QLinearArgs& a) {
     const gptq_qweight& w = a.w;
     if (w.bits != 4 || a.M <= 8) return false;
-    if (a.dual && (!al(a.w2.qweight, 4))) return false;
+    if (a.dual && (!aligned(a.w2.qweight, 4))) return false;
     if (w.groupsize <= 0 || w.groupsize % BK != 0) return false;
     if (w.N % BN != 0 || w.K % BK != 0) return false;
-    if (!al(a.x, 16) || a.ldx % 8 != 0 || !al(a.out, 16) || a.ldo % 8 != 0) return false;
+    if (!aligned(a.x, 16) || a.ldx % 8 != 0 || !aligned(a.out, 16) || a.ldo % 8 != 0) return false;
     if (a.norm_w != nullptr || a.residual != nullptr) return false;
     return true;
 }
@@ -244,15 +233,8 @@ cudaError_t launch_qlinear_gemm_tc(const QLinearArgs& a) {
     const int nw = a.dual ? 2 : 1;
     const int stages = (wt + nw == 2) ? 6 : 4;
     const size_t smem = 1024 + (size_t)(wt + nw) * stages * kTileBytes;
-    const dim3 grid(a.w.N / BN, ceil_div(a.M, 128 * wt));
-    auto go = [&](auto kernel) -> cudaError_t {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        kernel<<<grid, kGemmThreads, smem, a.stream>>>(tmA, p);
-        return cudaGetLastError();
-    };
-    if (a.dual) return go(qgemm_wgmma_kernel<true, 1, 4>);
-    return wt == 2 ? go(qgemm_wgmma_kernel<false, 2, 4>) : go(qgemm_wgmma_kernel<false, 1, 6>);
+    const auto kernel = a.dual ? qgemm_wgmma_kernel<true, 1, 4> : wt == 2 ? qgemm_wgmma_kernel<false, 2, 4> : qgemm_wgmma_kernel<false, 1, 6>;
+    return launch_kernel(kernel, dim3(a.w.N / BN, ceil_div(a.M, 128 * wt)), dim3(kGemmThreads), smem, a.stream, false, tmA, p);
 }
 
 }  // namespace gptq

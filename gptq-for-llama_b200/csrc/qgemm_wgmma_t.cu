@@ -100,19 +100,13 @@ __global__ void __launch_bounds__(kGemmTThreads, 1) qgemm_wgmma_t_kernel(const _
     // dequantise step j (held in bq[0]) into its stage, then rotate the ring and request step j + kAhead + 1
     auto produce_b = [&](int j) {
         const int s = j % S;
-        const float z = (float)(((bq[0].z >> zshift) & 0xfu) + 1u);  // stored minus one, +1 unmasked (quant_linear.py:120-121)
-        const __half2 za = __float2half2_rn(1024.f + z), zb = __float2half2_rn(-(64.f + z)), sc2 = __half2half2(bq[0].s);
+        __half2 za, zb;
+        zero_consts(bq[0].z, zshift, za, zb);
+        const __half2 sc2 = __half2half2(bq[0].s);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            uint32_t v[4];  // (k0,k4) (k1,k5) (k2,k6) (k3,k7)
-            dequant8<0>(bq[0].q[i], za, zb, sc2, v);
-            uint4 o;
-            o.x = __byte_perm(v[0], v[1], 0x5410);  // (k0,k1)
-            o.y = __byte_perm(v[2], v[3], 0x5410);  // (k2,k3)
-            o.z = __byte_perm(v[0], v[1], 0x7632);  // (k4,k5)
-            o.w = __byte_perm(v[2], v[3], 0x7632);  // (k6,k7)
             const int c = (pr0 & 7) + i;
-            *reinterpret_cast<uint4*>(b_dst + s * kTileBytes + ((c ^ (bn & 7)) << 4)) = o;
+            *reinterpret_cast<uint4*>(b_dst + s * kTileBytes + ((c ^ (bn & 7)) << 4)) = dequant_chunk(bq[0].q[i], za, zb, sc2);
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to wgmma (async proxy)
 #pragma unroll
@@ -171,16 +165,14 @@ __global__ void __launch_bounds__(kGemmTThreads, 1) qgemm_wgmma_t_kernel(const _
     }
 }
 
-inline bool al(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
-
 }  // namespace
 
 bool gemm_t_tc_supported(const void* g, int64_t ldg, const gptq_qweight& w, const void* out, int64_t ldo, int M) {
     if (w.bits != 4 || M <= 8) return false;
     if (w.groupsize <= 0 || w.groupsize % 32 != 0) return false;  // a thread's 32 consecutive k share one scale and zero
     if (w.K % BF != 0 || w.N % BR != 0) return false;
-    if (!al(g, 16) || ldg % 8 != 0 || !al(out, 16) || ldo % 8 != 0) return false;  // TMA rows of g, paired fp16 stores of out
-    if (ceil_div(M, 128) > 65535) return false;                                       // gridDim.y
+    if (!aligned(g, 16) || ldg % 8 != 0 || !aligned(out, 16) || ldo % 8 != 0) return false;  // TMA rows of g, paired fp16 stores of out
+    if (ceil_div(M, 128) > 65535) return false;                                                 // gridDim.y
     return true;
 }
 
@@ -198,14 +190,8 @@ cudaError_t launch_qlinear_transpose_tc(const void* g, int64_t ldg, const gptq_q
     const int wt = M > 128 ? 2 : 1;
     const int stages = wt == 2 ? 4 : 6;
     const size_t smem = 1024 + (size_t)(wt + 1) * stages * kTileBytes;
-    const dim3 grid(w.K / BF, ceil_div(M, 128 * wt));
-    auto go = [&](auto kernel) -> cudaError_t {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        kernel<<<grid, kGemmTThreads, smem, stream>>>(tmG, p);
-        return cudaGetLastError();
-    };
-    return wt == 2 ? go(qgemm_wgmma_t_kernel<2, 4>) : go(qgemm_wgmma_t_kernel<1, 6>);
+    return launch_kernel(wt == 2 ? qgemm_wgmma_t_kernel<2, 4> : qgemm_wgmma_t_kernel<1, 6>, dim3(w.K / BF, ceil_div(M, 128 * wt)), dim3(kGemmTThreads), smem,
+                         stream, false, tmG, p);
 }
 
 }  // namespace gptq

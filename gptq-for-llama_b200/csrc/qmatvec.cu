@@ -181,7 +181,7 @@ __global__ void __launch_bounds__(kThreads, 2) qmatvec_int4_kernel(const SkinnyP
             float tot = 0.f;
 #pragma unroll
             for (int wv = 0; wv < kWarps; ++wv) tot += red_s[wv];
-            if (tid == 0) rstd_s[m] = 1.0f / sqrtf(tot / (float)p.K + p.eps);
+            if (tid == 0) rstd_s[m] = rms_rstd(tot, p.K, p.eps);
             __syncthreads();
         }
     }
@@ -230,10 +230,7 @@ __global__ void __launch_bounds__(kThreads, 2) qmatvec_int4_kernel(const SkinnyP
                     const uint32_t wv[4] = {nw.x, nw.y, nw.z, nw.w};
                     const float rs = rstd_s[m];
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float2 xf = __half22float2(u32_as_h2(xv[j])), wf = __half22float2(u32_as_h2(wv[j]));
-                        xv[j] = h2_as_u32(__floats2half2_rn(__fmul_rn(__fmul_rn(xf.x, rs), wf.x), __fmul_rn(__fmul_rn(xf.y, rs), wf.y)));
-                    }
+                    for (int j = 0; j < 4; ++j) xv[j] = h2_as_u32(rms_apply2(__half22float2(u32_as_h2(xv[j])), rs, __half22float2(u32_as_h2(wv[j]))));
                     v = make_uint4(xv[0], xv[1], xv[2], xv[3]);
                 }
                 uint4 o;  // (k0,k4) (k1,k5) (k2,k6) (k3,k7): the order dequant8 produces
@@ -422,8 +419,6 @@ __global__ void __launch_bounds__(kThreads, 2) qmatvec_int4_kernel(const SkinnyP
     TRACE(6);
 }
 
-inline bool aligned_to(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
-
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -447,7 +442,7 @@ SkinnyPlan plan_skinny(int M, int K, int N) {
 size_t skinny_workspace_bytes(int M, int K, int N, bool dual) {
     if (M < 1 || M > 8 || K % 32 || N % 32) return 0;
     const SkinnyPlan pl = plan_skinny(M, K, N);
-    const size_t counters = ((size_t)pl.nslabs * sizeof(int) + 255) & ~(size_t)255;
+    const size_t counters = align256((size_t)pl.nslabs * sizeof(int));
     const size_t partial = (size_t)pl.nslabs * pl.max_contrib * (dual ? 2 : 1) * M * kSlabCols * sizeof(float);
     return counters + partial;
 }
@@ -456,11 +451,11 @@ bool skinny_supported(const QLinearArgs& a) {
     const gptq_qweight& w = a.w;
     if (w.bits != 4 || a.M < 1 || a.M > 8) return false;
     if (w.groupsize <= 0 || w.groupsize % 32 != 0) return false;
-    if (!aligned_to(a.x, 16) || a.ldx % 8 != 0) return false;
-    if (!aligned_to(w.qweight, 16) || !aligned_to(w.scales, 8)) return false;
-    if (!aligned_to(a.out, 8) || a.ldo % 4 != 0) return false;
-    if (a.dual && (!aligned_to(a.w2.qweight, 16) || !aligned_to(a.w2.scales, 8))) return false;
-    if (a.norm_w != nullptr && !aligned_to(a.norm_w, 16)) return false;
+    if (!aligned(a.x, 16) || a.ldx % 8 != 0) return false;
+    if (!aligned(w.qweight, 16) || !aligned(w.scales, 8)) return false;
+    if (!aligned(a.out, 8) || a.ldo % 4 != 0) return false;
+    if (a.dual && (!aligned(a.w2.qweight, 16) || !aligned(a.w2.scales, 8))) return false;
+    if (a.norm_w != nullptr && !aligned(a.norm_w, 16)) return false;
     const SkinnyPlan pl = plan_skinny(a.M, w.K, w.N);
     if (pl.total_units * (2LL * kNumSMs + 1) >= (1LL << 31)) return false;  // 32-bit unit arithmetic in the kernel
     const size_t smem = (size_t)kWarps * kRingBytesPerWarp + (size_t)a.M * (pl.seg_steps * 32 + 32) * sizeof(__half);
@@ -492,7 +487,7 @@ cudaError_t launch_qlinear_skinny(const QLinearArgs& a, bool pdl) {
     p.nk = pl.nk;
     p.total_units = (int)pl.total_units;
     p.max_contrib = pl.max_contrib;
-    const size_t counters = ((size_t)pl.nslabs * sizeof(int) + 255) & ~(size_t)255;
+    const size_t counters = align256((size_t)pl.nslabs * sizeof(int));
     p.ws_counter = reinterpret_cast<int*>(a.workspace);
     p.ws_partial = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a.workspace) + counters);
     // pitch: 64 B-odd multiple so that up to 8 x-rows map to distinct bank groups
@@ -501,25 +496,7 @@ cudaError_t launch_qlinear_skinny(const QLinearArgs& a, bool pdl) {
     p.xs_pitch = pitch;
     const size_t smem = (size_t)kWarps * kRingBytesPerWarp + (size_t)a.M * pitch * sizeof(__half);
 
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(pl.grid);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = a.stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl ? 1 : 0;
-    cudaError_t e;
-    if (a.dual) {
-        e = cudaFuncSetAttribute(qmatvec_int4_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-        if (e != cudaSuccess) return e;
-        return cudaLaunchKernelEx(&cfg, qmatvec_int4_kernel<true>, p);
-    }
-    e = cudaFuncSetAttribute(qmatvec_int4_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-    if (e != cudaSuccess) return e;
-    return cudaLaunchKernelEx(&cfg, qmatvec_int4_kernel<false>, p);
+    return launch_kernel(a.dual ? qmatvec_int4_kernel<true> : qmatvec_int4_kernel<false>, dim3(pl.grid), dim3(kThreads), smem, a.stream, pdl, p);
 }
 
 }  // namespace gptq

@@ -1,6 +1,7 @@
 // Hopper tensor-core helpers shared by the wgmma kernels (qgemm_wgmma.cu, qgemm_wgmma_t.cu, lm_head_logprob.cu, cached_attention.cu):
 // shared-memory matrix descriptors, the wgmma fence / commit / wait protocol, the m64n128k16 f16 MMAs (both operands in shared memory, B
-// K-major or transposed; A in registers with a transposed B), and the TMA tensor map of a K-major fp16 matrix with its box load.
+// K-major or transposed; A in registers with a transposed B), and the TMA tensor maps: the encoder (decode_mega.cu's weight maps use it
+// too) and the map of a K-major fp16 matrix with its box load.
 #pragma once
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -106,10 +107,11 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm,
                  : "memory");
 }
 
-// TMA tensor map of an fp16 [rows, K] matrix with `ld` elements between rows (K-major, like the wgmma operands): box 64 (k) x 128 rows,
-// SWIZZLE_128B; rows past `rows` read as zeros.  cuTensorMapEncodeTiled is reached through the runtime's driver entry point (libcuda is
+// A tiled TMA tensor map of `rank` (at most 3) dimensions, innermost first, with unit element strides, SWIZZLE_128B and 256-byte L2
+// promotion; boxes past the end read as zeros.  cuTensorMapEncodeTiled is reached through the runtime's driver entry point (libcuda is
 // not linked: the library must load without a driver).
-inline bool make_kmajor_tensor_map(CUtensorMap* tm, const void* base, int rows, int K, int64_t ld) {
+inline bool encode_tensor_map(CUtensorMap* tm, CUtensorMapDataType type, cuuint32_t rank, const void* base, const cuuint64_t* dims,
+                              const cuuint64_t* strides, const cuuint32_t* box) {
     static PFN_cuTensorMapEncodeTiled encode = []() -> PFN_cuTensorMapEncodeTiled {
         void* fn = nullptr;
         cudaDriverEntryPointQueryResult q;
@@ -117,17 +119,22 @@ inline bool make_kmajor_tensor_map(CUtensorMap* tm, const void* base, int rows, 
         return reinterpret_cast<PFN_cuTensorMapEncodeTiled>(fn);
     }();
     if (encode == nullptr) return false;
-    const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};  // innermost first
-    const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};            // bytes between rows
-    const cuuint32_t box[2] = {(cuuint32_t)kWgmmaBK, 128};         // 64 halves (128 B) x 128 rows
-    const cuuint32_t estr[2] = {1, 1};
+    const cuuint32_t estr[3] = {1, 1, 1};
     auto go = [&] {
-        return encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+        return encode(tm, type, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
     };
     // The encode is a driver call and needs a context current on the calling thread.  A host thread whose first CUDA work is this launch
     // (an autograd worker running a backward) has none until a runtime call binds the primary context: bind it and try once more.
     return go() || (cudaFree(nullptr) == cudaSuccess && go());
+}
+
+// TMA tensor map of an fp16 [rows, K] matrix with `ld` elements between rows (K-major, like the wgmma operands): box 64 (k) x 128 rows
+inline bool make_kmajor_tensor_map(CUtensorMap* tm, const void* base, int rows, int K, int64_t ld) {
+    const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};     // bytes between rows
+    const cuuint32_t box[2] = {(cuuint32_t)kWgmmaBK, 128};  // 64 halves (128 B) x 128 rows
+    return encode_tensor_map(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, dims, strides, box);
 }
 
 }  // namespace gptq
