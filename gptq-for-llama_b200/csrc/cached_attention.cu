@@ -6,8 +6,8 @@
 //
 //   CTA = 2 consumer warpgroups (64 query rows each) on one (span, head, 128-query-row tile); thread 0 issues the TMA loads
 //   Q, K, V          : all K-major for TMA (head_dim contiguous), box 64 (dims) x 128 rows, SWIZZLE_128B: Q through a map over the q columns
-//                      (column h * 128 + {0, 64}), K and V through maps over the layer's cache viewed as [batch * heads * max_seq, 128]
-//                      (row (b * heads + h) * max_seq + key0).  Q is loaded once (32 KB); K | V tiles of 128 keys (64 KB) go through a
+//                      (column h * 128 + {0, 64}), K and V through maps over the layer's cache viewed as [batch * kv_heads * max_seq, 128]
+//                      (row (b * kv_heads + h / g) * max_seq + key0: query head h reads K/V head h / g, g = heads / kv_heads).  Q is loaded once (32 KB); K | V tiles of 128 keys (64 KB) go through a
 //                      2-stage ring behind mbarriers: 1 KB alignment + 32 KB + 2 x 64 KB = 161 KB of shared memory
 //   S = Q K^T        : wgmma m64n128k16, both operands K-major from shared memory (8 k-steps over head_dim)
 //   O += P V         : wgmma m64n128k16 with P from registers (the S accumulator fragment is the A-register layout) and V read MN-major
@@ -51,7 +51,7 @@ struct CachedAttnParams {
     int seq[kCachedAttnMaxSpans], start[kCachedAttnMaxSpans], rows[kCachedAttnMaxSpans];
     int row0[kCachedAttnMaxSpans];       // first q / out row of the span
     int tile0[kCachedAttnMaxSpans + 1];  // first 128-row query tile of the span; [n_spans] = all tiles
-    int n_spans, n_heads, max_seq;
+    int n_spans, n_kv_heads, kv_group, max_seq;  // kv_group: query heads per K/V head
     int64_t ldo;
     __half* out;
 };
@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(kThreads, 1) cached_attention_kernel(const __g
     const int r0 = (t - p.tile0[sp]) * BQ;           // first query row of the tile inside the span
     const int key_end = s0 + n;                      // keys at or past this are never read into the result
     const int nkt = (s0 + min(r0 + BQ, n) - 1) / BKV + 1;  // key tiles up to the last key a row of this tile sees
-    const int kv_row0 = (p.seq[sp] * p.n_heads + h) * p.max_seq;  // < 2^31: checked by the host
+    const int kv_row0 = (p.seq[sp] * p.n_kv_heads + h / p.kv_group) * p.max_seq;  // < 2^31: checked by the host
 
     const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B atoms need 1024 B alignment
     const uint32_t bar0 = smem_u32(&bars[0]);
@@ -205,8 +205,8 @@ __global__ void __launch_bounds__(kThreads, 1) cached_attention_kernel(const __g
 
 }  // namespace
 
-cudaError_t launch_cached_attention(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int max_seq, int n_spans,
-                                    const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
+cudaError_t launch_cached_attention(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int n_kv_heads, int max_seq,
+                                    int n_spans, const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
                                     cudaStream_t stream) {
     CachedAttnParams p{};
     int M = 0, tiles = 0;
@@ -218,10 +218,10 @@ cudaError_t launch_cached_attention(const void* q, int64_t ldq, const void* k_ca
     }
     p.tile0[n_spans] = tiles;
     if (tiles == 0) return cudaSuccess;
-    p.n_spans = n_spans, p.n_heads = n_heads, p.max_seq = max_seq, p.ldo = ldo;
+    p.n_spans = n_spans, p.n_kv_heads = n_kv_heads, p.kv_group = n_heads / n_kv_heads, p.max_seq = max_seq, p.ldo = ldo;
     p.out = static_cast<__half*>(out);
     CUtensorMap tmQ, tmK, tmV;
-    const int kv_rows = batch * n_heads * max_seq;
+    const int kv_rows = batch * n_kv_heads * max_seq;
     if (!make_kmajor_tensor_map(&tmQ, q, M, n_heads * kHeadDim, ldq) || !make_kmajor_tensor_map(&tmK, k_cache, kv_rows, kHeadDim, kHeadDim) ||
         !make_kmajor_tensor_map(&tmV, v_cache, kv_rows, kHeadDim, kHeadDim))
         return cudaErrorNotSupported;

@@ -36,11 +36,26 @@ __global__ void residual_add_kernel(__half* __restrict__ x, const __half* __rest
     if (i < n) x[i] = __hadd(x[i], y[i]);
 }
 
+// dims [16 j, 16 j + 16) of row t of a head's K or V: row pos from this CTA's own copy in shared memory, the others from the cache
+__device__ __forceinline__ void load_key_dims(const __half* cache, const __half* fresh, int t, int pos, int j, uint4& a, uint4& b) {
+    if (t == pos) {
+        a = reinterpret_cast<const uint4*>(fresh)[2 * j];
+        b = reinterpret_cast<const uint4*>(fresh)[2 * j + 1];
+    } else {
+        const uint4* src = reinterpret_cast<const uint4*>(cache + (size_t)t * kHeadDim) + 2 * j;
+        a = src[0];
+        b = src[1];
+    }
+}
+
 // RoPE(q, k) + KV append + attention over keys [split*256, min(split*256+256, pos+1)).
 //   rotation: rotate_half_kernel (quant/fused_attn.py:23-58): freq_i = exp(i * inv_base) * pos, fp32, results rounded to fp16
 //   scores:   fp16 q.k with fp32 accumulation, * head_dim^-0.5, softmax in fp32, fp32 P.V  (SDPA, fused_attn.py:154-155)
 // grid (heads, nsplit, batch).  Partial (m, l, o[128]) per (batch, head, split) goes to `part`.
-__global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half* __restrict__ qkv, int hidden, __half* __restrict__ k_cache,
+// Grouped-query attention: qkv rows are [hidden q | n_kv_heads * 128 k | n_kv_heads * 128 v] and query head h reads K/V head h / g
+// (g = n_heads / n_kv_heads).  The g CTAs of a group that own the new key all rotate it, and each reads its own copy of the new row from shared
+// memory, never from the cache (a sibling's store may not have landed); only the group's first head stores it.
+__global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half* __restrict__ qkv, int hidden, int n_kv_heads, __half* __restrict__ k_cache,
                                                                    __half* __restrict__ v_cache, const int32_t* __restrict__ positions, int n_heads, int max_seq,
                                                                    int batch, float inv_base, float scale, float* __restrict__ part, int nsplit) {
     const int head = blockIdx.x, split = blockIdx.y, b = blockIdx.z;
@@ -55,14 +70,18 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half*
 
     __shared__ float q_s[kHeadDim];
     __shared__ float cs_s[kHeadDim];  // cos[0..63], sin[0..63]
+    __shared__ __align__(16) __half knew_s[kHeadDim], vnew_s[kHeadDim];  // row pos of K and V (if this CTA owns it)
     __shared__ float red_m[16], red_l[16];
     __shared__ float red_o[16][kHeadDim + 4];
 
-    const __half* q = qkv + (size_t)b * 3 * hidden + head * kHeadDim;
-    const __half* k = q + hidden;
-    const __half* v = q + 2 * hidden;
-    __half* kc = k_cache + ((size_t)(b * n_heads + head) * max_seq) * kHeadDim;
-    __half* vc = v_cache + ((size_t)(b * n_heads + head) * max_seq) * kHeadDim;
+    const int group = n_heads / n_kv_heads, kv_head = head / group;
+    const int Hkv = n_kv_heads * kHeadDim;
+    const __half* row = qkv + (size_t)b * (hidden + 2 * Hkv);
+    const __half* q = row + head * kHeadDim;
+    const __half* k = row + hidden + kv_head * kHeadDim;
+    const __half* v = k + Hkv;
+    __half* kc = k_cache + ((size_t)(b * n_kv_heads + kv_head) * max_seq) * kHeadDim;
+    __half* vc = v_cache + ((size_t)(b * n_kv_heads + kv_head) * max_seq) * kHeadDim;
 
     if (tid < 64) {
         const float f = rope_inv_freq(tid, inv_base) * (float)pos;
@@ -80,8 +99,12 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half*
         if (pos >= c0 && pos < c1) {                   // this CTA owns the new key/value: append them
             const float kx = __half2float(k[i]), ky = __half2float(k[i + 64]);
             const float kr = hi ? rope_y(kx, ky, c, s) : rope_x(kx, ky, c, s);
-            kc[(size_t)pos * kHeadDim + tid] = __float2half_rn(kr);
-            vc[(size_t)pos * kHeadDim + tid] = v[tid];
+            knew_s[tid] = __float2half_rn(kr);
+            vnew_s[tid] = v[tid];
+            if (head == kv_head * group) {
+                kc[(size_t)pos * kHeadDim + tid] = knew_s[tid];
+                vc[(size_t)pos * kHeadDim + tid] = vnew_s[tid];
+            }
         }
     }
     __syncthreads();
@@ -99,8 +122,8 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half*
         const int t = c0 + grp + it * 16;
         float s = 0.f;
         if (t < c1) {
-            const uint4* kp = reinterpret_cast<const uint4*>(kc + (size_t)t * kHeadDim + 16 * j);
-            const uint4 a = kp[0], bq = kp[1];
+            uint4 a, bq;
+            load_key_dims(kc, knew_s, t, pos, j, a, bq);
             const uint32_t w[8] = {a.x, a.y, a.z, a.w, bq.x, bq.y, bq.z, bq.w};
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
@@ -126,8 +149,8 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half*
         if (t < c1) {
             const float p = expf(sc[it] - mloc);
             lloc += p;
-            const uint4* vp = reinterpret_cast<const uint4*>(vc + (size_t)t * kHeadDim + 16 * j);
-            const uint4 a = vp[0], bq = vp[1];
+            uint4 a, bq;
+            load_key_dims(vc, vnew_s, t, pos, j, a, bq);
             const uint32_t w[8] = {a.x, a.y, a.z, a.w, bq.x, bq.y, bq.z, bq.w};
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
@@ -332,7 +355,7 @@ void chain_linears(const gptq_llama_model& m, const gptq_llama_layer& ly, const 
         c.skinny = skinny_supported(a);
         return c;
     };
-    out[0] = make(ly.qkv, nullptr, x, H, ly.input_norm, nullptr, sc + L.qkv, 3 * H);
+    out[0] = make(ly.qkv, nullptr, x, H, ly.input_norm, nullptr, sc + L.qkv, ly.qkv.N);  // q | k | v rows of (n_heads + 2 n_kv_heads) heads
     out[1] = make(ly.o, nullptr, sc + L.attn, H, nullptr, x, x, H);
     out[2] = make(ly.gate, &ly.up, x, H, ly.post_norm, nullptr, sc + L.h, I);
     out[3] = make(ly.down, nullptr, sc + L.h, I, nullptr, x, x, H);
@@ -405,12 +428,15 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
     const int Hq = m.n_heads * m.head_dim;  // = hidden, or this rank's share of it under tensor parallelism
     if ((st->tp == nullptr && Hq != m.hidden) || Hq < 1 || Hq > m.hidden || m.hidden % 32 != 0 || m.intermediate % 32 != 0 || m.n_layers < 1 || m.vocab < 1) return GPTQ_ERR_SHAPE;
     if (st->batch < 1 || st->batch > 8 || st->max_seq < 1) return GPTQ_ERR_SHAPE;
+    const int n_kv = llama_kv_heads(m);
+    if (n_kv < 1) return GPTQ_ERR_SHAPE;
+    if (st->tp != nullptr && n_kv != m.n_heads) return GPTQ_ERR_UNSUPPORTED;  // tensor-parallel shards are dealt by whole query heads
     const ScratchLayout L = scratch_layout(m, st->batch, st->max_seq);
     if (st->scratch_bytes < L.total) return GPTQ_ERR_WORKSPACE;
     if (!aligned(st->scratch, 256)) return GPTQ_ERR_ALIGN;
     for (int l = 0; l < m.n_layers; ++l) {
         const gptq_llama_layer& ly = m.layers[l];
-        if (ly.qkv.K != m.hidden || ly.qkv.N != 3 * Hq || ly.o.K != Hq || ly.o.N != m.hidden || ly.gate.K != m.hidden ||
+        if (ly.qkv.K != m.hidden || ly.qkv.N != Hq + 2 * n_kv * m.head_dim || ly.o.K != Hq || ly.o.N != m.hidden || ly.gate.K != m.hidden ||
             ly.gate.N != m.intermediate || ly.up.K != m.hidden || ly.up.N != m.intermediate || ly.down.K != m.intermediate || ly.down.N != m.hidden)
             return GPTQ_ERR_SHAPE;
         if (ly.input_norm == nullptr || ly.post_norm == nullptr) return GPTQ_ERR_NULL;
@@ -431,7 +457,7 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
     const int B = st->batch, H = m.hidden;
     const float inv_base = rope_inv_base(m.rope_base, m.head_dim);
     const float scale = attn_scale(m.head_dim);
-    const size_t layer_stride = (size_t)B * m.n_heads * st->max_seq * m.head_dim;
+    const size_t layer_stride = (size_t)B * n_kv * st->max_seq * m.head_dim;
 
 #define GPTQ_TRY(expr)                                   \
     do {                                                 \
@@ -443,7 +469,7 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
         ChainLinear c[4];
         chain_linears(m, m.layers[l], *st, L, stream, c);
         GPTQ_TRY(engine_linear(c[0], sc, L));
-        GPTQ_TRY(launch_kernel(attn_decode_kernel, dim3(m.n_heads, L.nsplit, B), dim3(kAttnThreads), 0, stream, true, qkv, H,
+        GPTQ_TRY(launch_kernel(attn_decode_kernel, dim3(m.n_heads, L.nsplit, B), dim3(kAttnThreads), 0, stream, true, qkv, H, n_kv,
                                reinterpret_cast<__half*>(st->k_cache) + l * layer_stride, reinterpret_cast<__half*>(st->v_cache) + l * layer_stride,
                                st->positions, m.n_heads, st->max_seq, B, inv_base, scale, part, L.nsplit));
         GPTQ_TRY(launch_kernel(attn_combine_kernel, dim3(m.n_heads, B), dim3(kHeadDim), 0, stream, true, part, st->positions, attn, H, m.n_heads, L.nsplit));

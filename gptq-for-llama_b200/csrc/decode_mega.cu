@@ -117,7 +117,7 @@ struct MatDesc {
     const __half* sc;
     const uint32_t* qz;
     int gs_steps;  // k-steps per quantisation group (groupsize / 32)
-    int tmap;      // tensor-map class of qweight (0: N = 3H, 1: N = H, 2: N = I)
+    int tmap;      // tensor-map class of qweight (0: N = Nqkv, 1: N = H, 2: N = I)
     int chunk0;    // chunk coordinate of the matrix: (qweight - class base) / 128 bytes
 };
 struct LayerDesc {
@@ -133,6 +133,9 @@ struct MegaParams {
     // H: hidden size (the residual stream, replicated under tensor parallelism); n_heads, Hq = 128 * n_heads, I: this rank's attention heads
     // / attention width / MLP width (the full ones on a single GPU); V: vocabulary, [v0, v1): the lm_head rows of this rank
     int n_layers, H, Hq, I, V, v0, v1, n_heads, max_seq, n_stages, lm_rows;
+    // grouped-query attention: n_kv_heads K/V heads, kv_group = n_heads / n_kv_heads query heads per K/V head; Nqkv = Hq + 2 * 128 * n_kv_heads is
+    // the width of the fused q | k | v output (3 Hq for multi-head attention)
+    int n_kv_heads, kv_group, Nqkv;
     int tp_size, tp_rank, tp_exchange;  // tp_exchange: reduce locally first, then hand slices to the ranks (else: every team REDs into every rank)
     float eps, inv_base, scale;
     const __half* embed;
@@ -147,7 +150,7 @@ struct MegaParams {
     int32_t* next_token;
     // scratch (device)
     __half* resid[2];  // residual stream ping-pong, fp16 [H]
-    float* acc_qkv;    // [3H]
+    float* acc_qkv;    // [Nqkv]
     float* acc_o;      // [H]
     float* acc_g;      // [I]
     float* acc_u;      // [I]
@@ -169,7 +172,7 @@ struct MegaParams {
     CUtensorMap tmaps[6];  // [class]: 16-row boxes (a full stage), [3 + class]: 4-row boxes (one k-step)
     // BATCH instantiation only: sequences of the step, and halves between the sequences' rows of the staged x (H + 32: a stride of
     // 64 mod 128 bytes puts the two lane groups of a quarter-warp on different banks).  Per-sequence vectors are [batch][n] with
-    // n = H, 3 Hq, I, V or 128 (rope_cs); resid, acc_* and rope_cs are sized for the batch.
+    // n = H, Nqkv, I, V or 128 (rope_cs); resid, acc_* and rope_cs are sized for the batch.
     int batch, xs_stride;
 };
 
@@ -310,7 +313,7 @@ struct StageWalk {
     enum { kQ, kA, kO, kG, kD, kL, kEnd };
     int l = 0, op = -1, u = 0, u1 = 0;  // layer, operation, next unit of the team's range [u, u1) of that operation
     int Tlen = 0;                       // A: the sequence's key count
-    size_t kv = 0;                      // A: offset of the team's head (row 0) in the layer's K / V cache, in halves
+    size_t kv = 0;                      // A: offset of the team's K/V head (row 0) in the layer's K / V cache, in halves
 
     // the descriptor of the next stage; false once the token's last stage has been taken
     __device__ __forceinline__ bool next(const MegaParams& p, unsigned T, unsigned nb, StageLoad& s) {
@@ -323,7 +326,7 @@ struct StageWalk {
             if (op == kA) {
                 int pos, head;
                 const int seq = attn_work<BATCH>(p, T, nb, pos, Tlen, head, u, u1);
-                kv = (size_t)l * p.layer_stride + (size_t)(seq * p.n_heads + head) * p.max_seq * kHD;
+                kv = (size_t)l * p.layer_stride + (size_t)(seq * p.n_kv_heads + head / p.kv_group) * p.max_seq * kHD;
             } else if (op == kL) {
                 team_range(T, (unsigned)((p.v1 - p.v0 + p.lm_rows - 1) / p.lm_rows), nb, u, u1);
             } else if (op != kEnd) {
@@ -379,7 +382,7 @@ struct StageWalk {
     // K x N of the current matvec; nm = 2: gate|up side by side
     __device__ __forceinline__ void matvec_shape(const MegaParams& p, int& K, int& N, int& nm) const {
         K = op == kO ? p.Hq : op == kD ? p.I : p.H;
-        N = op == kQ ? 3 * p.Hq : op == kG ? p.I : p.H;
+        N = op == kQ ? p.Nqkv : op == kG ? p.I : p.H;
         nm = op == kG ? 2 : 1;
     }
 };
@@ -1066,6 +1069,9 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
 // Work units (head, 32 keys); a team serves one head (attn_range); one unit = one ring stage (K rows, V rows).  The team writes
 // one partial record (m, l, o[128]) to p.part[T].
 // BATCH: the team serves one (sequence, head) pair (attn_work), at that sequence's position, in that sequence's cache slot.
+// Grouped-query attention: query head h reads K/V head h / kv_group.  Every team owning the unit that holds pos rotates the new key itself
+// and patches its own staged copy with it; only the group's first query head stores the row to the cache, and no team reads another
+// team's store within the step.
 template <bool BATCH>
 __device__ void run_attention(const MegaParams& p, ConsRing& ring, const TeamCtx& tc, int layer) {
     int pos, Tlen, head, b0, b_end;
@@ -1096,21 +1102,25 @@ __device__ void run_attention(const MegaParams& p, ConsRing& ring, const TeamCtx
             const int i = ttid & 63;
             const bool hi = ttid >= 64;
             const float c = ld_cg(p.rope_cs + seq * kHD + i), s = ld_cg(p.rope_cs + seq * kHD + 64 + i);
-            const float* aq = p.acc_qkv + (size_t)seq * 3 * p.Hq + head * kHD;
+            const float* arow = p.acc_qkv + (size_t)seq * p.Nqkv;
+            const float* aq = arow + head * kHD;
             const float qx = __half2float(__float2half_rn(ld_cg(aq + i))), qy = __half2float(__float2half_rn(ld_cg(aq + i + 64)));  // the qkv projection output is fp16
             const float qr = hi ? rope_y(qx, qy, c, s) : rope_x(qx, qy, c, s);
             q_s[ttid] = __half2float(__float2half_rn(qr));
             if (owns_new) {  // this segment owns the new key/value: RoPE(k), append both to the cache
-                const float* ak = aq + p.Hq;
-                const float* av = aq + 2 * p.Hq;
+                const int kvh = head / p.kv_group;
+                const float* ak = arow + p.Hq + kvh * kHD;
+                const float* av = ak + p.n_kv_heads * kHD;
                 const float kx = __half2float(__float2half_rn(ld_cg(ak + i))), ky = __half2float(__float2half_rn(ld_cg(ak + i + 64)));
                 const float kr = hi ? rope_y(kx, ky, c, s) : rope_x(kx, ky, c, s);
                 const __half kh = __float2half_rn(kr), vh = __float2half_rn(ld_cg(av + ttid));
                 knew[ttid] = kh;
                 vnew[ttid] = vh;
-                const size_t off = ((size_t)(seq * p.n_heads + head) * p.max_seq + pos) * kHD + ttid;
-                kc_l[off] = kh;
-                vc_l[off] = vh;
+                if (head == kvh * p.kv_group) {
+                    const size_t off = ((size_t)(seq * p.n_kv_heads + kvh) * p.max_seq + pos) * kHD + ttid;
+                    kc_l[off] = kh;
+                    vc_l[off] = vh;
+                }
             }
         }
         team_sync(tc.team);
@@ -1508,7 +1518,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         zero_slice(p.acc_u, nbat * p.I);
         {
             OPTRACE_BEGIN(ring);
-            run_matvec<1, X_FULL, false, BATCH>(p, ring, tc, L.qkv.gs_steps, p.H, 3 * p.Hq, p.acc_qkv, nullptr, xs, xsum, xinv_s[0]);
+            run_matvec<1, X_FULL, false, BATCH>(p, ring, tc, L.qkv.gs_steps, p.H, p.Nqkv, p.acc_qkv, nullptr, xs, xsum, xinv_s[0]);
             OPTRACE_END(ring, l, 0);
         }
         MTRACE(l * 12 + 2);
@@ -1525,7 +1535,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         grid_barrier(p.bar, gen);
         MTRACE(l * 12 + 5);
         // ---- O ----
-        zero_slice(p.acc_qkv, nbat * 3 * p.Hq);
+        zero_slice(p.acc_qkv, nbat * p.Nqkv);
         {
             OPTRACE_BEGIN(ring);
             if constexpr (BATCH)
@@ -1637,7 +1647,8 @@ bool mega_plan(const gptq_llama_model& m, int batch, int sms, size_t smem_max, s
 
 // Byte offsets of the persistent kernel's buffers in its scratch region.  The head (resid, acc_o, acc_d, xbar) depends on the hidden size
 // and the batch only, so it has the same layout on every tensor-parallel rank: peers address acc_o / acc_d / xbar of this rank through its
-// scratch base.  Every per-sequence buffer is [B][n] (gptq_b200.h); acc_qkv has room for 3 H (a tensor-parallel rank uses 3 Hq of it).
+// scratch base.  Every per-sequence buffer is [B][n] (gptq_b200.h); acc_qkv has room for 3 H, which bounds Nqkv (a tensor-parallel rank uses
+// 3 Hq of it, a grouped-query model Hq + 2 * 128 n_kv_heads <= 3 H).
 struct MegaScratch {
     size_t resid[2], acc_o, acc_d, xbar, acc_o_loc, acc_d_loc, acc_qkv, acc_g, acc_u, part, rope_cs, bar, total;
 };
@@ -1675,7 +1686,8 @@ cudaError_t mega_step_plan(const gptq_llama_model& m, const gptq_llama_state& st
     if (st.batch < 1 || st.batch > kMaxBatch || m.n_layers > kMaxLayers || m.head_dim != kHD) return kNo;
     if (st.batch > 1 && st.tp != nullptr) return kNo;  // tensor parallelism: batch 1 only
     if (m.hidden % kSlabCols || m.intermediate % kSlabCols || m.hidden > 8192 || m.intermediate > 32768 || m.hidden % 64) return kNo;
-    if ((3 * m.n_heads * m.head_dim) % kSlabCols) return kNo;  // the (local) fused qkv width is dealt in 256-column slabs
+    const int n_kv = llama_kv_heads(m);
+    if (n_kv < 1 || (m.n_heads + 2 * n_kv) * m.head_dim % kSlabCols) return kNo;  // the (local) fused qkv width is dealt in 256-column slabs
     if (st.tp != nullptr) {
         const gptq_llama_tp& tp = *st.tp;
         if (tp.size < 1 || tp.size > kMaxTP || tp.rank < 0 || tp.rank >= tp.size) return kNo;
@@ -1726,6 +1738,9 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
 
     MegaParams p{};
     p.n_layers = m.n_layers; p.H = m.hidden; p.Hq = m.n_heads * m.head_dim; p.I = m.intermediate; p.V = m.vocab; p.n_heads = m.n_heads;
+    p.n_kv_heads = llama_kv_heads(m);  // >= 1: checked by mega_step_plan
+    p.kv_group = m.n_heads / p.n_kv_heads;
+    p.Nqkv = p.Hq + 2 * p.n_kv_heads * m.head_dim;
     p.v0 = st.tp != nullptr ? st.tp->vocab_begin : 0;
     p.v1 = st.tp != nullptr ? st.tp->vocab_end : m.vocab;
     p.max_seq = st.max_seq;
@@ -1741,7 +1756,7 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     p.positions = st.positions;
     p.k_cache = reinterpret_cast<__half*>(st.k_cache);
     p.v_cache = reinterpret_cast<__half*>(st.v_cache);
-    p.layer_stride = (size_t)B * m.n_heads * st.max_seq * m.head_dim;
+    p.layer_stride = (size_t)B * p.n_kv_heads * st.max_seq * m.head_dim;
     p.logits = reinterpret_cast<__half*>(st.logits);
     p.next_token = st.next_tokens;
     p.batch = B;
@@ -1771,9 +1786,9 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     p.part = reinterpret_cast<float*>(scratch + ms.part);
     p.rope_cs = reinterpret_cast<float*>(scratch + ms.rope_cs);
     p.bar = reinterpret_cast<unsigned long long*>(scratch + ms.bar);
-    // One tensor map per row stride serves every layer: class 0 = qkv (N = 3H), 1 = o and down (N = H), 2 = gate and up (N = I).
+    // One tensor map per row stride serves every layer: class 0 = qkv (N = Nqkv), 1 = o and down (N = H), 2 = gate and up (N = I).
     // Its base is the lowest qweight address of the class; a matrix is addressed through the chunk coordinate (128-byte units).
-    const int classN[3] = {3 * m.n_heads * m.head_dim, m.hidden, m.intermediate};
+    const int classN[3] = {p.Nqkv, m.hidden, m.intermediate};
     uintptr_t base[3] = {UINTPTR_MAX, UINTPTR_MAX, UINTPTR_MAX}, top[3] = {0, 0, 0};
     int rows_max[3] = {0, 0, 0};
     auto visit = [&](const gptq_qweight& w, int c) {

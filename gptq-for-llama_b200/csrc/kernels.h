@@ -13,6 +13,19 @@ inline bool has_input_perm(const gptq_llama_model& m) {
     return false;
 }
 
+// K/V heads of a decode model, carried by the width of its fused q|k|v weight (gptq_llama_layer.qkv):
+// n_kv_heads = (qkv.N / head_dim - n_heads) / 2.  -1 unless it is a positive divisor of n_heads and every layer has the same width.
+inline int llama_kv_heads(const gptq_llama_model& m) {
+    if (m.layers == nullptr || m.n_layers < 1 || m.n_heads < 1 || m.head_dim < 1) return -1;
+    const int N = m.layers[0].qkv.N;
+    for (int l = 1; l < m.n_layers; ++l)
+        if (m.layers[l].qkv.N != N) return -1;
+    if (N % m.head_dim != 0) return -1;
+    const int rest = N / m.head_dim - m.n_heads;  // 2 * n_kv_heads
+    if (rest <= 0 || rest % 2 != 0 || m.n_heads % (rest / 2) != 0) return -1;
+    return rest / 2;
+}
+
 struct QLinearArgs {
     const void* x;
     int64_t ldx;
@@ -62,8 +75,8 @@ cudaError_t launch_lm_head_logprob(const void* x, int64_t ldx, const void* w, in
 
 // cached_attention.cu -- causal attention of new rows over a sequence's cached prefix (wgmma, read in place from the KV cache), head_dim 128
 constexpr int kCachedAttnMaxSpans = 64;
-cudaError_t launch_cached_attention(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int max_seq, int n_spans,
-                                    const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
+cudaError_t launch_cached_attention(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int n_kv_heads, int max_seq,
+                                    int n_spans, const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
                                     cudaStream_t stream);
 
 // sample.cu -- one token per row of decode-step logits: temperature / top-k / top-p / Philox draw, or the argmax (gptq_sample_tokens)

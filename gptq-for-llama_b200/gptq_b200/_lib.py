@@ -89,6 +89,8 @@ SIGNATURES = {
     'gptq_lm_head_logprob': (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'gptq_cached_attention': (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                                       c_void_p]),
+    'gptq_cached_attention_gqa': (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_int64, c_void_p]),
     'gptq_sample_tokens': (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, ctypes.POINTER(Sampling), c_void_p, c_void_p]),
     'gptq_ipc_alloc':(c_int, [c_size_t, ctypes.POINTER(c_void_p), ctypes.c_char_p]),
     'gptq_ipc_open': (c_int, [ctypes.c_char_p, ctypes.POINTER(c_void_p)]),

@@ -26,7 +26,21 @@ LLAMA_SHAPES = {  # hidden, intermediate, layers, heads (SURVEY.md section 8)
     'tiny': (256, 704, 2, 2),    # intermediate not a multiple of 256: exercises the kernel-chain engine
     'tiny256': (256, 768, 2, 2),  # eligible for the persistent single-kernel path
     'tiny512': (512, 1024, 2, 4),  # shardable over 2 tensor-parallel ranks (2 heads and 2 slabs of 256 MLP columns each)
+    # grouped-query attention: their K/V head counts are in KV_HEADS
+    '70b': (8192, 28672, 80, 64),        # LLaMA-2-70B
+    '34b': (8192, 22016, 48, 64),        # CodeLlama-34B (RoPE base 1e6)
+    'llama3-8b': (4096, 14336, 32, 32),  # LLaMA-3-8B (RoPE base 5e5, vocabulary 128256)
+    'tiny-gqa2': (512, 1024, 2, 4),      # persistent single-kernel path, 2 query heads per K/V head
+    'tiny-gqa1': (512, 1024, 2, 4),      # persistent, one K/V head for all 4 query heads
+    'tiny-gqa2-chain': (512, 704, 2, 4),  # intermediate not a multiple of 256: the kernel-chain engine
+    'tiny-gqa1-chain': (512, 704, 2, 4),
 }
+KV_HEADS = {'70b': 8, '34b': 8, 'llama3-8b': 8, 'tiny-gqa2': 2, 'tiny-gqa1': 1, 'tiny-gqa2-chain': 2, 'tiny-gqa1-chain': 1}  # other shapes: one per head
+
+
+def kv_heads(size):
+    """K/V heads of a named shape (LLAMA_SHAPES): KV_HEADS, else one per query head (multi-head attention)."""
+    return KV_HEADS.get(size, LLAMA_SHAPES[size][3])
 
 
 def random_qlayer(K, N, bits, groupsize, device, gen, act_order=False):
@@ -80,14 +94,27 @@ class LlamaDecoder:
     """Owns the weights, the KV cache and the captured graph; `step()` decodes one token per sequence."""
 
     def __init__(self, layers, embed, final_norm, lm_head, n_heads, rms_eps=1e-6, rope_base=10000.0, batch=1, max_seq=2048, use_graph=True, head_dim=None,
-                 tp=None):
+                 tp=None, n_kv_heads=None):
         """tp = (rank, size, vocab_begin, vocab_end[, reduce_mode]): this process holds one tensor-parallel shard (see shard_for_rank / gptq_llama_tp): `layers`,
         `lm_head` and `n_heads` are the LOCAL ones, head_dim must be given, and torch.distributed must be initialised (the scratch and logits
-        buffers of the ranks are exchanged as CUDA IPC handles)."""
+        buffers of the ranks are exchanged as CUDA IPC handles).
+        n_kv_heads: K/V heads of grouped-query attention (None: n_heads, multi-head attention).  It must divide n_heads, and every layer's fused
+        qkv must be (n_heads + 2 n_kv_heads) * head_dim wide (q, then k, then v heads; the width is how the kernels learn the count).
+        The KV cache holds n_kv_heads heads.  Tensor parallelism needs n_kv_heads == n_heads."""
         self.dev = embed.device
         self.tp = tp
         self.head_dim = head_dim or embed.shape[1] // n_heads
         self.layers = layers  # list of dicts: qkv, o, gate, up, down (QLayerWeights), input_norm, post_norm (fp16 tensors)
+        self.n_kv_heads = n_heads if n_kv_heads is None else int(n_kv_heads)
+        if self.n_kv_heads < 1 or n_heads % self.n_kv_heads != 0:
+            raise ValueError(f'n_kv_heads ({n_kv_heads}) must be a positive divisor of n_heads ({n_heads})')
+        if tp is not None:
+            _refuse_gqa_tp(n_heads, self.n_kv_heads)
+        qkv_width = (n_heads + 2 * self.n_kv_heads) * self.head_dim
+        for i, ly in enumerate(layers):
+            if ly['qkv'].qweight.shape[1] != qkv_width:
+                raise ValueError(f'layer {i}: fused qkv has {ly["qkv"].qweight.shape[1]} columns, {n_heads} query and {self.n_kv_heads} K/V heads of '
+                                 f'{self.head_dim} need {qkv_width}')
         self.embed, self.final_norm, self.lm_head = embed.contiguous(), final_norm.contiguous(), lm_head.contiguous()
         self.hidden = embed.shape[1]
         self.vocab = embed.shape[0]
@@ -102,7 +129,7 @@ class LlamaDecoder:
             m.layers = ctypes.cast(self._layer_arr, ctypes.POINTER(LlamaLayer))
             m.embed, m.final_norm, m.lm_head = self.embed.data_ptr(), self.final_norm.data_ptr(), self.lm_head.data_ptr()
             self.model = m
-            cache_shape = (len(layers), batch, n_heads, max_seq, self.head_dim)
+            cache_shape = (len(layers), batch, self.n_kv_heads, max_seq, self.head_dim)
             self.k_cache = torch.zeros(cache_shape, dtype=torch.float16, device=self.dev)
             self.v_cache = torch.zeros(cache_shape, dtype=torch.float16, device=self.dev)
             self.tokens = torch.zeros(batch, dtype=torch.int32, device=self.dev)
@@ -334,7 +361,7 @@ class LlamaDecoder:
         Returns the residual stream after the last layer, fp16 [M, hidden] (final norm not applied)."""
         ns = [len(s) for s in seqs]
         total = sum(ns)
-        H, nh, hd = self.hidden, self.n_heads, self.head_dim
+        H, nh, nkv, hd = self.hidden, self.n_heads, self.n_kv_heads, self.head_dim
         ids = [int(t) for s in seqs for t in s]
         x = self.embed[torch.tensor(ids, device=self.dev)]  # [total, H]
         if starts is None:
@@ -343,24 +370,28 @@ class LlamaDecoder:
             assert cache
             pos = torch.cat([torch.arange(p, p + n, dtype=torch.int64) for p, n in zip(starts, ns)]).to(self.dev)[None, :]
         spans = [(b, sum(ns[:b]), n) for b, n in enumerate(ns) if n > 0]  # (list, first row, rows)
+        sdpa = dict(enable_gqa=True) if nkv != nh else {}
         for li, ly in enumerate(self.layers):
-            qkv = ops.matmul248(ops.rmsnorm(x, ly['input_norm'], self.model.rms_eps), *ly['qkv'].parts(), ly['qkv'].bits, groupsize=ly['qkv'].hint).view(1, total, 3, nh, hd)
-            ops.rotate_half_(qkv[:, :, :2], pos, base=self.model.rope_base)
+            qkv = ops.matmul248(ops.rmsnorm(x, ly['input_norm'], self.model.rms_eps), *ly['qkv'].parts(), ly['qkv'].bits,
+                                groupsize=ly['qkv'].hint).view(1, total, nh + 2 * nkv, hd)  # q | k | v heads
+            # q and k are the first nh + nkv rows of head_dim of every token: one RoPE call rotates both
+            ops.rotate_half_(qkv[:, :, :nh + nkv].unsqueeze(2), pos, base=self.model.rope_base)
+            q_rows, k_rows, v_rows = qkv[0].split([nh, nkv, nkv], dim=1)  # [total, heads, hd]
             if starts is None:
                 atts = []
                 for b, r0, n in spans:
-                    q, k, v = (qkv[0, r0:r0 + n, i].transpose(0, 1) for i in range(3))  # [nh, n, hd]
+                    q, k, v = (t[r0:r0 + n].transpose(0, 1) for t in (q_rows, k_rows, v_rows))  # [heads, n, hd]
                     if cache:
                         self.k_cache[li, b, :, :n] = k
                         self.v_cache[li, b, :, :n] = v
-                    atts.append(torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None], is_causal=True)[0].transpose(0, 1).reshape(n, H))
+                    atts.append(torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None], is_causal=True, **sdpa)[0].transpose(0, 1).reshape(n, H))
                 att = atts[0] if len(atts) == 1 else torch.cat(atts)
             else:
                 for b, r0, n in spans:
                     p = starts[b]
-                    self.k_cache[li, b, :, p:p + n] = qkv[0, r0:r0 + n, 1].transpose(0, 1)
-                    self.v_cache[li, b, :, p:p + n] = qkv[0, r0:r0 + n, 2].transpose(0, 1)
-                att = ops.cached_attention(qkv.view(total, 3 * H)[:, :H], self.k_cache[li], self.v_cache[li], [(b, starts[b], n) for b, _, n in spans])
+                    self.k_cache[li, b, :, p:p + n] = k_rows[r0:r0 + n].transpose(0, 1)
+                    self.v_cache[li, b, :, p:p + n] = v_rows[r0:r0 + n].transpose(0, 1)
+                att = ops.cached_attention(qkv.view(total, -1)[:, :H], self.k_cache[li], self.v_cache[li], [(b, starts[b], n) for b, _, n in spans])
             x = x + ops.matmul248(att, *ly['o'].parts(), ly['o'].bits, groupsize=ly['o'].hint)
             h = ops.fused_mlp(ops.rmsnorm(x, ly['post_norm'], self.model.rms_eps), ly['gate'].parts(), ly['up'].parts(), ly['gate'].bits, ly['gate'].hint)
             x = x + ops.matmul248(h, *ly['down'].parts(), ly['down'].bits, groupsize=ly['down'].hint)
@@ -591,7 +622,8 @@ def _synthetic_draws(size, bits, groupsize, act_order, vocab, device, seed, n_la
     embedding, the lm_head and the final norm.  synthetic_llama and synthetic_llama_tp both build their model from these draws, so a
     tensor-parallel rank holds a shard of the very model synthetic_llama builds from the same seed.  groupsize -1: one group per linear (the
     reference's --groupsize -1, where QuantLinear takes groupsize = infeatures): hidden for qkv / o / gate / up, intermediate for down."""
-    hidden, inter, layers, _ = LLAMA_SHAPES[size]
+    hidden, inter, layers, heads = LLAMA_SHAPES[size]
+    qkv_cols = hidden + 2 * kv_heads(size) * (hidden // heads)  # q | k | v
     gs_h, gs_i = (hidden, inter) if groupsize == -1 else (groupsize, groupsize)
     dev = torch.device(device)
     gen = torch.Generator(device=dev).manual_seed(seed)
@@ -602,7 +634,7 @@ def _synthetic_draws(size, bits, groupsize, act_order, vocab, device, seed, n_la
         if act_order:  # gate and up see the same input, hence the same Hessian diagonal and the same act-order map (gptq.py:210-216)
             up = QLayerWeights(up.qweight, up.scales, up.qzeros, gate.g_idx.clone(), bits, gs_h)
         # q/k/v share their input, hence their act-order map (quant/fused_attn.py:180): nothing to do, qkv is one layer here
-        yield dict(qkv=qlayer(hidden, 3 * hidden, gs_h), o=qlayer(hidden, hidden, gs_h), gate=gate, up=up, down=qlayer(inter, hidden, gs_i),
+        yield dict(qkv=qlayer(hidden, qkv_cols, gs_h), o=qlayer(hidden, hidden, gs_h), gate=gate, up=up, down=qlayer(inter, hidden, gs_i),
                    input_norm=norm(), post_norm=norm())
     yield (torch.randn(vocab, hidden, device=dev, generator=gen) * 0.5).half()
     yield (torch.randn(vocab, hidden, device=dev, generator=gen) * 0.02).half()
@@ -613,16 +645,24 @@ def synthetic_llama(size='7b', bits=4, groupsize=128, act_order=False, vocab=320
     """Random-init GPTQ LLaMA of the named size (no checkpoints are reachable offline): every layer has its
     own distinct packed tensors so that a decode step streams the full model from HBM.  groupsize -1 as in _synthetic_draws."""
     *L, embed, lm_head, final_norm = _synthetic_draws(size, bits, groupsize, act_order, vocab, device, seed, n_layers)
-    return LlamaDecoder(L, embed, final_norm, lm_head, LLAMA_SHAPES[size][3], **kw)
+    return LlamaDecoder(L, embed, final_norm, lm_head, LLAMA_SHAPES[size][3], n_kv_heads=kv_heads(size), **kw)
+
+
+def _refuse_gqa_tp(n_heads, n_kv_heads):
+    if n_kv_heads != n_heads:
+        raise ValueError(f'tensor parallelism needs one K/V head per query head; this model has {n_heads} query and {n_kv_heads} K/V heads')
 
 
 def shard_for_rank(layers, lm_head, n_heads, head_dim, rank, size):
     """Tensor-parallel shard of a layer stack (BASELINE config 5; DESIGN.md section 6): qkv columns of this rank's heads (q | k | v), o_proj rows
     of the same heads, gate/up column slabs of 256 with the matching down_proj rows, lm_head rows.  Plain g_idx only (row shards keep whole groups).
+    Multi-head attention only: a grouped-query stack (qkv narrower than 3 * n_heads * head_dim) raises ValueError.
     Returns (local layers, local lm_head, local heads, (vocab_begin, vocab_end))."""
+    H = n_heads * head_dim
+    for ly in layers:
+        _refuse_gqa_tp(n_heads, (ly['qkv'].qweight.shape[1] // head_dim - n_heads) / 2)
     assert n_heads % size == 0, 'heads must divide over the ranks'
     hl = n_heads // size
-    H = n_heads * head_dim
     dev = lm_head.device
     hcols = torch.arange(rank * hl * head_dim, (rank + 1) * hl * head_dim, device=dev)
     out = []
@@ -644,6 +684,7 @@ def synthetic_llama_tp(size_name, rank, world, bits=4, groupsize=128, vocab=3200
     seed layer by layer and keeps its shard), or of the given `full` decoder's weights.  groupsize -1 as in synthetic_llama."""
     hidden, _, _, heads = LLAMA_SHAPES[size_name]
     hd = hidden // heads
+    _refuse_gqa_tp(heads, full.n_kv_heads if full is not None else kv_heads(size_name))
     if full is not None:
         L, lm_head, hl, (v0, v1) = shard_for_rank(full.layers, full.lm_head, heads, hd, rank, world)
         return LlamaDecoder(L, full.embed, full.final_norm, lm_head, hl, head_dim=hd, tp=(rank, world, v0, v1, reduce_mode), **kw)
@@ -673,4 +714,5 @@ def from_hf_quant_model(model, batch=1, max_seq=2048, **kw):
                  input_norm=layer.input_layernorm.weight.data.half().contiguous(), post_norm=layer.post_attention_layernorm.weight.data.half().contiguous()))
     cfg = model.config
     return LlamaDecoder(L, model.model.embed_tokens.weight.data.half(), model.model.norm.weight.data.half().contiguous(), model.lm_head.weight.data.half(),
-                        cfg.num_attention_heads, rms_eps=cfg.rms_norm_eps, rope_base=rope_bases.pop(), batch=batch, max_seq=max_seq, **kw)
+                        cfg.num_attention_heads, rms_eps=cfg.rms_norm_eps, rope_base=rope_bases.pop(), batch=batch, max_seq=max_seq,
+                        n_kv_heads=model.model.layers[0].self_attn.num_key_value_heads, **kw)  # (make_quant_attn read it from the config)

@@ -208,9 +208,11 @@ def lm_head_logprob(x, weight, targets):
 
 def cached_attention(q, k_cache, v_cache, spans):
     """fp16 [M, n_heads * head_dim]: causal attention of new query rows over their sequences' cached prefixes, read in place from one layer's
-    slice of the KV cache (k_cache / v_cache fp16 [batch, n_heads, max_seq, head_dim], keys after RoPE; see gptq_cached_attention).
-    `spans` lists (seq, start, rows): the next `rows` rows of q (fp16 [M, >= n_heads * head_dim], rows may be strided, e.g. the q part of the
-    fused qkv output) are sequence seq's positions start .. start + rows - 1, whose K and V rows the caller has already written."""
+    slice of the KV cache (k_cache / v_cache fp16 [batch, n_kv_heads, max_seq, head_dim], keys after RoPE; see gptq_cached_attention_gqa).
+    `spans` lists (seq, start, rows): the next `rows` rows of q (fp16 [M, n_heads * head_dim], rows may be strided, e.g. the q part of the
+    fused qkv output) are sequence seq's positions start .. start + rows - 1, whose K and V rows the caller has already written.
+    n_heads is q's width over head_dim and n_kv_heads the caches' head count (grouped-query attention: query head h reads K/V head
+    h / (n_heads / n_kv_heads); n_kv_heads = n_heads is multi-head attention)."""
     _require_cuda(q, k_cache, v_cache)
     if q.dim() != 2 or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
         raise ValueError(f'expected q [M, heads * head_dim] and caches [batch, heads, max_seq, head_dim], got {tuple(q.shape)}, {tuple(k_cache.shape)}, '
@@ -219,11 +221,12 @@ def cached_attention(q, k_cache, v_cache, spans):
         raise ValueError('cached_attention expects float16 q and caches')
     if not (k_cache.is_contiguous() and v_cache.is_contiguous()):
         raise ValueError('the KV cache slices must be contiguous')
-    B, nh, S, hd = k_cache.shape
+    B, nkv, S, hd = k_cache.shape
     spans = [(int(b), int(s), int(n)) for b, s, n in spans]
     M = sum(n for _, _, n in spans)
-    if q.shape[0] != M or q.shape[1] != nh * hd:
-        raise ValueError(f'q has shape {tuple(q.shape)}, the spans need [{M}, {nh * hd}]')
+    nh = q.shape[1] // hd
+    if q.shape[0] != M or q.shape[1] != nh * hd or nh % nkv != 0:
+        raise ValueError(f'q has shape {tuple(q.shape)}, the spans need [{M}, n_heads * {hd}] with n_heads a multiple of the cache\'s {nkv} heads')
     out = torch.empty((M, nh * hd), device=q.device, dtype=torch.float16)
     if M == 0:
         return out
@@ -231,8 +234,8 @@ def cached_attention(q, k_cache, v_cache, spans):
     arr = lambda i: (ctypes.c_int32 * len(spans))(*[sp[i] for sp in spans])
     with torch.cuda.device(q.device):
         check(
-            lib.gptq_cached_attention(q.data_ptr(), ld, k_cache.data_ptr(), v_cache.data_ptr(), B, nh, hd, S, len(spans), arr(0), arr(1), arr(2), out.data_ptr(),
-                                      nh * hd, _stream(q)))
+            lib.gptq_cached_attention_gqa(q.data_ptr(), ld, k_cache.data_ptr(), v_cache.data_ptr(), B, nh, nkv, hd, S, len(spans), arr(0), arr(1), arr(2),
+                                          out.data_ptr(), nh * hd, _stream(q)))
     return out
 
 

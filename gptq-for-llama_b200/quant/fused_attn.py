@@ -41,19 +41,30 @@ def rope_base_from_config(config):
     return 10000.0 if base is None else float(base)
 
 
-class QuantLlamaAttention(nn.Module):
-    """Multi-headed attention from 'Attention Is All You Need' paper"""
+def kv_heads_from_config(config):
+    """K/V heads an HF LLaMA config asks for: num_key_value_heads (transformers >= 4.31, and 5.x), else -- older configs, which predate
+    grouped-query attention -- one per attention head."""
+    return getattr(config, 'num_key_value_heads', None) or config.num_attention_heads
 
-    def __init__(self, hidden_size, num_heads, qkv_proj, o_proj, layer_idx=None, rope_base=10000.0):
+
+class QuantLlamaAttention(nn.Module):
+    """Multi-headed attention from 'Attention Is All You Need' paper, and grouped-query attention (num_key_value_heads < num_heads: query head h
+    reads K/V head h / (num_heads / num_key_value_heads)).  qkv_proj is the fused q | k | v projection of num_heads + 2 num_key_value_heads
+    heads; the cache holds num_key_value_heads heads."""
+
+    def __init__(self, hidden_size, num_heads, qkv_proj, o_proj, layer_idx=None, rope_base=10000.0, num_key_value_heads=None):
         super().__init__()
         self.hidden_size = hidden_size
         self.num_heads = num_heads
+        self.num_key_value_heads = num_heads if num_key_value_heads is None else num_key_value_heads
         self.head_dim = hidden_size // num_heads
         self.layer_idx = layer_idx
         self.rope_base = float(rope_base)
         if (self.head_dim * num_heads) != self.hidden_size:
             raise ValueError(f"hidden_size must be divisible by num_heads (got `hidden_size`: {self.hidden_size}"
                              f" and `num_heads`: {num_heads}).")
+        if self.num_key_value_heads < 1 or num_heads % self.num_key_value_heads != 0:
+            raise ValueError(f'num_key_value_heads ({self.num_key_value_heads}) must divide num_heads ({num_heads})')
         self.qkv_proj = qkv_proj
         self.o_proj = o_proj
 
@@ -73,12 +84,14 @@ class QuantLlamaAttention(nn.Module):
         if position_ids is None:
             position_ids = torch.arange(past_len, past_len + q_len, device=hidden_states.device, dtype=torch.long).unsqueeze(0).expand(bsz, -1).contiguous()
 
+        nh, nkv = self.num_heads, self.num_key_value_heads
         qkv_states = self.qkv_proj(hidden_states)
-        qkv_states = qkv_states.view(bsz, q_len, 3, self.num_heads, self.head_dim)
-        ops.rotate_half_(qkv_states[:, :, :2], position_ids, base=self.rope_base)  # q and k rotated in place (:126)
+        qkv_states = qkv_states.view(bsz, q_len, nh + 2 * nkv, self.head_dim)  # q | k | v heads
+        ops.rotate_half_(qkv_states[:, :, :nh + nkv].unsqueeze(2), position_ids, base=self.rope_base)  # q and k rotated in place (:126)
 
-        query_states, key_states, value_states = (t.squeeze(2).transpose(1, 2) for t in torch.split(qkv_states, 1, dim=2))
+        query_states, key_states, value_states = (t.transpose(1, 2) for t in torch.split(qkv_states, [nh, nkv, nkv], dim=2))
         del qkv_states
+        sdpa = dict(enable_gqa=True) if nkv != nh else {}
 
         if modern:
             key_states, value_states = past_key_values.update(key_states, value_states, self.layer_idx)
@@ -91,12 +104,12 @@ class QuantLlamaAttention(nn.Module):
 
         kv_len = key_states.shape[-2]
         if kv_len == q_len:
-            attn_output = F.scaled_dot_product_attention(query_states, key_states, value_states, is_causal=q_len > 1)
+            attn_output = F.scaled_dot_product_attention(query_states, key_states, value_states, is_causal=q_len > 1, **sdpa)
         elif q_len == 1:
-            attn_output = F.scaled_dot_product_attention(query_states, key_states, value_states, is_causal=False)
+            attn_output = F.scaled_dot_product_attention(query_states, key_states, value_states, is_causal=False, **sdpa)
         else:  # chunked prefill on top of a cache: bottom-right aligned causal mask
             mask = torch.ones(q_len, kv_len, dtype=torch.bool, device=hidden_states.device).tril(diagonal=kv_len - q_len)
-            attn_output = F.scaled_dot_product_attention(query_states, key_states, value_states, attn_mask=mask)
+            attn_output = F.scaled_dot_product_attention(query_states, key_states, value_states, attn_mask=mask, **sdpa)
         del query_states, key_states, value_states
 
         attn_output = attn_output.transpose(1, 2).reshape(bsz, q_len, self.hidden_size)
@@ -130,7 +143,8 @@ def fuse_qkv(q_proj, k_proj, v_proj):
 
 
 def make_quant_attn(model):
-    """Replace all LlamaAttention modules with QuantLlamaAttention modules, fusing the q, k, v projections."""
+    """Replace all LlamaAttention modules with QuantLlamaAttention modules, fusing the q, k, v projections (k and v are narrower than q under
+    grouped-query attention).  Only the 'default' RoPE type is accepted (rope_base_from_config)."""
     if not LlamaAttention:
         return
     targets = [name for name, m in model.named_modules() if isinstance(m, LlamaAttention)]
@@ -141,13 +155,12 @@ def make_quant_attn(model):
         cfg = getattr(m, 'config', None)
         hidden_size = getattr(m, 'hidden_size', None) or cfg.hidden_size
         num_heads = getattr(m, 'num_heads', None) or cfg.num_attention_heads
-        kv_heads = getattr(m, 'num_key_value_heads', None) or getattr(cfg, 'num_key_value_heads', num_heads) or num_heads
-        if kv_heads != num_heads:
-            raise ValueError('fused QKV attention requires num_key_value_heads == num_attention_heads (LLaMA-1 style MHA)')
+        kv_heads = getattr(m, 'num_key_value_heads', None) or kv_heads_from_config(cfg if cfg is not None else model.config)
         rope_base = rope_base_from_config(cfg if cfg is not None else model.config)
         qkv_layer = fuse_qkv(m.q_proj, m.k_proj, m.v_proj)
         # the rotary embedding module is dropped: RoPE is computed in the kernel from position_ids and the config's base
-        attn = QuantLlamaAttention(hidden_size, num_heads, qkv_layer, m.o_proj, layer_idx=getattr(m, 'layer_idx', None), rope_base=rope_base)
+        attn = QuantLlamaAttention(hidden_size, num_heads, qkv_layer, m.o_proj, layer_idx=getattr(m, 'layer_idx', None), rope_base=rope_base,
+                                   num_key_value_heads=kv_heads)
         parent_name, _, child_name = name.rpartition('.')
         parent = model.get_submodule(parent_name) if parent_name else model
         setattr(parent, child_name, attn)

@@ -39,8 +39,8 @@ extern "C" {
 
 #define GPTQ_B200_ABI_VERSION 6 /* 2: act-order input gathers; 3: gptq_llama_persistent_scratch_offset; 4: tensor parallelism (gptq_llama_tp, gptq_ipc_*);
                                    5: persistent path at batch 2..8 ([batch][hidden] residual rows in the persistent region);
-                                   6: gptq_lm_head_logprob (scoring); gptq_cached_attention and gptq_sample_tokens added later without a
-                                   change to any existing struct or signature */
+                                   6: gptq_lm_head_logprob (scoring); gptq_cached_attention, gptq_sample_tokens and gptq_cached_attention_gqa
+                                   added later without a change to any existing struct or signature */
 
 typedef void* gptq_stream_t; /* cudaStream_t */
 
@@ -131,7 +131,13 @@ int gptq_dequant(const gptq_qweight* w, void* out, int64_t ldo, gptq_stream_t st
  * [o_proj + residual] -> [RMSNorm + gate/up matvec + SwiGLU] -> [down_proj + residual].
  */
 typedef struct gptq_llama_layer {
-    gptq_qweight qkv;  /* fused q|k|v: N = 3*hidden (quant/fused_attn.py:177-181) */
+    /* fused q|k|v (quant/fused_attn.py:177-181): n_heads query heads, then n_kv_heads key heads, then n_kv_heads value heads of head_dim
+     * columns each, N = (n_heads + 2 * n_kv_heads) * head_dim.  The K/V head count is not a field: it is read from this width,
+     * n_kv_heads = (N / head_dim - n_heads) / 2, and must be a positive divisor of n_heads, the same in every layer (else GPTQ_ERR_SHAPE).
+     * N = 3 * n_heads * head_dim is multi-head attention (LLaMA-1); fewer K/V heads is grouped-query attention (LLaMA-2-70B, CodeLlama-34B,
+     * LLaMA-3): query head h reads K/V head h / (n_heads / n_kv_heads).  Tensor parallelism requires n_kv_heads == n_heads
+     * (GPTQ_ERR_UNSUPPORTED otherwise). */
+    gptq_qweight qkv;
     gptq_qweight o, gate, up, down;
     const void* input_norm;  /* fp16 [hidden] */
     const void* post_norm;   /* fp16 [hidden] */
@@ -177,7 +183,7 @@ typedef struct gptq_llama_tp {
 typedef struct gptq_llama_state {
     int batch;   /* sequences decoded in lock-step, 1..8 */
     int max_seq; /* KV-cache capacity in tokens */
-    void* k_cache; /* fp16 [n_layers, batch, n_heads, max_seq, head_dim], keys stored after RoPE */
+    void* k_cache; /* fp16 [n_layers, batch, n_kv_heads, max_seq, head_dim] (n_kv_heads: gptq_llama_layer.qkv), keys stored after RoPE */
     void* v_cache; /* fp16, same shape */
     const int32_t* tokens;    /* device int32 [batch]: token ids of this step */
     const int32_t* positions; /* device int32 [batch]: position of this step's token (= tokens already cached) */
@@ -228,6 +234,12 @@ int gptq_lm_head_logprob(const void* x, int64_t ldx, const void* w, int64_t ldw,
 int gptq_cached_attention(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int head_dim, int max_seq,
                           int n_spans, const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
                           gptq_stream_t stream);
+/* The same over a grouped-query cache: the caches hold n_kv_heads heads (fp16 [batch, n_kv_heads, max_seq, head_dim]) and query head h reads
+ * K/V head h / (n_heads / n_kv_heads).  n_kv_heads must be a positive divisor of n_heads (GPTQ_ERR_SHAPE otherwise).  gptq_cached_attention is
+ * this call with n_kv_heads = n_heads. */
+int gptq_cached_attention_gqa(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int batch, int n_heads, int n_kv_heads, int head_dim,
+                              int max_seq, int n_spans, const int32_t* span_seq, const int32_t* span_start, const int32_t* span_rows, void* out, int64_t ldo,
+                              gptq_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Sampling (model.generate(do_sample=True, ...) of llama_inference.py:119-127, with HF's warpers in HF's order): one token per row of the
