@@ -63,13 +63,15 @@ constexpr int kStageBytes = 17 * 1024;                  // 17408: stages are 1 K
 constexpr int kHD = 128;
 constexpr int kKeysPerUnit = 32;       // attention work unit: 32 keys of one head = 8 KB of K + 8 KB of V = one stage
 constexpr int kVOff = 8192 + 256;      // V rows of a KV stage (K rows at offset 0)
-constexpr int kRec = kHD + 4;          // floats per attention partial record: m, l, 2 pad, o[128]
+constexpr int kRec = 2 + kHD;          // 64-bit words per attention partial record: m, l, o[128] (each tagged with its epoch: record_epoch)
 constexpr int kMaxLayers = 80;
 constexpr int kMaxStages = 8;
 constexpr int kTeamScratch = 4224;     // per-team scratch (attention merge buffers / lm_head partials)
 constexpr int kLmStageBytes = 16384;   // lm_head bytes per stage (whole rows)
 constexpr int kMaxBatch = 8;           // sequences of one step (the columns of the mma B operand)
-constexpr int kMaxTeams = 1024;        // >= kTeams * SM count of any device this library runs on (attention records in the scratch region)
+constexpr int kMaxTeams = 512;         // >= kTeams * SM count of any device this library runs on (attention records in the scratch region)
+constexpr size_t kPartBytes = 528 * 1024;  // the scratch region of the records: its size is part of the pinned scratch layout
+static_assert((size_t)kMaxTeams * kRec * 8 <= kPartBytes, "attention records exceed their scratch region");
 
 #ifdef GPTQ_TRACE
 }  // namespace
@@ -155,7 +157,7 @@ struct MegaParams {
     float* acc_g;      // [I]
     float* acc_u;      // [I]
     float* acc_d;      // [H]
-    float* part;       // [teams][kRec]  attention partial records (m, l, pad, pad, o[128]), one per team and layer
+    unsigned long long* part;  // [teams][kRec]  attention partial records (m, l, o[128]), one per team and layer, each word tagged with its epoch
     float* rope_cs;    // [128]: cos[64], sin[64] of this step's position
     unsigned long long* bar;  // [0]: monotonic arrival counter of the grid barrier, [1]: its value when the previous launch ended
     // tensor parallelism (tp_size > 1): a rank first reduces its o_proj / down_proj partial sums locally (acc_*_loc), then every CTA adds its
@@ -503,6 +505,45 @@ __device__ __forceinline__ void tp_exchange(const MegaParams& p, float* loc, flo
     }
 }
 
+// ---- attention -> o_proj hand-off: tagged records instead of a grid barrier ---------------------------------------------------
+// Every word of a partial record is one aligned 64-bit access (single-copy atomic): the float's bits in the low half, the epoch of the
+// (launch, layer) that wrote it in the high half.  o_proj's staging loads the words of the records it merges and re-loads only those whose
+// epoch is not yet the current one, so a team starts o_proj as soon as the teams of its own heads are done.
+//
+// Epoch of layer l of the launch whose barrier counter began at `base` (bar[1]): (base + l) mod (2^32 - 1), plus 1, so 0 (the zeroed
+// scratch of a fresh engine) is never used.  A reader can only find, in place of the word it waits for, the same team's word of an
+// earlier layer: every team writes its record in every layer, and the record region is written by nothing else.  Inside a launch that
+// word carries the previous layer's epoch.  Across launches the counter advances by grid times the grid barriers of a launch: 4 n_layers + 1
+// on one GPU; under tensor parallelism, where the hand-offs after O, D and L wait at the cross-GPU barrier, 2 n_layers (direct REDs) or
+// 4 n_layers (with the local exchange).  That is always more than n_layers and far less than 2^32 - 1, so no epoch of the previous launch
+// equals one of this launch.
+__device__ __forceinline__ uint32_t record_epoch(unsigned long long base, int l) { return (uint32_t)((base + (unsigned)l) % 0xffffffffull) + 1u; }
+__device__ __forceinline__ unsigned long long tagged(float v, uint32_t epoch) { return ((unsigned long long)epoch << 32) | __float_as_uint(v); }
+__device__ __forceinline__ void st_record(unsigned long long* w, float v, uint32_t epoch) {
+    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(w), "l"(tagged(v, epoch)) : "memory");
+}
+__device__ __forceinline__ unsigned long long ld_record(const unsigned long long* w) {
+    unsigned long long v;
+    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(w));
+    return v;
+}
+// Waits until the N words loaded into v (from addr(i)) all carry the epoch: each pass re-loads the stale ones together, so a batch of
+// records costs one round trip after its last writer, not one per stale word.
+template <int N, class Addr>
+__device__ __forceinline__ void await_records(unsigned long long (&v)[N], Addr addr, uint32_t epoch) {
+#pragma unroll 1
+    for (;;) {
+        bool stale = false;
+#pragma unroll
+        for (int i = 0; i < N; ++i) stale |= (uint32_t)(v[i] >> 32) != epoch;
+        if (!stale) return;
+#pragma unroll
+        for (int i = 0; i < N; ++i)
+            if ((uint32_t)(v[i] >> 32) != epoch) v[i] = ld_record(addr(i));
+    }
+}
+__device__ __forceinline__ float record_value(unsigned long long v) { return __uint_as_float((uint32_t)v); }
+
 __device__ __forceinline__ void zero_slice(float* buf, int n) {
     // this CTA's share of a distributed memset (n is a multiple of 4)
     const int per = ((n / 4 + gridDim.x - 1) / gridDim.x);
@@ -737,35 +778,52 @@ struct TeamCtx {
     float* xinv_seg;           // [batch]: 2^-e of the staged segment (XScale)
     uint32_t* xmax;            // [batch]: largest fp16 magnitude of the staged segment
     uint8_t* scratch;          // kTeamScratch bytes
+    uint32_t epoch;            // of this layer's attention records (record_epoch)
+#ifdef GPTQ_TRACE
+    int layer;
+#endif
 };
 
-// softmax merge of dimension d of the partial records of teams [ht.first, ht.first + ht.count), NB records per round trip
-template <int NB>
-__device__ __forceinline__ float merge_records(const MegaParams& p, const HeadTeams& ht, int d) {
+// softmax merge of dimension d of the partial records of teams [ht.first, ht.first + ht.count), in rounds of NB records: the round's
+// largest m rescales the running sums once, then l and o[d] are accumulated in record order (a slot past the head's records merges as a
+// neutral record: m = -inf, l = o = 0).  The tagged 64-bit words of a round are fetched in steps -- its NB m words, then the m, l and o[d]
+// words of NG records at a time -- so that no more of them are in flight than in the fast path; the arithmetic and its order do not
+// depend on NG.
+template <int NB, int NG>
+__device__ __forceinline__ float merge_records(const MegaParams& p, const HeadTeams& ht, int d, uint32_t epoch) {
+    static_assert(NB % NG == 0, "a round is a whole number of steps");
     float M = -INFINITY, Ls = 0.f, O = 0.f;
 #pragma unroll 1
     for (int ib = 0; ib < ht.count; ib += NB) {
-        float mv[NB], lv[NB], ov[NB];
-#pragma unroll
-        for (int i = 0; i < NB; ++i) {  // all loads of the batch are in flight together
-            const bool on = ib + i < ht.count;
-            const float* rc = p.part + (size_t)(ht.first + (on ? ib + i : 0)) * kRec;
-            const float m = ld_cg(rc), l = ld_cg(rc + 1), o = ld_cg(rc + 4 + d);
-            mv[i] = on ? m : -INFINITY;
-            lv[i] = on ? l : 0.f;
-            ov[i] = on ? o : 0.f;
-        }
+        const int nb = min(NB, ht.count - ib);  // records of this round
+        const unsigned long long* rc = p.part + (size_t)(ht.first + ib) * kRec;
         float Mb = M;
+        {
+            auto addr = [&](int i) { return rc + i * kRec; };
+            unsigned long long w[NB];
 #pragma unroll
-        for (int i = 0; i < NB; ++i) Mb = fmaxf(Mb, mv[i]);
+            for (int i = 0; i < NB; ++i) w[i] = i < nb ? ld_record(addr(i)) : tagged(-INFINITY, epoch);
+            await_records(w, addr, epoch);
+#pragma unroll
+            for (int i = 0; i < NB; ++i) Mb = fmaxf(Mb, record_value(w[i]));
+        }
         const float w0 = (M == -INFINITY) ? 0.f : expf(M - Mb);
         Ls *= w0;
         O *= w0;
+#pragma unroll 1
+        for (int g = 0; g < NB; g += NG) {  // words [j] = m, [NG + j] = l, [2 NG + j] = o[d] of record g + j (a step past nb loads nothing)
+            auto addr = [&](int j) { return rc + (g + j % NG) * kRec + (j < NG ? 0 : j < 2 * NG ? 1 : 2 + d); };
+            unsigned long long w[3 * NG];
 #pragma unroll
-        for (int i = 0; i < NB; ++i) {
-            const float w = (mv[i] == -INFINITY) ? 0.f : expf(mv[i] - Mb);
-            Ls = fmaf(lv[i], w, Ls);
-            O = fmaf(ov[i], w, O);
+            for (int j = 0; j < 3 * NG; ++j) w[j] = g + j % NG < nb ? ld_record(addr(j)) : tagged(j < NG ? -INFINITY : 0.f, epoch);
+            await_records(w, addr, epoch);
+#pragma unroll
+            for (int j = 0; j < NG; ++j) {
+                const float m = record_value(w[j]);
+                const float wt = (m == -INFINITY) ? 0.f : expf(m - Mb);
+                Ls = fmaf(record_value(w[NG + j]), wt, Ls);
+                O = fmaf(record_value(w[2 * NG + j]), wt, O);
+            }
         }
         M = Mb;
     }
@@ -811,8 +869,10 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
         }
     } else {
         // attention output: softmax-merge of the partial records (m, l, o[128]) of the head's teams (head_teams: contiguous, one
-        // record each; BATCH: the head's teams inside the sequence's teams, seq_teams).
-        constexpr int kBatch = 12;  // records fetched per round trip (a 7B head has 9 or 10 teams)
+        // record each; BATCH: the head's teams inside the sequence's teams, seq_teams).  No grid barrier precedes this: a record word is
+        // used once it carries this layer's epoch (await_records), while other teams may still be in attention.
+        constexpr int kBatch = 12;  // records fetched per round trip (a 7B head has 9 or 10 teams); merge_records' round
+        constexpr int kMergeStep = 3;  // records whose m, l, o words merge_records fetches per round trip (more spill)
         uint32_t vmax = 0;  // largest fp16 magnitude this thread put (per sequence: flushed into xmax)
         auto put = [&](__half* xseg, int e, float v) {
             const __half hv = __float2half_rn(v);
@@ -839,8 +899,14 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
                     const int head = k / kHD, d = k - head * kHD;
                     slot = ((e >> 5) < nA) ? head - hA0 : nslotA + head;
                     const HeadTeams ht = head_teams(head, p.n_heads, tc.nb);
+                    const unsigned long long* rc = p.part + (size_t)ht.first * kRec + 2 + d;
+                    auto addr = [&](int i) { return rc + i * kRec; };
+                    unsigned long long w[kBatch];
 #pragma unroll
-                    for (int i = 0; i < kBatch; ++i) ov[i] = (active && i < ht.count) ? ld_cg(p.part + (size_t)(ht.first + i) * kRec + 4 + d) : 0.f;
+                    for (int i = 0; i < kBatch; ++i) w[i] = (active && i < ht.count) ? ld_record(addr(i)) : tagged(0.f, tc.epoch);
+                    await_records(w, addr, tc.epoch);
+#pragma unroll
+                    for (int i = 0; i < kBatch; ++i) ov[i] = record_value(w[i]);
                 };
                 auto emit = [&](int e) {
                     if (e < nfeat) {
@@ -857,8 +923,12 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
                     const HeadTeams ht = head_teams(head, p.n_heads, tc.nb);
                     float m = -INFINITY, l = 0.f;
                     if (lane < ht.count) {
-                        m = ld_cg(p.part + (size_t)(ht.first + lane) * kRec);
-                        l = ld_cg(p.part + (size_t)(ht.first + lane) * kRec + 1);
+                        const unsigned long long* rc = p.part + (size_t)(ht.first + lane) * kRec;
+                        auto addr = [&](int i) { return rc + i; };
+                        unsigned long long w[2] = {ld_record(rc), ld_record(rc + 1)};
+                        await_records(w, addr, tc.epoch);
+                        m = record_value(w[0]);
+                        l = record_value(w[1]);
                     }
                     float M = m;
 #pragma unroll
@@ -892,7 +962,7 @@ __device__ void stage_range(const MegaParams& p, const TeamCtx& tc, int nk, int 
                     const int head = k / kHD, d = k - head * kHD;
                     HeadTeams ht = head_teams(head, p.n_heads, st.count);
                     ht.first += st.first;
-                    put(tc.xseg + (size_t)s * p.xs_stride, e, merge_records<kBatch>(p, ht, d));
+                    put(tc.xseg + (size_t)s * p.xs_stride, e, merge_records<kBatch, kMergeStep>(p, ht, d, tc.epoch));
                 }
                 atomicMax(tc.xmax + s, vmax);
                 vmax = 0;
@@ -947,6 +1017,9 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
             if (g_mega_trace != nullptr && threadIdx.x == 0) g_mega_trace[blockIdx.x * 64 + 36 + XMODE] += (unsigned long long)(clock64() - stg0);
 #endif
         }
+#ifdef GPTQ_TRACE
+        if (XMODE == X_ATTN) MTRACE(tc.layer * 12 + 5);
+#endif
     }
 
 #pragma unroll 1
@@ -1067,7 +1140,7 @@ __device__ void run_matvec(const MegaParams& p, ConsRing& ring, const TeamCtx& t
 
 // ---- attention ----------------------------------------------------------------------------------------------------------
 // Work units (head, 32 keys); a team serves one head (attn_range); one unit = one ring stage (K rows, V rows).  The team writes
-// one partial record (m, l, o[128]) to p.part[T].
+// one partial record (m, l, o[128]) to p.part[T], tagged with the layer's epoch.
 // BATCH: the team serves one (sequence, head) pair (attn_work), at that sequence's position, in that sequence's cache slot.
 // Grouped-query attention: query head h reads K/V head h / kv_group.  Every team owning the unit that holds pos rotates the new key itself
 // and patches its own staged copy with it; only the group's first query head stores the row to the cache, and no team reads another
@@ -1085,12 +1158,12 @@ __device__ void run_attention(const MegaParams& p, ConsRing& ring, const TeamCtx
     const int ub_new = pos / kKeysPerUnit;  // the unit that holds this step's key
     __half* kc_l = p.k_cache + layer * p.layer_stride;
     __half* vc_l = p.v_cache + layer * p.layer_stride;
-    float* rec = p.part + (size_t)tc.T * kRec;
+    unsigned long long* rec = p.part + (size_t)tc.T * kRec;
     if (b0 >= b_end) {  // no unit for this team (short context): a neutral record keeps the merge uniform
-        if (ttid < kHD) rec[4 + ttid] = 0.f;
+        if (ttid < kHD) st_record(rec + 2 + ttid, 0.f, tc.epoch);
         if (ttid == 0) {
-            rec[0] = -INFINITY;
-            rec[1] = 0.f;
+            st_record(rec, -INFINITY, tc.epoch);
+            st_record(rec + 1, 0.f, tc.epoch);
         }
         return;
     }
@@ -1222,10 +1295,10 @@ __device__ void run_attention(const MegaParams& p, ConsRing& ring, const TeamCtx
                 L = fmaf(red_ml[w * 2 + 1], wgt, L);
                 O = fmaf(red_o[w * kHD + ttid], wgt, O);
             }
-            rec[4 + ttid] = O;
+            st_record(rec + 2 + ttid, O, tc.epoch);
             if (ttid == 0) {
-                rec[0] = M;
-                rec[1] = L;
+                st_record(rec, M, tc.epoch);
+                st_record(rec + 1, L, tc.epoch);
             }
         }
     }
@@ -1465,6 +1538,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p.bar + 1) : "memory");
         gen = v;
     }
+    const unsigned long long epoch_base = gen;  // the same in every thread (record_epoch)
     unsigned long long xgen = 0;  // the same for the cross-GPU barrier (tensor parallelism)
     if (p.tp_size > 1) asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(xgen) : "l"(p.xbar_peer[p.tp_rank] + 32 * kMaxTP) : "memory");
     // after the o_proj, down_proj and lm_head operations every rank needs every rank's contributions
@@ -1509,6 +1583,10 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
 #pragma unroll 1
     for (int l = 0; l < p.n_layers; ++l) {
         const LayerDesc& L = p.layers[l];
+        tc.epoch = record_epoch(epoch_base, l);
+#ifdef GPTQ_TRACE
+        tc.layer = l;
+#endif
         // ---- Q ----
         MTRACE(l * 12 + 0);
         stage_norms(false, resid_src, resid_acc, L.input_norm, p.resid[cur ^ 1], L.qkv_perm);
@@ -1532,10 +1610,8 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
             OPTRACE_END(ring, l, 1);
         }
         MTRACE(l * 12 + 4);
-        grid_barrier(p.bar, gen);
-        MTRACE(l * 12 + 5);
-        // ---- O ----
-        zero_slice(p.acc_qkv, nbat * p.Nqkv);
+        // ---- O ---- (no barrier: the staging waits for the records it merges, tagged with tc.epoch.  Nothing else that A reads or
+        // writes is touched by O: acc_qkv is cleared in G, xs and the team scratch are per team, and rope_cs is written once per launch)
         {
             OPTRACE_BEGIN(ring);
             if constexpr (BATCH)
@@ -1548,6 +1624,7 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         sync_all_ranks(p.acc_o_loc, p.acc_o_peer);
         MTRACE(l * 12 + 7);
         // ---- G ----
+        zero_slice(p.acc_qkv, nbat * p.Nqkv);  // last read by this layer's A, which every CTA finished before the O barrier
         stage_norms(false, p.resid[cur], p.acc_o, L.post_norm, p.resid[cur ^ 1], L.mlp_perm);
         cur ^= 1;
         MTRACE(l * 12 + 8);
@@ -1665,7 +1742,7 @@ MegaScratch mega_scratch(const gptq_llama_model& m, int batch) {
     s.acc_qkv = carve(s.total, B * 3 * H * 4);
     s.acc_g = carve(s.total, B * I * 4);
     s.acc_u = carve(s.total, B * I * 4);
-    s.part = carve(s.total, (size_t)kMaxTeams * kRec * 4);
+    s.part = carve(s.total, kPartBytes);
     s.rope_cs = carve(s.total, B * 128 * 4);
     s.bar = carve(s.total, 256);
     return s;
@@ -1783,7 +1860,7 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     p.acc_qkv = reinterpret_cast<float*>(scratch + ms.acc_qkv);
     p.acc_g = reinterpret_cast<float*>(scratch + ms.acc_g);
     p.acc_u = reinterpret_cast<float*>(scratch + ms.acc_u);
-    p.part = reinterpret_cast<float*>(scratch + ms.part);
+    p.part = reinterpret_cast<unsigned long long*>(scratch + ms.part);
     p.rope_cs = reinterpret_cast<float*>(scratch + ms.rope_cs);
     p.bar = reinterpret_cast<unsigned long long*>(scratch + ms.bar);
     // One tensor map per row stride serves every layer: class 0 = qkv (N = Nqkv), 1 = o and down (N = H), 2 = gate and up (N = I).

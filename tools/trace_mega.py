@@ -20,12 +20,15 @@ torch.cuda.synchronize()
 print('logits finite:', bool(torch.isfinite(dec.logits).all()), 'rms', dec.logits.float().pow(2).mean().sqrt().item())
 t = buf.cpu().view(NCTA, 64).double()
 t0 = t[:, 0].min()
-names = ['Q start', 'Q x staged', 'Q matvec done', 'Q barrier passed', 'A done', 'A barrier passed', 'O done', 'O barrier passed', 'G x staged', 'G done', 'D start(after barrier)', 'D done']
+# no barrier between A and O: O starts when A is done, and its staging waits for the records of its heads ('O x staged': team 0)
+names = ['Q start', 'Q x staged', 'Q matvec done', 'Q barrier passed', 'A done', 'O x staged', 'O done', 'O barrier passed', 'G x staged', 'G done', 'D start(after barrier)', 'D done']
 for l in range(1, 3):
     print(f'layer {l}: (min / median / max over CTAs, us since kernel start)')
     for k in range(12):
         c = (t[:, l * 12 + k] - t0) / 1e3
         print(f'  {names[k]:24s} {c.min().item():8.2f} {c.median().item():8.2f} {c.max().item():8.2f}')
+    early = int((t[:, l * 12 + 5] < t[:, l * 12 + 4].max()).sum())
+    print(f'  CTAs whose O staging ended before the last CTA finished A: {early} / {NCTA}')
     if (l + 1) * 12 < 36:  # only ids below 36 are recorded: the next layer's start is known for layer 1 alone
         print(f'  layer total {((t[:, (l + 1) * 12] - t[:, l * 12]) / 1e3).median().item():.2f} us')
 print('layer 2, team 0 of every CTA (median over CTAs): cycles in op / waiting for stages / stages / busy cycles per stage')
