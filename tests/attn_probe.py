@@ -4,9 +4,13 @@
   exactly +-1 in both engines (the sum of squares is H * 2^-8, so every sqrtf and division is exact).
 * qkv.  int4 with scale 2^-4, every weight equal to its column's zero point except one tap per column (exact_fixtures.pow2_packed taken to
   a single term): q_n = x_k * d * 2^-4 with |d| in [4, 7] on a feature k >= V_TAPS, v_n = d * 2^-4 with d in [8, 14] on a feature
-  k < V_TAPS (so v > 0).  Every sum is exact in any order.  The k columns are a copy of the q columns, and both engines rotate q and k with
-  the same expression (decode.cu attn_decode_kernel, decode_mega.cu run_attention), so the appended K row IS the kernel's rotated q, bit for
-  bit: the reference reads it back from a first pass instead of re-deriving the fp32 RoPE (which check_rope_row holds to fp64 separately).
+  k < V_TAPS (so v > 0).  Every sum is exact in any order.  With n_kv_heads K/V heads (g = nh / nkv query heads per K/V head) the 64 RoPE
+  pairs (i, i + 64) of each K/V group are split into g disjoint sets, one per query head (pair_split): query head h taps only the pairs of
+  its set, its other q columns stay at the zero point and are exactly 0, and on pair i the k columns of K/V head h / g copy the taps of the
+  query head that owns i.  RoPE works pair by pair (a zero pair rotates to zeros), and both engines rotate q and k with the same
+  expression (decode.cu attn_decode_kernel, decode_mega.cu run_attention), so the kernel's rotated q of head h IS the appended K row of its
+  K/V head masked to h's pairs, bit for bit: the reference reads it back from a first pass instead of re-deriving the fp32 RoPE (which
+  check_rope_row holds to fp64 separately).  At g = 1 the set is every pair and the k columns are a copy of the q columns.
 * o_proj.  int4 identity (q - z = delta, z = 1, scale 1); with act_order a random g_idx, which kernel_form regroups (o_perm).
 * MLP.  gate, up and down have scale 0: the MLP adds exactly 0, so the residual after the step is the residual after attention,
   x_out = fp16(x_in + fp16(att)).
@@ -59,17 +63,44 @@ def _g_idx(K, gs, act_order, gen):
     return g.to(torch.int32)
 
 
-def probe_weights(H, I, act_order=False, seed=0, gs=128):
-    """CPU tensors of the probe layer: dict of (qweight, scales, qzeros, g_idx, groupsize) per linear, plus the qkv taps."""
+def pair_split(nh, nkv, gen):
+    """support [nh, 64] bool: the RoPE pairs (i, i + 64) on which query head h has q taps.  Within each K/V group the g = nh / nkv query
+    heads get disjoint sets that together cover the 64 pairs exactly once, split at random (drawn from gen); at g = 1 the single set is every
+    pair and nothing is drawn."""
+    g = nh // nkv
+    assert nh % nkv == 0 and g <= 64, (nh, nkv)
+    if g == 1:
+        return torch.ones(nh, 64, dtype=torch.bool)
+    sup = torch.zeros(nh, 64, dtype=torch.bool)
+    for c in range(nkv):
+        perm = torch.randperm(64, generator=gen)
+        for j in range(g):
+            sup[c * g + j, perm[j * 64 // g:(j + 1) * 64 // g]] = True
+    return sup
+
+
+def probe_weights(H, I, act_order=False, seed=0, gs=128, n_kv_heads=None):
+    """CPU tensors of the probe layer: dict of (qweight, scales, qzeros, g_idx, groupsize) per linear, the qkv taps
+    (tq, dq, tk, dk, tv, dv) and the pair support of every query head (pair_split).  n_kv_heads: K/V heads (None: H / 128, multi-head).
+    The qkv is (nh + 2 nkv) * 128 wide; query head h taps only the pairs of its set (its other columns are exactly 0), and on pair i of K/V
+    head c the k columns copy the taps of the query head whose set holds i."""
+    nh = H // HD
+    nkv = nh if n_kv_heads is None else n_kv_heads
+    Hkv = nkv * HD
     gen = torch.Generator().manual_seed(seed)
     tq = torch.randint(V_TAPS, H, (H, ), generator=gen)
     dq = torch.randint(4, 8, (H, ), generator=gen) * (1 - 2 * torch.randint(0, 2, (H, ), generator=gen))
-    tv = torch.randint(0, V_TAPS, (H, ), generator=gen)
-    dv = torch.randint(8, 15, (H, ), generator=gen)
+    tv = torch.randint(0, V_TAPS, (Hkv, ), generator=gen)
+    dv = torch.randint(8, 15, (Hkv, ), generator=gen)
+    sup = pair_split(nh, nkv, gen)
+    dq = dq * pair_mask(sup).reshape(-1)  # off the head's pairs the tap is the zero point: q = 0
+    owner = torch.arange(nkv)[:, None] * (nh // nkv) + sup.view(nkv, nh // nkv, 64).to(torch.int64).argmax(1)  # [nkv, 64]: query head of pair i
+    src = ((owner * HD).repeat(1, 2) + torch.arange(HD)).reshape(-1)  # the q column each k column copies
+    tk, dk = tq[src], dq[src]
     G = H // gs
-    base = torch.cat([torch.full((2 * H, ), 8), torch.full((H, ), 1)])  # nibble of the zero point: z = stored zero + 1
-    qkv = (_pack_taps(H, base, torch.cat([tq, tq, tv]), torch.cat([8 + dq, 8 + dq, 1 + dv]), 'cpu'), torch.full((G, 3 * H), 2.0**-4).half(),
-           _as_int32(torch.cat([torch.full((G, 2 * H // 8), _word(7)), torch.zeros(G, H // 8, dtype=torch.int64)], 1)), _g_idx(H, gs, act_order, gen), gs)
+    base = torch.cat([torch.full((H + Hkv, ), 8), torch.full((Hkv, ), 1)])  # nibble of the zero point: z = stored zero + 1
+    qkv = (_pack_taps(H, base, torch.cat([tq, tk, tv]), torch.cat([8 + dq, 8 + dk, 1 + dv]), 'cpu'), torch.full((G, H + 2 * Hkv), 2.0**-4).half(),
+           _as_int32(torch.cat([torch.full((G, (H + Hkv) // 8), _word(7)), torch.zeros(G, Hkv // 8, dtype=torch.int64)], 1)), _g_idx(H, gs, act_order, gen), gs)
     eye = _pack_taps(H, torch.ones(H, dtype=torch.int64), torch.arange(H), torch.full((H, ), 2), 'cpu')
     o = (eye, torch.ones(G, H).half(), torch.zeros(G, H // 8, dtype=torch.int32), _g_idx(H, gs, act_order, gen), gs)
     gm = 128 if I % 128 == 0 else 64
@@ -79,7 +110,7 @@ def probe_weights(H, I, act_order=False, seed=0, gs=128):
         return (_as_int32(torch.full((K // 8, N), _word(8))), torch.zeros(K // gm, N).half(), torch.zeros(K // gm, N // 8, dtype=torch.int32), g, gm)
 
     return dict(qkv=qkv, o=o, gate=zero_layer(H, I, g_mlp), up=zero_layer(H, I, g_mlp.clone()), down=zero_layer(I, H, _g_idx(I, gm, act_order, gen)),
-                taps=(tq, dq, tv, dv))
+                taps=(tq, dq, tk, dk, tv, dv), support=sup)
 
 
 def probe_embed(vocab, H, seed=0):
@@ -90,10 +121,16 @@ def probe_embed(vocab, H, seed=0):
 
 
 def exact_qv(w, embed_row):
-    """float64 q (before RoPE) and v [H] of the probe for one embedding row: one tap per column, x = embed * 16 = +-1."""
-    tq, dq, tv, dv = w['taps']
+    """float64 q (before RoPE) [H], k (before RoPE) and v [nkv * 128] of the probe for one embedding row: one tap per column, x = embed * 16
+    = +-1."""
+    tq, dq, tk, dk, tv, dv = w['taps']
     x = embed_row.double().cpu() * 16
-    return x[tq] * dq * 2.0**-4, x[tv] * dv * 2.0**-4
+    return x[tq] * dq * 2.0**-4, x[tk] * dk * 2.0**-4, x[tv] * dv * 2.0**-4
+
+
+def pair_mask(support):
+    """[nh, 128] bool: the columns of each query head's pairs (i and i + 64 for every pair i of its set)."""
+    return support.repeat(1, 2)
 
 
 def align256(v):
@@ -109,15 +146,17 @@ def resid_buffers(dec):
 
 
 class Probe:
-    """The probe model on a LlamaDecoder (1 layer).  learn() is pass 1 of a (tokens, positions) step: it reads the appended K rows (= the
-    kernel's rotated q) and V rows; run() is pass 2: it plants the cache, poisons the rows at and after each position with NaN, steps, checks
-    that the appended rows are bit-identical to pass 1 and returns (x_in, x_out) [B, H] fp16."""
+    """The probe model on a LlamaDecoder (1 layer, n_kv_heads K/V heads: default engine.kv_heads(size)).  learn() is pass 1 of a (tokens,
+    positions) step: it reads the appended K and V rows of every K/V head (k_new, v_new) and from them each query head's rotated q (q_rot:
+    the K row of its K/V head masked to its pairs); run() is pass 2: it plants the cache, poisons the rows at and after each position with
+    NaN, steps, checks that exactly row pos of every K/V head was written, bit-identical to pass 1, and returns (x_in, x_out) [B, H] fp16."""
 
-    def __init__(self, size, batch=1, max_seq=2048, act_order=False, vocab=64, seed=0, lm_head=None, rope_base=10000.0):
+    def __init__(self, size, batch=1, max_seq=2048, act_order=False, vocab=64, seed=0, lm_head=None, rope_base=10000.0, n_kv_heads=None):
         from gptq_b200 import engine
         H, I, _, nh = engine.LLAMA_SHAPES[size]
+        nkv = engine.kv_heads(size) if n_kv_heads is None else n_kv_heads
         dev = torch.device('cuda:0')
-        self.w = probe_weights(H, I, act_order, seed)
+        self.w = probe_weights(H, I, act_order, seed, n_kv_heads=nkv)
         L = {}
         for name in ('qkv', 'o', 'gate', 'up', 'down'):
             qw, sc, qz, g, gs = self.w[name]
@@ -128,11 +167,12 @@ class Probe:
         if lm_head is None:
             lm_head = (torch.randn(vocab, H, generator=torch.Generator().manual_seed(seed + 2)) * 0.02).half()
         self.dec = engine.LlamaDecoder([L], embed, torch.ones(H, dtype=torch.float16, device=dev), lm_head.to(dev), nh, rms_eps=0.0, batch=batch,
-                                       max_seq=max_seq, rope_base=rope_base)
-        self.H, self.nh, self.B, self.max_seq, self.rope_base = H, nh, batch, max_seq, rope_base
+                                       max_seq=max_seq, rope_base=rope_base, n_kv_heads=nkv)
+        self.H, self.nh, self.nkv, self.g, self.B, self.max_seq, self.rope_base = H, nh, nkv, nh // nkv, batch, max_seq, rope_base
+        self.mask = pair_mask(self.w['support']).to(dev)
         self.persistent = self.dec.launches_per_step() == 1
         self.nb = 2 * torch.cuda.get_device_properties(dev).multi_processor_count
-        self.q_rot = self.v_new = None
+        self.q_rot = self.k_new = self.v_new = None
 
     def _step(self, toks, positions):
         self.dec.set_input(toks, positions)
@@ -147,11 +187,12 @@ class Probe:
         self.dec.k_cache.zero_()
         self.dec.v_cache.zero_()
         self._step(toks, positions)
-        self.q_rot, self.v_new = self.appended(positions)
+        self.k_new, self.v_new = self.appended(positions)
+        self.q_rot = [k.repeat_interleave(self.g, 0).masked_fill(~self.mask, 0) for k in self.k_new]
         return self.q_rot, self.v_new
 
     def run(self, toks, positions, plants):
-        """plants[b] = (K, V) fp16 [nh, positions[b], 128]: the cache rows before sequence b's position."""
+        """plants[b] = (K, V) fp16 [nkv, positions[b], 128]: the cache rows before sequence b's position."""
         kc, vc = self.dec.k_cache, self.dec.v_cache
         for b, (p, (K, V)) in enumerate(zip(positions, plants)):
             kc[0, b, :, :p] = K
@@ -160,8 +201,10 @@ class Probe:
             vc[0, b, :, p:] = float('nan')
         self._step(toks, positions)
         k2, v2 = self.appended(positions)
-        for b in range(self.B):
-            assert torch.equal(k2[b], self.q_rot[b]) and torch.equal(v2[b], self.v_new[b]), f'sequence {b}: pass 2 appended other K / V rows'
+        for b, (p, (K, V)) in enumerate(zip(positions, plants)):
+            assert torch.equal(k2[b], self.k_new[b]) and torch.equal(v2[b], self.v_new[b]), f'sequence {b}: pass 2 appended other K / V rows'
+            assert torch.equal(kc[0, b, :, :p], K) and torch.equal(vc[0, b, :, :p], V), f'sequence {b}: a planted row before pos {p} changed'
+            assert bool(kc[0, b, :, p + 1:].isnan().all() and vc[0, b, :, p + 1:].isnan().all()), f'sequence {b}: a row after pos {p} was written'
         if self.persistent:
             x_in, x_out = resid_buffers(self.dec)
             assert torch.equal(x_in, self.dec.embed[torch.tensor(toks, device=x_in.device)]), 'residual entering the layer is not the embedding row'
@@ -196,12 +239,15 @@ def x_bound(att, x_ref, E):
 
 
 # ----------------------------------------------------------------------------- planted keys
-def keys_for_scores(q, alpha, gen, noise=0.02):
-    """K [nh, T, 128] fp16 whose scores scale * q.K_t are about alpha [nh, T]: alpha_t times q / (scale |q|^2), plus small noise."""
+def keys_for_scores(q, alpha, gen, noise=0.02, g=1):
+    """K [nh / g, T, 128] fp16 whose scores scale * q_h.K_t are about alpha [nh, T] for every query head h: K/V head c holds
+    sum_j alpha_{cg+j} u_{cg+j} plus small noise, u_h = q_h / (scale |q_h|^2).  The query heads of a group have disjoint supports
+    (pair_split), so q_h.u_h' = 0 for h' != h and each head scores against its own alpha."""
     qd = q.double()
     u = qd / (SCALE * (qd * qd).sum(-1, keepdim=True))
-    eta = torch.randn(alpha.shape + (HD, ), generator=gen, device=q.device, dtype=torch.float64) * noise
-    return (alpha[..., None] * u[:, None, :] + eta).half()
+    nh, T = alpha.shape
+    eta = torch.randn((nh // g, T, HD), generator=gen, device=q.device, dtype=torch.float64) * noise
+    return ((alpha[..., None] * u[:, None, :]).view(nh // g, g, T, HD).sum(1) + eta).half()
 
 
 def new_key_score(q):
@@ -236,15 +282,16 @@ def random_values(nh, n, gen, device):
 PROFILES = ('heavy', 'ramp', 'late', 'new_max', 'offset', 'wide', 'uniform')
 
 
-def profile(kind, q, n, gen, heavy=None):
-    """(K, V) [nh, n, 128] fp16 planted before a new key whose score is new_key_score(q):
+def profile(kind, q, n, gen, heavy=None, g=1):
+    """(K, V) [nh / g, n, 128] fp16 planted before a new key whose score is new_key_score(q), per query head h of q [nh, 128]:
       heavy    background N(0, 1), the keys heavy[h] of head h about 10 above it (distinct random V rows)
       ramp     the scores climb with t: the running max moves in every unit and split (the alpha / w0 rescale)
       late     background N(0, 1), the max (+12) in the last unit and at the first key of the last split
       new_max  every planted key 10 below the new key
       offset   scores about +90 (fp32 exp overflows without the max subtraction); the new key ends up with weight 0
       wide     scores spread over 60: most of the background underflows next to the max
-      uniform  near-equal scores: a missing unit of 32 keys shifts att by 32 / T of |V - att|"""
+      uniform  near-equal scores: a missing unit of 32 keys shifts att by 32 / T of |V - att|
+    g query heads share each K/V head (keys_for_scores)."""
     nh, dev = q.shape[0], q.device
     rnd = lambda *s: torch.randn(*s, generator=gen, device=dev, dtype=torch.float64)
     t = torch.arange(n, device=dev, dtype=torch.float64)
@@ -270,7 +317,7 @@ def profile(kind, q, n, gen, heavy=None):
         alpha = 0.05 * rnd(nh, n)
     else:
         raise ValueError(kind)
-    return keys_for_scores(q, alpha, gen), random_values(nh, n, gen, dev)
+    return keys_for_scores(q, alpha, gen, g=g), random_values(nh // g, n, gen, dev)
 
 
 # ----------------------------------------------------------------------------- the persistent kernel's attention partition
@@ -377,15 +424,15 @@ def emulate_persistent(q, K, V, ranges):
 
 
 # ----------------------------------------------------------------------------- RoPE of the appended K row
-def check_rope_row(k_row, q_exact, pos, rope_base):
-    """The appended K row [nh, 128] (fp16) against fp64 RoPE of the exact q / k [H] at base rope_base, the angle computed in fp32 as the
+def check_rope_row(k_row, k_exact, pos, rope_base):
+    """The appended K rows [nkv, 128] (fp16) against fp64 RoPE of the exact k [nkv * 128] (exact_qv) at base rope_base, the angle computed in fp32 as the
     reference formula does (quant/fused_attn.py:43): within 1 ulp16, plus a 4-ulp difference in the fp32 angle and in cos / sin.  Returns the
     worst |err| / bound."""
     f = np.float32
     inv_base = f(-2.0 * math.log(rope_base) / HD)
     th = (np.exp(np.arange(64, dtype=f) * inv_base).astype(f) * f(pos)).astype(np.float64)
-    x = q_exact.view(-1, HD)[:, :64].numpy()
-    y = q_exact.view(-1, HD)[:, 64:].numpy()
+    x = k_exact.view(-1, HD)[:, :64].numpy()
+    y = k_exact.view(-1, HD)[:, 64:].numpy()
     c, s = np.cos(th), np.sin(th)
     ref = torch.from_numpy(np.concatenate([x * c - y * s, x * s + y * c], 1))
     dth = 4 * np.spacing(th.astype(f)).astype(np.float64) + 4 * U24

@@ -8,7 +8,11 @@ v, identity o_proj, zero MLP: the residual after a step is fp16(x_in + fp16(att)
 * Bounded profiles (attn_probe.PROFILES): x_out against x_in + att of a float64 softmax over the kernel's own q_rot, K and V rows, per
   element within attn_probe.x_bound.  Heavy keys are put at 0, at the last planted key, on both sides of every unit and split edge and at
   both ends of every team range; at the longest 7B context the heavy sets rotate until every key has been heavy in some head.
-* The cache rows at and after each position hold NaN before the step: the kernel must write the new row and never read a later one.
+* The cache rows at and after each position hold NaN before the step: the kernel must write the new row and never read a later one.  After
+  the step the planted rows are bitwise unchanged and the later rows still NaN: exactly row pos of every K/V head was written.
+* Grouped-query shapes (tiny-gqa*, LLaMA-3-8B, LLaMA-2-70B, CodeLlama-34B, and one K/V head at 7B and tiny): the query heads of a group
+  have disjoint q supports, so each scores only the part of the shared K rows planted for it; a key read from another group, dropped at a
+  team edge or left unpatched in one team's stage moves that head's output as in the multi-head case.
 
 The worst |err| / bound of every sweep is printed (pytest -s)."""
 import numpy as np
@@ -39,10 +43,10 @@ class Worst:
 
 def anchors(probe, toks, positions, gen, what):
     """Equal scores and zero-sum values (pos 0: the lone new key): x_out must be x_in (fp16(x_in + v_new) at pos 0) bit for bit."""
-    plants = [(q[:, None, :].expand(-1, p, -1).contiguous(), P.zero_sum_values(v, p, gen)) for q, v, p in zip(probe.q_rot, probe.v_new, positions)]
+    plants = [(k[:, None, :].expand(-1, p, -1).contiguous(), P.zero_sum_values(v, p, gen)) for k, v, p in zip(probe.k_new, probe.v_new, positions)]
     x_in, x_out = probe.run(toks, positions, plants)
     for b, p in enumerate(positions):
-        want = x_in[b] if p > 0 else (x_in[b].double() + probe.v_new[b].reshape(-1).double()).half()
+        want = x_in[b] if p > 0 else (x_in[b].double() + probe.v_new[b].repeat_interleave(probe.g, 0).reshape(-1).double()).half()
         if not torch.equal(x_out[b], want):
             d = fp16_ulp_distance(x_out[b], want)
             i = int(torch.nonzero(d)[0])
@@ -53,8 +57,8 @@ def anchors(probe, toks, positions, gen, what):
 def bounded(probe, toks, positions, plants, worst, what):
     x_in, x_out = probe.run(toks, positions, plants)
     for b, p in enumerate(positions):
-        K = torch.cat([plants[b][0], probe.q_rot[b][:, None, :]], 1)
-        V = torch.cat([plants[b][1], probe.v_new[b][:, None, :]], 1)
+        K = torch.cat([plants[b][0], probe.k_new[b][:, None, :]], 1).repeat_interleave(probe.g, 0)
+        V = torch.cat([plants[b][1], probe.v_new[b][:, None, :]], 1).repeat_interleave(probe.g, 0)
         att, E = P.softmax_ref(probe.q_rot[b], K, V)
         x_ref = x_in[b].double().view(-1, P.HD) + att
         out = x_out[b].double().view(-1, P.HD)
@@ -88,9 +92,9 @@ def sweep(probe, position_sets, profiles, gen, worst, rope, tok0=0, rotate_heavy
         toks = [(tok0 + 7 * i + 3 * b) % vocab for b in range(probe.B)]
         what = f'toks {toks} positions {positions}'
         probe.learn(toks, positions)
-        for b, p in enumerate(positions):  # the appended K row (= q_rot) against fp64 RoPE of the exact q
-            q_exact = P.exact_qv(probe.w, probe.dec.embed[toks[b]])[0]
-            rope.update(P.check_rope_row(probe.q_rot[b], q_exact, p, probe.rope_base), f'{what} seq {b}')
+        for b, p in enumerate(positions):  # the appended K rows (q_rot, masked) against fp64 RoPE of the exact k
+            k_exact = P.exact_qv(probe.w, probe.dec.embed[toks[b]])[1]
+            rope.update(P.check_rope_row(probe.k_new[b], k_exact, p, probe.rope_base), f'{what} seq {b}')
         anchors(probe, toks, positions, gen, what)
         for kind in profiles:
             if kind == 'heavy':
@@ -98,10 +102,10 @@ def sweep(probe, position_sets, profiles, gen, worst, rope, tok0=0, rotate_heavy
                 if len(positions) == 1 and positions[0] in full_rotation:
                     passes += [[r] for r in rotation_passes(probe.nh, positions[0])]
                 for heavy in passes:
-                    plants = [P.profile('heavy', q, p, gen, heavy=hv) for q, p, hv in zip(probe.q_rot, positions, heavy)]
+                    plants = [P.profile('heavy', q, p, gen, heavy=hv, g=probe.g) for q, p, hv in zip(probe.q_rot, positions, heavy)]
                     bounded(probe, toks, positions, plants, worst[kind], what + ' heavy')
             else:
-                plants = [P.profile(kind, q, p, gen) for q, p in zip(probe.q_rot, positions)]
+                plants = [P.profile(kind, q, p, gen, g=probe.g) for q, p in zip(probe.q_rot, positions)]
                 bounded(probe, toks, positions, plants, worst[kind], f'{what} {kind}')
 
 
@@ -114,19 +118,36 @@ def run_sweeps(probe, name, position_sets, profiles=P.PROFILES, **kw):
         w.done()
 
 
+def label(probe, size):
+    """The shape's name in the printed sweeps, with its query and K/V head counts when they differ."""
+    return size if probe.nkv == probe.nh else f'{size} ({probe.nh} / {probe.nkv} K/V heads)'
+
+
 # ----------------------------------------------------------------------------- batch 1, every position of a 600-key cache
+def every_position(probe, name, seed):
+    """Every position 0..599 at batch 1: heavy keys at every position (rotating over the edges), one more profile in turn."""
+    gen = torch.Generator(device='cuda:0').manual_seed(seed)
+    worst = {k: Worst(f'{name} {k}') for k in P.PROFILES}
+    rope = Worst(f'{name} appended K row vs fp64 RoPE')
+    for i in range(600):
+        sweep(probe, [[i]], ('heavy', P.PROFILES[1 + i % 6]), gen, worst, rope, tok0=i, rotate_heavy=True)
+    for w in list(worst.values()) + [rope]:
+        w.done()
+
+
 def test_chain_tiny_every_position():
     """Kernel chain (tiny: intermediate 704 keeps it off the persistent path): 256-key splits and the combine, every position 0..599."""
     probe = P.Probe('tiny', max_seq=600)
     assert not probe.persistent and probe.dec.launches_per_step() > 1
-    sets = [[p] for p in range(600)]
-    gen = torch.Generator(device='cuda:0').manual_seed(7)
-    worst = {k: Worst(f'chain tiny {k}') for k in P.PROFILES}
-    rope = Worst('chain tiny appended K row vs fp64 RoPE')
-    for i, s in enumerate(sets):  # heavy keys at every position (rotating over the edges), one more profile in turn
-        sweep(probe, [s], ('heavy', P.PROFILES[1 + i % 6]), gen, worst, rope, tok0=i, rotate_heavy=True)
-    for w in list(worst.values()) + [rope]:
-        w.done()
+    every_position(probe, 'chain tiny', 7)
+
+
+def test_chain_tiny_gqa1_every_position():
+    """The kernel chain with one K/V head for 4 query heads (tiny-gqa1-chain): the 4 CTAs of every 256-key split read the same K/V head and
+    the first of them stores the new row, every position 0..599."""
+    probe = P.Probe('tiny-gqa1-chain', max_seq=600)
+    assert not probe.persistent and probe.dec.launches_per_step() > 1 and probe.nkv == 1
+    every_position(probe, f'chain {label(probe, "tiny-gqa1-chain")}', 17)
 
 
 def test_persistent_tiny256_every_position():
@@ -134,17 +155,21 @@ def test_persistent_tiny256_every_position():
     probe = P.Probe('tiny256', max_seq=600)
     assert probe.persistent
     assert probe.nb // probe.nh + 1 > 12, 'the fast merge would serve this shape'
-    gen = torch.Generator(device='cuda:0').manual_seed(8)
-    worst = {k: Worst(f'persistent tiny256 {k}') for k in P.PROFILES}
-    rope = Worst('persistent tiny256 appended K row vs fp64 RoPE')
-    for i in range(600):
-        sweep(probe, [[i]], ('heavy', P.PROFILES[1 + i % 6]), gen, worst, rope, tok0=i, rotate_heavy=True)
-    for w in list(worst.values()) + [rope]:
-        w.done()
+    every_position(probe, 'persistent tiny256', 8)
+
+
+def test_persistent_tiny_gqa2_every_position():
+    """Persistent kernel at tiny-gqa2 (4 query heads on 2 K/V heads, 66 teams per query head): the general record merge over teams that
+    share a K/V head, every team owning the new key's unit patching its own stage, every position 0..599."""
+    probe = P.Probe('tiny-gqa2', max_seq=600)
+    assert probe.persistent and probe.nkv == 2
+    assert probe.nb // probe.nh + 1 > 12, 'the fast merge would serve this shape'
+    every_position(probe, f'persistent {label(probe, "tiny-gqa2")}', 18)
 
 
 # ----------------------------------------------------------------------------- batch 1 at the 7B and 13B shapes
 POS_7B = [0, 1, 31, 32, 33, 255, 256, 257, 511, 512, 1023, 1024, 2015, 2016, 2046, 2047]
+LLAMA2_EDGES = [0, 1, 31, 32, 33, 255, 256, 257, 1023, 1024, 2047, 2048, 2049, 4063, 4064, 4094, 4095]  # max_seq 4096
 
 
 def test_persistent_7b_positions():
@@ -160,8 +185,7 @@ def test_persistent_7b_llama2_context():
     """LLaMA-2-7B context (max_seq 4096): the unit, split and team edges, both sides of 2048 and the last position 4095."""
     probe = P.Probe('7b', max_seq=4096)
     assert probe.persistent
-    edges = {0, 1, 31, 32, 33, 255, 256, 257, 1023, 1024, 2047, 2048, 2049, 4063, 4064, 4094, 4095}
-    positions = sorted(edges | set(P.team_edge_positions(probe.nh, probe.nb)))
+    positions = sorted(set(LLAMA2_EDGES) | set(P.team_edge_positions(probe.nh, probe.nb)))
     run_sweeps(probe, '7b max_seq 4096', [[p] for p in positions])
 
 
@@ -181,12 +205,38 @@ def test_persistent_7b_last_unit_past_the_slot():
     run_sweeps(probe, '7b max_seq 2000', [[1999], [1998], [1984]])
 
 
+def test_persistent_llama3_8b_positions():
+    """LLaMA-3-8B (32 query heads on 8 K/V heads, RoPE base 5e5; 8 or 9 teams per query head: the fast merge): the edges of
+    test_persistent_7b_positions, each K/V head streamed by the teams of its 4 query heads; at 2047 every key is heavy once."""
+    probe = P.Probe('llama3-8b', max_seq=2048, rope_base=5e5)
+    assert probe.persistent and probe.nkv == 8
+    assert probe.nb // probe.nh + 1 <= 12, 'the general merge would serve this shape'
+    positions = sorted(set(POS_7B) | set(P.team_edge_positions(probe.nh, probe.nb)))
+    run_sweeps(probe, f'{label(probe, "llama3-8b")} base 5e5', [[p] for p in positions], full_rotation=(2047, ))
+
+
+def test_persistent_llama3_8b_last_unit_past_the_slot():
+    """LLaMA-3-8B at max_seq 2000: the last 32-key unit at pos 1999 reaches past the end of its K/V head's slot (16 rows are fetched), next to
+    the rows of the following K/V head, which must not enter the softmax."""
+    probe = P.Probe('llama3-8b', max_seq=2000, rope_base=5e5)
+    assert probe.persistent and probe.nkv == 8
+    run_sweeps(probe, f'{label(probe, "llama3-8b")} max_seq 2000', [[1999], [1998], [1984]])
+
+
 def test_persistent_13b_act_order():
     """LLaMA-13B shapes with act-order layers: the qkv input gather (qkv_perm) and o_perm, whose staging takes the general merge path."""
     probe = P.Probe('13b', max_seq=2048, act_order=True)
     assert probe.persistent
     assert probe.dec.perms[0]['qkv'] is not None and probe.dec.perms[0]['o'] is not None
     run_sweeps(probe, '13b act-order', [[0], [1], [32], [257], [1023], [2047]])
+
+
+def test_persistent_70b_act_order():
+    """LLaMA-2-70B shapes with act-order layers: the qkv input gather (qkv_perm) at the grouped-query width (64 + 2 x 8 heads of 128)."""
+    probe = P.Probe('70b', max_seq=2048, act_order=True)
+    assert probe.persistent and probe.nkv == 8
+    assert probe.dec.perms[0]['qkv'] is not None and probe.dec.perms[0]['o'] is not None
+    run_sweeps(probe, f'{label(probe, "70b")} act-order', [[0], [1], [32], [257], [1023], [2047]])
 
 
 # ----------------------------------------------------------------------------- batches
@@ -204,13 +254,20 @@ def test_persistent_7b_batched(batch, position_sets, max_seq):
     run_sweeps(probe, f'7b batch {batch} max_seq {max_seq}', position_sets)
 
 
-@pytest.mark.parametrize('batch,position_sets', [(2, [[599, 0], [300, 301], [37, 599], [0, 0]]), (3, [[599, 1, 256], [0, 0, 0]])])
-def test_persistent_tiny256_batched(batch, position_sets):
-    """tiny256 batches: tens of teams per (sequence, head), so merge_records takes several rounds of 12 records (the w0 rescale)."""
-    probe = P.Probe('tiny256', batch=batch, max_seq=600)
+TINY_BATCHES = [(2, [[599, 0], [300, 301], [37, 599], [0, 0]]), (3, [[599, 1, 256], [0, 0, 0]])]
+
+
+@pytest.mark.parametrize('size,batch,position_sets', [pytest.param('tiny256', *TINY_BATCHES[0], id='2-position_sets0'),
+                                                      pytest.param('tiny256', *TINY_BATCHES[1], id='3-position_sets1'),
+                                                      pytest.param('tiny-gqa2', *TINY_BATCHES[0], id='tiny-gqa2-2'),
+                                                      pytest.param('tiny-gqa2', *TINY_BATCHES[1], id='tiny-gqa2-3')])
+def test_persistent_tiny256_batched(size, batch, position_sets):
+    """tiny256 batches, and the same at tiny-gqa2 (4 query heads on 2 K/V heads): tens of teams per (sequence, head), so merge_records takes
+    several rounds of 12 records (the w0 rescale)."""
+    probe = P.Probe(size, batch=batch, max_seq=600)
     assert probe.persistent
     assert max(P.seq_teams(position_sets[0], probe.nh, probe.nb, s)[1] for s in range(batch)) // probe.nh > 12
-    run_sweeps(probe, f'tiny256 batch {batch}', position_sets)
+    run_sweeps(probe, f'{label(probe, size)} batch {batch}', position_sets)
 
 
 def test_persistent_13b_batch6():
@@ -249,39 +306,69 @@ def max_persistent_batch(size):
     return min(8, 2 * torch.cuda.get_device_properties(0).multi_processor_count // nh)
 
 
-@pytest.mark.parametrize('size', ['65b', '33b'])
+LARGE_CONTEXTS = {  # max_seq, RoPE base, positions (besides the team edges), the position at which every key is heavy once
+    '65b': (2048, 10000.0, POS_7B, 2047),
+    '33b': (2048, 10000.0, POS_7B, None),
+    '70b': (4096, 10000.0, LLAMA2_EDGES, 4095),
+    '34b': (16384, 1e6, [0, 1, 8191, 8192, 16383], 16383),
+}
+
+
+@pytest.mark.parametrize('size', ['65b', '33b', '70b', '34b'])
 def test_persistent_large_positions(size):
     """LLaMA-65B (64 heads, 4 or 5 teams per head on 132 SMs) and LLaMA-33B (52 heads, 5 or 6) at batch 1: the unit, split and team edges
-    of POS_7B and of this shape's team partition; at 65B every key of the 2047-key context is heavy once."""
-    probe = P.Probe(size, max_seq=2048)
+    of POS_7B and of this shape's team partition; at 65B every key of the 2047-key context is heavy once.  LLaMA-2-70B (64 query heads on 8
+    K/V heads) at its 4096 context and CodeLlama-34B (the same heads, RoPE base 1e6) at 16384: the 8 query heads of a group read one K/V
+    head through 4 or 5 teams each; every key of the longest context is heavy once."""
+    max_seq, base, edges, rotation = LARGE_CONTEXTS[size]
+    probe = P.Probe(size, max_seq=max_seq, rope_base=base)
     assert probe.persistent and probe.dec.launches_per_step() == 1
     assert probe.nb // probe.nh + 1 <= 12, 'the general merge would serve this shape'
-    positions = sorted(set(POS_7B) | set(P.team_edge_positions(probe.nh, probe.nb)))
-    run_sweeps(probe, size, [[p] for p in positions], full_rotation=(2047, ) if size == '65b' else ())
+    positions = sorted(set(edges) | set(P.team_edge_positions(probe.nh, probe.nb)))
+    name = label(probe, size) if max_seq == 2048 else f'{label(probe, size)} max_seq {max_seq} base {base:g}'
+    run_sweeps(probe, name, [[p] for p in positions], full_rotation=(rotation, ) if rotation else ())
 
 
 def _ragged(B):
     return [[2047, 0, 255, 256, 1023, 31, 32, 1500][:B], [0] * B]
 
 
-@pytest.mark.parametrize('size', ['65b', '33b'])
+@pytest.mark.parametrize('size', ['65b', '33b', '70b', 'llama3-8b'])
 def test_persistent_large_largest_batch(size):
-    """The largest batch the persistent plan takes at 65B / 33B (4 / 5 sequences on 132 SMs): every team serves one (sequence, head) pair or
-    a share of one; ragged positions and every sequence at position 0."""
+    """The largest batch the persistent plan takes at 65B / 33B / 70B / LLaMA-3-8B (4 / 5 / 4 / 8 sequences on 132 SMs): every team serves one
+    (sequence, query head) pair or a share of one (256 of the 264 teams at LLaMA-3-8B); ragged positions and every sequence at position 0."""
     B = max_persistent_batch(size)
     probe = P.Probe(size, batch=B, max_seq=2048)
     assert probe.persistent and probe.dec.launches_per_step() == 1, f'{size} batch {B}'
-    run_sweeps(probe, f'{size} batch {B}', _ragged(B))
+    run_sweeps(probe, f'{label(probe, size)} batch {B}', _ragged(B))
 
 
-@pytest.mark.parametrize('size', ['65b', '33b'])
+@pytest.mark.parametrize('size', ['65b', '33b', '70b'])
 def test_chain_large_above_the_plan(size):
-    """One sequence more than the persistent plan takes at 65B / 33B: the kernel chain serves the batch."""
+    """One sequence more than the persistent plan takes at 65B / 33B / 70B: the kernel chain serves the batch."""
     B = max_persistent_batch(size) + 1
     assert B <= 8
     probe = P.Probe(size, batch=B, max_seq=1024)
     assert not probe.persistent and probe.dec.launches_per_step() > 1, f'{size} batch {B}'
-    run_sweeps(probe, f'chain {size} batch {B}', [[1023, 0, 1, 255, 256, 511, 800, 31][:B], [0] * B])
+    run_sweeps(probe, f'chain {label(probe, size)} batch {B}', [[1023, 0, 1, 255, 256, 511, 800, 31][:B], [0] * B])
+
+
+def test_chain_70b_batch8_llama2_context():
+    """LLaMA-2-70B at batch 8 on the kernel chain, the engine that serves it (8 x 64 (sequence, query head) pairs exceed the persistent
+    kernel's teams), at its 4096 context: 16 splits of 256 keys per query head, the 8 query heads of a group on one K/V head."""
+    probe = P.Probe('70b', batch=8, max_seq=4096)
+    assert not probe.persistent and probe.dec.launches_per_step() > 1 and probe.nkv == 8
+    run_sweeps(probe, f'chain {label(probe, "70b")} batch 8 max_seq 4096', [[4095, 0, 1, 2047, 2048, 3839, 3840, 255], [0] * 8])
+
+
+@pytest.mark.parametrize('size,batch', [('7b', 1), ('7b', 8), ('tiny', 1), ('tiny', 8)])
+def test_one_kv_head(size, batch):
+    """One K/V head for every query head: at 7B (g = 32, each q on 2 of the 64 pairs) every team of the persistent kernel streams the same
+    K/V head; tiny (g = 2) runs on the kernel chain."""
+    probe = P.Probe(size, batch=batch, max_seq=2048, n_kv_heads=1)
+    assert probe.persistent == (size == '7b') and (probe.dec.launches_per_step() == 1) == probe.persistent
+    sets = [[p] for p in (0, 1, 31, 32, 255, 256, 1024, 2016, 2047)] if batch == 1 else [[0, 31, 32, 255, 256, 1023, 2046, 2047], [0] * 8]
+    run_sweeps(probe, f'{"persistent" if probe.persistent else "chain"} {label(probe, size)} batch {batch}', sets)
 
 
 # ----------------------------------------------------------------------------- lm_head and greedy token
@@ -290,6 +377,8 @@ def test_chain_large_above_the_plan(size):
     ('7b', 8, 32001, [1001, 1002, 32000], True),
     ('tiny', 1, 600, [7, 8, 599], False),
     ('tiny', 3, 600, [7, 8, 599], False),
+    ('llama3-8b', 1, 128256, [1001, 1002, 128255], True),
+    ('llama3-8b', 8, 128256, [1001, 1002, 128255], True),
 ])
 def test_lm_head_and_greedy_token(size, batch, vocab, dups, persistent):
     lm_head_and_greedy_token(size, batch, vocab, dups, persistent)
@@ -319,9 +408,9 @@ def lm_head_and_greedy_token(size, batch, vocab, dups, persistent):
     toks = [(977 * b + 5) % vocab for b in range(batch)]
     positions = [0] * batch
     probe.learn(toks, positions)
-    empty = torch.zeros(probe.nh, 0, P.HD, dtype=torch.float16, device='cuda:0')
+    empty = torch.zeros(probe.nkv, 0, P.HD, dtype=torch.float16, device='cuda:0')
     x_in, x_out = probe.run(toks, positions, [(empty, empty)] * batch)
-    want = (x_in.double() + torch.stack([v.reshape(-1) for v in probe.v_new]).double()).half()
+    want = (x_in.double() + torch.stack([v.repeat_interleave(probe.g, 0).reshape(-1) for v in probe.v_new]).double()).half()
     assert torch.equal(x_out, want)
     f = np.float32
     x = x_out.float().cpu().numpy()
