@@ -7,7 +7,8 @@
   a multiple of 2^-10 of magnitude <= 16 * 2^-6, every product a multiple of 2^-10 of magnitude <= 0.5, so at K <= 16384
   every partial sum is a multiple of 2^-10 below 2^13: under 2^23 units, exact in fp32 in any order.  out = fp16(exact sum).
 
-Also the stream-K plan of the split-K matvec (qmatvec.cu: plan_skinny and the CTA unit ranges), restated for error reports.
+Also the stream-K plan of the split-K matvec (qmatvec.cu: plan_skinny and the CTA unit ranges), restated for error reports, and
+which products the matvec takes at all (skinny_supported), restated for the tests' expected routes.
 """
 import math
 
@@ -85,6 +86,26 @@ def matvec_plan(K: int, N: int):
     nslabs, nk = -(-N // SLAB), K // STEP
     U = nslabs * nk
     return nslabs, nk, U, min(U, 2 * NUM_SMS)
+
+
+MATVEC_RING_BYTES = 8 * 8192  # 8 warps x an 8 KB weight ring each
+MATVEC_SMEM_LIMIT = 110 * 1024  # two CTAs per SM
+
+
+def matvec_smem_bytes(M: int, K: int, N: int) -> int:
+    """The shared memory skinny_supported budgets: the weight rings plus M rows of the CTA's x segment, seg_steps = ceil(U / grid)
+    k-steps of 32 (at most nk) and one step more for the bank-spreading pitch."""
+    _, nk, U, nb = matvec_plan(K, N)
+    seg_steps = min(nk, -(-U // nb))
+    return MATVEC_RING_BYTES + M * (seg_steps * 32 + 32) * 2
+
+
+def matvec_takes(M: int, K: int, N: int) -> bool:
+    """Whether the split-K matvec serves an int4 product of M rows at (K, N), groupsize a multiple of 32 and aligned operands
+    (qmatvec.cu skinny_supported); otherwise the generic kernel does, and the kernel chain runs the RMSNorm and the residual add as
+    kernels of their own around it."""
+    _, _, U, _ = matvec_plan(K, N)
+    return 1 <= M <= 8 and K % 32 == 0 and U * (2 * NUM_SMS + 1) < 2**31 and matvec_smem_bytes(M, K, N) <= MATVEC_SMEM_LIMIT
 
 
 def matvec_cta(K: int, N: int, k: int, n: int):

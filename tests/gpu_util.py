@@ -296,23 +296,36 @@ def tiny_quant_llama(bits=4, gs=32, act=False, hidden=128, intermediate=352, hea
 # ----------------------------------------------------------------------------- lm_head + log-softmax (gptq_lm_head_logprob)
 U = 2.0**-24
 # fp32 part of the bound (everything after the fp16 logits).  The row's sum s = sum exp(l - max) is formed by 31 sequential adds per
-# thread, 2 quad shuffles, at most 8 per-lane merges (ceil(251 / 32) vocabulary tiles) and 5 butterfly merges, each merge 2 expf (2 ulp),
-# 2 multiplies and 1 add; with 2 ulp for the terms' expf that is <= 31 + 2 + 13 * 6 + 2 = 113 roundings of relative size 2^-24, so
-# |log s' - log s| <= 128 * 2^-24 = 7.6e-6.  The exp arguments l - max are rounded relative to their size; weighted by exp(-a) that adds at
-# most (log V + 1) 2^-24, and logf, max + log s and l_t - (...) round relative to their magnitudes: 2^-23 (|max l| + log V + |logprob|).
+# thread, 2 quad shuffles, ceil(ntiles / 32) per-lane merges of the ntiles = ceil(V / 128) vocabulary tiles and 5 butterfly merges, each
+# merge 2 expf (2 ulp), 2 multiplies and 1 add; with 2 ulp for the terms' expf that is 31 + 2 + (merges + 5) * 6 + 2 roundings of relative
+# size 2^-24: 113 at V = 32000 (8 merges), 257 at LLaMA-3's 128256 (1002 tiles, 32 merges), so |log s' - log s| <= max(128, that) 2^-24.
+# The exp arguments l - max are rounded relative to their size; weighted by exp(-a) that adds at most (log V + 1) 2^-24, and logf,
+# max + log s and l_t - (...) round relative to their magnitudes: 2^-23 (|max l| + log V + |logprob|).
 LSE_EPS = 128 * U
 
 
+def lse_roundings(V):
+    """Roundings of relative size 2^-24 in a row's sum of exponentials (above)."""
+    merges = -(-(-(-V // 128)) // 32)
+    return 31 + 2 + (merges + 5) * 6 + 2
+
+
 def lse_tol(lmax, V, ref):
-    return LSE_EPS + 2 * U * (lmax + math.log(V) + ref.abs())
+    return max(LSE_EPS, lse_roundings(V) * U) + 2 * U * (lmax + math.log(V) + ref.abs())
 
 
-def ref_logprob(x, W, targets):
-    """float64 log-softmax of the fp16 logits fp16(x . W^T), on the GPU.  (CUDA's float64 -> fp16 cast goes through fp32, which can move a
-    logit by one fp16 ulp at a tie: the per-logit ulp terms of the bound cover it; on the integer grid every logit is exact.)"""
-    l = (x.double() @ W.double().t()).half().double()
-    lt = l.gather(1, targets.long()[:, None])[:, 0]
-    return lt - torch.logsumexp(l, -1), lt, l.abs().amax(-1)
+def ref_logprob(x, W, targets, rows=2048):
+    """float64 log-softmax of the fp16 logits fp16(x . W^T), on the GPU, `rows` rows at a time (an 8191 x 128256 float64 logit matrix
+    alone is 8.4 GB).  (CUDA's float64 -> fp16 cast goes through fp32, which can move a logit by one fp16 ulp at a tie: the per-logit ulp
+    terms of the bound cover it; on the integer grid every logit is exact.)"""
+    W64 = W.double().t()
+    out = []
+    for r in range(0, x.shape[0], rows):
+        l = (x[r:r + rows].double() @ W64).half().double()
+        lt = l.gather(1, targets[r:r + rows].long()[:, None])[:, 0]
+        out.append((lt - torch.logsumexp(l, -1), lt, l.abs().amax(-1)))
+        del l
+    return tuple(torch.cat(t) for t in zip(*out))
 
 
 def check_logprob(lp, x, W, targets, what, exact=False):
@@ -369,6 +382,17 @@ def make_kv_cache(B, nh, S, spans, seed=0, layers=3, layer=1, poison=True):
         k[:, heavy] += 4 * u
         kc[layer, b, :, :L] = k.half()
         vc[layer, b, :, :L] = torch.randn(nh, L, HD, device='cuda', generator=g).half()
+    return q, kc, vc
+
+
+def make_gqa_kv_cache(B, nh, nkv, S, spans, seed=0, layers=3, layer=1):
+    """make_kv_cache with q rows of nh query heads over a cache of nkv K/V heads: q is drawn right after the heavy-key direction u, before
+    the cache, so both draws of one seed share u.  Compare against the reference with each K/V head repeated nh / nkv times."""
+    if nkv == nh:
+        return make_kv_cache(B, nh, S, spans, seed=seed, layers=layers, layer=layer)
+    q = make_kv_cache(B, nh, S, spans, seed=seed, layers=1, layer=0)[0]
+    torch.cuda.empty_cache()
+    _, kc, vc = make_kv_cache(B, nkv, S, spans, seed=seed, layers=layers, layer=layer)
     return q, kc, vc
 
 

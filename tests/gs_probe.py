@@ -4,7 +4,8 @@ engines (persistent kernel and kernel chain).  CPU-only: the GPU tests pack the 
 * Inputs.  Embedding rows of +-2^-4 (+2^-4 on features [0, POS_FEATS)), rms_eps = 0, unit norm weights: both RMSNorms give exactly +-1.
 * Fields.  Every (group, column) has its own zero z in [1, 2^bits - 2] and power-of-two scale 2^-j, and adjacent groups differ in both.
   A weight either sits at its own group's zero (it adds exactly 0 -- with the right group only) or is a tap, q != z.
-    qkv   q and k columns dense (every weight a tap), j in [6, 10]; v columns one tap each, j in [5, 7] (|v| <= 15/32, a multiple of 2^-7)
+    qkv   q and k columns dense (every weight a tap), j in [6, 10]; v columns one tap each, j in [5, 7] (|v| <= 15/32, a multiple of 2^-7);
+          H q columns, then Hkv = n_kv_heads * 128 k and Hkv v columns (grouped-query attention: Hkv < H)
     o     dense, j in [6, 8]
     gate  one tap per column on a feature k < POS_FEATS (x_k = +1), q = 2^bits - 1 and the tap group's scale 2^e chosen so that
           a = (q - z) 2^e lies in [20, 40)
@@ -20,7 +21,8 @@ engines (persistent kernel and kernel chain).  CPU-only: the GPU tests pack the 
 
 Where each linear is read after one step at position 0 (RoPE is the identity there and attention over the one key returns v_new):
     qkv              the appended K and V rows of the cache (exact(...).k / .v)
-    o_proj           x after attention = fp16(x_in + fp16(o(v_new))), with gate/up/down scales 0 (the MLP adds exactly 0)
+    o_proj           x after attention = fp16(x_in + fp16(o(v_new))), with gate/up/down scales 0 (the MLP adds exactly 0); query head h
+                     reads the V row of K/V head h // g (g = n_heads / n_kv_heads), so o_proj's input repeats each K/V head g times
     gate/up -> down  x after the layer = fp16(x_in + fp16(down(h))), with o_proj scales 0 (x after attention is x_in)
 """
 import math
@@ -30,8 +32,10 @@ import torch
 from gpu_util import fp16_from_fp64
 from oracle import gptq_oracle as O
 
-# hidden, intermediate, heads (engine.LLAMA_SHAPES)
-SHAPES = {'7b': (4096, 11008, 32), '13b': (5120, 13824, 40), '33b': (6656, 17920, 52), '65b': (8192, 22016, 64)}
+# hidden, intermediate, heads, K/V heads (engine.LLAMA_SHAPES, engine.kv_heads)
+SHAPES = {'7b': (4096, 11008, 32, 32), '13b': (5120, 13824, 40, 40), '33b': (6656, 17920, 52, 52), '65b': (8192, 22016, 64, 64),
+          '70b': (8192, 28672, 64, 8), '34b': (8192, 22016, 64, 8), 'llama3-8b': (4096, 14336, 32, 8)}
+HEAD_DIM = 128
 POS_FEATS = 64  # every embedding row is +2^-4 on these features: the gate taps read x = +1
 STAGE_K = 128   # k per stage of the persistent kernel (4 k-steps of 32), inside one group
 STEP_K = 32
@@ -111,14 +115,16 @@ class ProbeLayer:
     """The probe's fields for one model size and groupsize (gs: an int or 'full' = each linear's K, the reference's --groupsize -1)."""
 
     def __init__(self, size, gs, bits=4, act_order=False, seed=0):
-        H, I, nh = SHAPES[size]
-        self.size, self.H, self.I, self.nh, self.bits, self.act_order = size, H, I, nh, bits, act_order
+        H, I, nh, nkv = SHAPES[size]
+        self.size, self.H, self.I, self.nh, self.nkv, self.bits, self.act_order = size, H, I, nh, nkv, bits, act_order
+        self.Hkv = nkv * HEAD_DIM  # the width of the k and of the v columns of qkv
         self.gs = gs
         gen = torch.Generator().manual_seed(seed)
         gh, gi = group_size(gs, H), group_size(gs, I)
         g_h = O.make_g_idx(H, gh, act_order, gen).long()
-        self.qkv = Linear.cat([Linear.random(H, 2 * H, gh, bits, gen, 6, 10, g_h),
-                               Linear.random(H, H, gh, bits, gen, 5, 7, g_h, tap_ks=torch.randint(0, H, (H, ), generator=gen))])
+        Hkv = self.Hkv  # (with one K/V head per query head, Hkv = H and every draw is the multi-head probe's)
+        self.qkv = Linear.cat([Linear.random(H, H + Hkv, gh, bits, gen, 6, 10, g_h),
+                               Linear.random(H, Hkv, gh, bits, gen, 5, 7, g_h, tap_ks=torch.randint(0, H, (Hkv, ), generator=gen))])
         self.o = Linear.random(H, H, gh, bits, gen, 6, 8, O.make_g_idx(H, gh, act_order, gen).long())
         g_mlp = O.make_g_idx(H, gh, act_order, gen).long()  # gate and up share their input, hence their act-order map
         self.gate = Linear.random(H, I, gh, bits, gen, 5, 7, g_mlp, tap_ks=torch.randint(0, POS_FEATS, (I, ), generator=gen))
@@ -152,6 +158,14 @@ def product(x, lin, device, cols=4096):
     return torch.cat([x @ lin.weight(slice(c, c + cols), device=device) for c in range(0, lin.N, cols)], 1)
 
 
+def attention_out(v, nh, kv_head=None):
+    """The o_proj input at position 0 from the appended V rows v [B, nkv * 128]: query head h attends to its K/V head's one key, so its
+    output is that head's v row.  kv_head(h, nkv) names the K/V head (h // g, g = nh / nkv; the teeth try a wrong one)."""
+    B, nkv = v.shape[0], v.shape[1] // HEAD_DIM
+    heads = [h // (nh // nkv) if kv_head is None else kv_head(h, nkv) for h in range(nh)]
+    return v.view(B, nkv, HEAD_DIM)[:, torch.tensor(heads, device=v.device)].reshape(B, nh * HEAD_DIM)
+
+
 class Expect:
     """The exact outputs of one step at position 0 for input rows x_in [B, H] (fp16 embedding rows), all float64 / fp16 on `device`."""
 
@@ -159,10 +173,11 @@ class Expect:
         L = layer
         self.x_in = x_in.to(device)
         self.x = self.x_in.double() * 16  # RMSNorm output, exactly +-1
-        H = L.H
+        H, Hkv = L.H, L.Hkv
         self.qkv64 = product(self.x, L.qkv, device)
-        self.k, self.v = fp16(self.qkv64[:, H:2 * H]), fp16(self.qkv64[:, 2 * H:])
-        self.o64 = product(self.v.double(), L.o, device)
+        self.k, self.v = fp16(self.qkv64[:, H:H + Hkv]), fp16(self.qkv64[:, H + Hkv:])
+        self.o_in = attention_out(self.v, L.nh)
+        self.o64 = product(self.o_in.double(), L.o, device)
         self.x_attn = fp16(self.x_in.double() + fp16(self.o64).double())  # o-probe: MLP scales 0
         self.a = product(self.x, L.gate, device)
         self.b = product(self.x, L.up, device)
@@ -176,7 +191,8 @@ def input_bounds(L):
     """{linear: (xmax [K] float64, grid gx)}: the largest |input| per feature over every token and the grid the inputs lie on."""
     H = L.H
     one = torch.ones(H, dtype=torch.float64)
-    vtap = L.qkv.taps_abs()[:, 2 * H:].max(0).values  # |v_n| <= its single tap's |q - z| 2^-j, on the grid 2^-7
+    vtap = L.qkv.taps_abs()[:, H + L.Hkv:].max(0).values  # |v_n| <= its single tap's |q - z| 2^-j, on the grid 2^-7
+    vtap = attention_out(vtap[None], L.nh)[0]  # o_proj's input feature of query head h is a feature of K/V head h // g
     gate_a = L.gate.weight().max(0).values  # the gate's one tap: a_n for x = +1
     up_b = L.up.taps_abs().max(0).values
     # h = fp16(a b): a is even, b a multiple of 2^-7, and the fp16 rounding moves |h| up by at most 2^-11 relative
@@ -233,7 +249,8 @@ def teeth(L, x_in, cols=1024):
     E = Expect(L, x_in)
     X1 = E.x
     res = {}
-    # K row of qkv: fp16 of the k columns
+    # K row of qkv: fp16 of the k columns (cols <= the K/V width of every shape)
+    assert cols <= L.Hkv
     kl = Linear(L.qkv.q[:, H:H + cols], L.qkv.z[:, H:H + cols], L.qkv.j[:, H:H + cols], L.qkv.g_idx, L.qkv.gs, L.bits)
     out, bad = corruptions(kl, X1)
     for name, o2 in bad.items():
@@ -242,7 +259,9 @@ def teeth(L, x_in, cols=1024):
     ol = Linear(L.o.q[:, :cols], L.o.z[:, :cols], L.o.j[:, :cols], L.o.g_idx, L.o.gs, L.bits)
     xin = E.x_in.double()[:, :cols]
     obs = lambda o: fp16(xin + fp16(o).double())
-    out, bad = corruptions(ol, E.v.double())
+    out, bad = corruptions(ol, E.o_in.double())
+    if L.nkv < L.nh:  # each query head reading K/V head h % nkv, not h // g
+        bad['K/V head h % nkv'] = attention_out(E.v, L.nh, kv_head=lambda h, nkv: h % nkv).double() @ ol.weight()
     for name, o2 in bad.items():
         res[('o', name)] = (int((obs(o2) != obs(out)).sum()), out.numel())
     dl = Linear(L.down.q[:, :cols], L.down.z[:, :cols], L.down.j[:, :cols], L.down.g_idx, L.down.gs, L.bits)
@@ -261,6 +280,16 @@ CASES += [('13b', 32, 3, True, 1, 'persistent'), ('13b', 32, 4, False, 7, 'chain
 CASES += [('65b', 128, 4, False, 1, 'persistent'), ('65b', 128, 4, False, 'max', 'persistent'), ('65b', 128, 4, False, 'max+1', 'chain'),
           ('65b', 1024, 4, False, 1, 'persistent'), ('65b', 128, 4, True, 1, 'persistent'),
           ('33b', 1024, 4, False, 1, 'persistent'), ('33b', 1024, 4, False, 'max', 'persistent'), ('33b', 'full', 4, False, 'max+1', 'chain')]
+# Grouped-query shapes.  LLaMA-2-70B (64 / 8 heads, qkv 8192 -> 10240): gs 128 at batch 1 and 'max' (persistent) and at 'max+1' (the
+# chain, every linear on the split-K matvec); at batch 8 and, gs 1024, batch 7 the chain runs gate|up and down_proj (8192 <-> 28672) on the
+# generic kernel (exact_fixtures.matvec_takes); int4 act-order gs 128 takes the persistent kernel's gathers at qkv width 10240.
+# CodeLlama-34B gs 1024: down_proj (K = 22016) ends in a partial group of 512; batch 8 is on the chain, all on the matvec.
+# LLaMA-3-8B (32 / 8 heads, qkv 4096 -> 6144): gs 128 at batch 1 and 8 (persistent), gs full (down_proj K = 14336) at batch 1.
+CASES += [('70b', 128, 4, False, 1, 'persistent'), ('70b', 128, 4, False, 'max', 'persistent'), ('70b', 128, 4, False, 'max+1', 'chain'),
+          ('70b', 128, 4, False, 8, 'chain'), ('70b', 1024, 4, False, 7, 'chain'), ('70b', 128, 4, True, 1, 'persistent'),
+          ('34b', 1024, 4, False, 1, 'persistent'), ('34b', 1024, 4, False, 8, 'chain'),
+          ('llama3-8b', 128, 4, False, 1, 'persistent'), ('llama3-8b', 128, 4, False, 8, 'persistent'),
+          ('llama3-8b', 'full', 4, False, 1, 'persistent')]
 VOCAB = 64
 
 
@@ -280,11 +309,22 @@ def resolve_batch(B, n_heads, sms):
     return B
 
 
+def chain_launches(L, B):
+    """Launches of one kernel-chain step of the one-layer probe model: embed, attention, combine, lm_head and argmax, and per quantized
+    linear 1 where the split-K matvec serves it whole, else the generic kernel plus the RMSNorm (qkv, gate|up) or the residual add (o_proj,
+    down_proj) as kernels of their own (decode.cu ChainLinear::launches)."""
+    from exact_fixtures import matvec_takes
+    n = 5
+    for K, N in ((L.H, L.H + 2 * L.Hkv), (L.H, L.H), (L.H, L.I), (L.I, L.H)):
+        n += 1 if matvec_takes(B, K, N) else 2
+    return n
+
+
 def tokens(B):
     return [(7 * b + 3) % VOCAB for b in range(B)]
 
 
 def layer_for(size, gs, bits, act_order):
     """The probe layer of a case (a fixed seed per configuration, so the CPU and GPU tests see the same fields)."""
-    seed = {'7b': 1, '13b': 2, '33b': 3, '65b': 4}[size] * 100000 + (0 if gs == 'full' else gs) * 10 + bits + 5 * int(act_order)
+    seed = {'7b': 1, '13b': 2, '33b': 3, '65b': 4, '70b': 5, '34b': 6, 'llama3-8b': 7}[size] * 100000 + (0 if gs == 'full' else gs) * 10 + bits + 5 * int(act_order)
     return ProbeLayer(size, gs, bits, act_order, seed)

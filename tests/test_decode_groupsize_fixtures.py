@@ -5,7 +5,8 @@
   stay above the fp16 subnormal grid after the 1/16 pre-scaling of the odd nibbles.
 * Teeth: a kernel that read the neighbouring group's scale or zero for one stage, took another sequence's sum of x, or dropped or repeated
   one k-step would produce an observed output (K row, x after attention, x after the layer) that differs from the anchor in many
-  elements, at every groupsize, the partial last group of down_proj at 1024 included, and at the 65B and 33B probe layers.
+  elements, at every groupsize, the partial last group of down_proj at 1024 included, and at the 65B, 33B, LLaMA-2-70B and LLaMA-3-8B
+  probe layers.  At the grouped-query shapes, query heads reading K/V head h % nkv instead of h // g would move the o_proj anchor too.
 """
 from functools import lru_cache
 
@@ -44,9 +45,10 @@ def test_probe_anchors_have_teeth(gs):
     check_teeth('7b', gs)
 
 
-@pytest.mark.parametrize('size,gs', [('65b', 128), ('65b', 1024), ('33b', 1024)])
+@pytest.mark.parametrize('size,gs', [('65b', 128), ('65b', 1024), ('33b', 1024), ('70b', 128), ('llama3-8b', 'full')])
 def test_probe_anchors_have_teeth_large(size, gs):
-    """The same at the 65B and 33B probe layers; at 33B gs 1024 every corruption lands in a partial last group of 512."""
+    """The same at the 65B, 33B, 70B and LLaMA-3-8B probe layers; at 33B gs 1024 every corruption lands in a partial last group of 512.
+    At 70B and LLaMA-3-8B (8 K/V heads) also the o_proj input of query head h taken from K/V head h % nkv instead of h // g."""
     check_teeth(size, gs)
 
 
@@ -58,6 +60,7 @@ def check_teeth(size, gs):
     assert {'dropped k-step', 'repeated k-step', 'other sequence sum of x'} <= names
     if gs != 'full':
         assert {'neighbour scale', 'neighbour zero'} <= names
+    assert ('K/V head h % nkv' in names) == (L.nkv < L.nh)
     for (lin, name), (diff, total) in sorted(res.items()):
         frac = diff / total
         print(f'  {size} gs={gs} {lin} {name}: {diff} / {total} observed elements differ')

@@ -92,3 +92,22 @@ def test_matvec_plan_matches_the_kernel_at_7b_shapes():
         assert set(np.bincount(owners)) <= {U // nb, U // nb + 1}
         assert len({X.matvec_cta(K, N, 0, n)[0] for n in range(0, N, 256)}) == nslabs  # every slab starts in its own CTA
         assert nk == K // 32
+
+
+# (K, N) of every quantized linear of the LLaMA-65B, LLaMA-2-70B, CodeLlama-34B and LLaMA-3-8B decode step (qkv, o_proj, gate|up, down_proj)
+ROUTE_SHAPES = [(8192, 24576), (8192, 8192), (8192, 22016), (22016, 8192), (8192, 10240), (8192, 28672), (28672, 8192), (4096, 6144),
+                (4096, 4096), (4096, 14336), (14336, 4096)]
+
+
+def test_matvec_route_rule():
+    """skinny_supported's shared-memory rule, worked by hand: the x segment of a CTA is ceil(U / 264) k-steps of 32 per row.  65B qkv at
+    M = 8: 94 steps, 64 KB + 8 x 3040 x 2 B = 114176 B > 110 KB.  70B gate|up and down_proj: U = 28672, 109 steps, 64 KB + M x 7040 B:
+    107776 B at M = 6, 114816 B at M = 7.  Every other (shape, M) of the table fits."""
+    generic = {(8192, 24576, 8), (8192, 28672, 7), (8192, 28672, 8), (28672, 8192, 7), (28672, 8192, 8)}
+    assert X.matvec_smem_bytes(8, 8192, 24576) == 114176
+    assert X.matvec_smem_bytes(6, 8192, 28672) == X.matvec_smem_bytes(6, 28672, 8192) == 107776
+    assert X.matvec_smem_bytes(7, 8192, 28672) == X.matvec_smem_bytes(7, 28672, 8192) == 114816
+    for K, N in ROUTE_SHAPES:
+        for M in range(1, 9):
+            assert X.matvec_takes(M, K, N) == ((K, N, M) not in generic), f'M={M} K={K} N={N}: {X.matvec_smem_bytes(M, K, N)} B'
+    assert not X.matvec_takes(9, 4096, 4096) and not X.matvec_takes(0, 4096, 4096)

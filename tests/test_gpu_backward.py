@@ -251,7 +251,9 @@ def test_fp64_bound_at_tile_edges(ops, K, gs):
     report(worst, f'transposed tile edges K={K} gs={gs}: all M, all inputs')
 
 
-FULL_SHAPES = [(4096, 12288), (4096, 4096), (4096, 11008), (11008, 4096), (8192, 24576), (22016, 8192)]  # 7B linears, 65B extremes
+# 7B linears, 65B extremes; LLaMA-2-70B qkv, gate|up and down_proj; LLaMA-3-8B gate|up
+FULL_SHAPES = [(4096, 12288), (4096, 4096), (4096, 11008), (11008, 4096), (8192, 24576), (22016, 8192), (8192, 10240), (8192, 28672), (28672, 8192),
+               (4096, 14336)]
 
 
 @pytest.mark.parametrize('K,N', FULL_SHAPES)

@@ -9,7 +9,7 @@ import sys
 import pytest
 import torch
 
-from gpu_util import HD, check_cached_attention, make_kv_cache, report, run_cached_attention
+from gpu_util import HD, check_cached_attention, make_gqa_kv_cache, make_kv_cache, report, run_cached_attention
 
 pytestmark = pytest.mark.gpu
 
@@ -17,19 +17,26 @@ STARTS = (0, 1, 63, 64, 65, 127, 128, 129, 1000, 2047, 2048, 4095, None)  # None
 ROWS = (1, 2, 63, 64, 65, 127, 128, 129, 300)
 
 
-@pytest.mark.parametrize('rows', ROWS)
-def test_against_fp64_softmax_at_every_edge(rows):
+# (query heads, K/V heads): multi-head, one K/V head for 8 query heads, and 16 / 2 (g = 8 over two K/V heads, as LLaMA-2-70B and
+# LLaMA-3-8B group them).  The multi-head cases keep their ids.
+EDGE_CASES = [(nh, nkv, rows) for nh, nkv in ((2, 2), (8, 1), (16, 2)) for rows in ROWS]
+
+
+@pytest.mark.parametrize('nh,nkv,rows', EDGE_CASES, ids=[str(r) if nh == nkv else f'{nh}-{nkv}-{r}' for nh, nkv, r in EDGE_CASES])
+def test_against_fp64_softmax_at_every_edge(nh, nkv, rows):
     """Every start of STARTS with `rows` query rows, one span per sequence (8 per call, the last call partly filled), on a cache of CodeLlama's
-    16384 positions; every cache row outside the spans' reach is NaN."""
-    S, nh = 16384, 2
+    16384 positions; every cache row outside the spans' reach is NaN.  With nkv < nh each K/V head serves nh / nkv query heads, and the
+    reference repeats it that many times."""
+    S, g = 16384, nh // nkv
     starts = [S - rows if s is None else s for s in STARTS]
     worst = 0.0
     for c in range(0, len(starts), 8):
         spans = [(b, s, rows) for b, s in enumerate(starts[c:c + 8])]
-        q, kc, vc = make_kv_cache(8, nh, S, spans, seed=rows * 100 + c)
+        q, kc, vc = make_gqa_kv_cache(8, nh, nkv, S, spans, seed=rows * 100 + c)
         out = run_cached_attention(q, kc, vc, spans)
-        worst = max(worst, check_cached_attention(out, q, kc[1], vc[1], spans, f'rows {rows}'))
-    report(worst, f'{rows} rows at starts {starts}')
+        worst = max(worst, check_cached_attention(out, q, kc[1].repeat_interleave(g, 1), vc[1].repeat_interleave(g, 1), spans, f'{nh} / {nkv} heads, rows {rows}'))
+        del q, kc, vc, out
+    report(worst, f'{nh} / {nkv} heads, {rows} rows at starts {starts}')
 
 
 def test_llama_7b_shape():

@@ -12,7 +12,12 @@ At LLaMA-65B shapes (hidden 8192, the persistent kernel's limit) the cases are g
 sequence above it (the kernel chain), gs 1024 (down_proj, K = 22016, ends in a partial group of 512) and int4 act-order gs 128 (the
 qkv_perm / mlp_perm gathers at H = 8192); at LLaMA-33B gs 1024, where every linear ends in a partial group of 512, at batch 1 and the
 largest persistent batch, and gs full on the kernel chain.  The batch limits come from the device's SM count (gs_probe.resolve_batch).
-Each case asserts its path: the launch count and the groupsize hint of every kernel layer.  tests/test_decode_groupsize_fixtures.py shows
+At the grouped-query shapes (qkv H + 2 Hkv wide, o_proj reading each K/V head's V row once per query head of its group): LLaMA-2-70B gs
+128 at batch 1, the largest persistent batch, one above it and batch 8, gs 1024 at batch 7, int4 act-order gs 128; CodeLlama-34B gs 1024
+at batch 1 and 8; LLaMA-3-8B gs 128 at batch 1 and 8 and gs full.  At 70B batch 7 and 8 the kernel chain runs gate|up and down_proj on
+the generic kernel (the split-K matvec's x segment exceeds its shared memory there), with the RMSNorm and the residual add as separate
+launches: 11 per step instead of 9.
+Each case asserts its path: the launch count (gs_probe.chain_launches on the kernel chain) and the groupsize hint of every kernel layer.  tests/test_decode_groupsize_fixtures.py shows
 on the CPU that the fixtures are exact and that a group, sequence or k-step mix-up would break these anchors; the last test here shows it
 on the device.
 """
@@ -26,9 +31,6 @@ from attn_probe import resid_buffers
 from gpu_util import fp16_ulp_distance
 
 pytestmark = pytest.mark.gpu
-
-CHAIN_LAUNCHES = 9  # one layer: embed, qkv, attention, combine, o_proj, gate|up, down_proj (all on the skinny matvec), lm_head, argmax
-
 
 def build(L, mode, B, n_layers):
     """LlamaDecoder of the probe layer: mode 'o' (gate / up / down scales 0) or 'mlp' (o_proj scales 0)."""
@@ -44,7 +46,7 @@ def build(L, mode, B, n_layers):
     embed = P.embed_rows(P.VOCAB, L.H).to(dev)
     lm_head = (torch.randn(P.VOCAB, L.H, generator=torch.Generator().manual_seed(5)) * 0.02).half().to(dev)
     return engine.LlamaDecoder([ly] * n_layers, embed, torch.ones(L.H, dtype=torch.float16, device=dev), lm_head, L.nh, rms_eps=0.0, batch=B,
-                               max_seq=32)
+                               max_seq=32, n_kv_heads=L.nkv)
 
 
 def step(dec, toks):
@@ -62,9 +64,11 @@ def mismatch(got, want):
     return f'{int((d > 0).sum())} / {d.numel()} elements off, up to {int(d.max())} ulp; first at {i}: {got.reshape(-1)[i].item()} vs {want.reshape(-1)[i].item()}'
 
 
-def check_path(dec, L, engine_name, what):
+def check_path(dec, L, B, engine_name, what):
+    """One launch on the persistent kernel; on the chain 9 when the split-K matvec serves every linear, 2 more per linear it does not
+    take (gs_probe.chain_launches)."""
     n = dec.launches_per_step()
-    assert n == (1 if engine_name == 'persistent' else CHAIN_LAUNCHES), f'{what}: {n} launches per step'
+    assert n == (1 if engine_name == 'persistent' else P.chain_launches(L, B)), f'{what}: {n} launches per step'
     for kl in dec.klayers:
         for name in ('qkv', 'o', 'gate', 'up', 'down'):
             K = L.linears()[name].K
@@ -97,12 +101,13 @@ def run_case(size, gs, bits, act, B, engine_name):
     x_in = P.embed_rows(P.VOCAB, H)[torch.tensor(toks)]
     E = P.Expect(L, x_in, device=dev)
     assert bool((E.a >= 20).all()), 'gate outputs below 20: the sigmoid is not exactly 1'
-    what = f'{size} int{bits} act={act} gs={gs} batch {B} ({engine_name})'
+    route = '' if engine_name == 'persistent' else f', {P.chain_launches(L, B)} launches'
+    what = f'{size} int{bits} act={act} gs={gs} batch {B} ({engine_name}{route})'
     bad = []
     for mode in ('o', 'mlp'):
         n_layers = 2 if (mode == 'mlp' and engine_name == 'persistent') else 1
         dec = build(L, mode, B, n_layers)
-        check_path(dec, L, engine_name, what)
+        check_path(dec, L, B, engine_name, what)
         step(dec, toks)
         for b in range(B):
             for name, got, want in (('K row', dec.k_cache[0, b, :, 0], E.k[b]), ('V row', dec.v_cache[0, b, :, 0], E.v[b])):

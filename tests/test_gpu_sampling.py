@@ -9,7 +9,7 @@ from oracle import sampling as S
 
 pytestmark = pytest.mark.gpu
 
-VOCABS = [1, 2, 33, 32000, 32001, 131072]
+VOCABS = [1, 2, 33, 32000, 32001, 128256, 131072]  # (128256: LLaMA-3)
 GRID = [(t, k, p) for t in (0.0, 0.1, 0.8, 1.0, 2.5) for k in ('0', '1', '50', 'V') for p in (0.05, 0.95, 1.0)]
 KINDS = ['random', 'equal', 'outlier', 'ties at k', 'top-p boundary', '+inf', '-inf and NaN', 'all -inf']
 

@@ -15,12 +15,20 @@ pytestmark = pytest.mark.gpu
 def test_exact_anchors_on_an_integer_grid():
     """x = a 2^-4, W = b 2^-4 with small integers: every product and partial sum is a multiple of 2^-8 below 2^16 (exact in fp32) and every
     logit is a multiple of 2^-8 below 8, or 1000: exact in fp16.  Then only the fp32 log-softmax separates the kernel from float64."""
-    from gptq_b200 import ops
-    K, V, P, vstar = 5120, 32001, 4000, 4242
+    check_integer_grid_anchors(32001)
+
+
+def test_exact_anchors_on_an_integer_grid_at_the_llama3_vocabulary():
+    """The same at LLaMA-3's vocabulary, 128256: the combine pass merges 1002 vocabulary tiles per row, 32 per lane."""
+    check_integer_grid_anchors(128256)
+
+
+def integer_grid_inputs(V, K=5120, P=4000, vstar=4242):
+    """(x [19, K], W [V, K], targets) on the device, every value exact in fp16 (W is built in fp16: 1.3 GB at V = 128256)."""
     g = torch.Generator().manual_seed(0)
-    W = torch.zeros(V, K)
+    W = torch.zeros(V, K, dtype=torch.float16)
     idx = torch.randint(0, K, (V, 64), generator=g)
-    W.scatter_(1, idx, (torch.randint(1, 3, (V, 64), generator=g) * (2 * torch.randint(0, 2, (V, 64), generator=g) - 1)).float())  # <= 64 nonzeros in +-{1,2}
+    W.scatter_(1, idx, (torch.randint(1, 3, (V, 64), generator=g) * (2 * torch.randint(0, 2, (V, 64), generator=g) - 1)).half())  # <= 64 nonzeros in +-{1,2}
     W[vstar] = 0
     W[vstar, :P] = 8  # only the dominant row reaches this vocabulary row
     x = torch.zeros(19, K)
@@ -28,16 +36,24 @@ def test_exact_anchors_on_an_integer_grid():
     # row 16: all zeros -> every logit 0 -> -log V; rows 17, 18: the dominant row, l[vstar] = 4000 * 64 * 2^-8 = 1000, every other |l| <= 4
     x[17:, :P] = 8
     targets = torch.tensor([0, 127, 128, V - 1, vstar] + torch.randint(0, V, (11, ), generator=g).tolist() + [5, vstar, 0], dtype=torch.int32)
-    x, W, targets = (x / 16).half().cuda(), (W / 16).half().cuda(), targets.cuda()
+    W = W.cuda()
+    W /= 16  # exact: a power of two on small integers
+    return (x / 16).half().cuda(), W, targets.cuda()
+
+
+def check_integer_grid_anchors(V):
+    from gptq_b200 import ops
+    x, W, targets = integer_grid_inputs(V)
     lp = ops.lm_head_logprob(x, W, targets)
-    ref = check_logprob(lp, x, W, targets, 'integer grid', exact=True)
+    ref = check_logprob(lp, x, W, targets, f'integer grid V={V}', exact=True)
     assert abs(ref[16].item() + math.log(V)) < 1e-12 and abs(lp[16].item() + math.log(V)) <= lse_tol(0.0, V, ref[16]).item()
     assert lp[17].item() == 0.0  # every other exp underflows: 1000 - (1000 + log 1)
     assert ref[18].item() < -990 and lp[18].item() == ref[18].item()  # l_0 - 1000 is exact
 
 
 EDGES = ([(M, 32001, 256, None, None) for M in (1, 2, 127, 128, 129, 255, 256, 257, 4099)] + [(257, V, 64, None, None) for V in (300, 1000, 32000, 32001)] +
-         [(129, 1000, K, None, None) for K in (64, 256, 4096, 5120)] + [(300, 32001, 4096, 4096 + 64, 4096 + 8), (129, 300, 64, 72, 128)])
+         [(129, 1000, K, None, None) for K in (64, 256, 4096, 5120)] + [(300, 32001, 4096, 4096 + 64, 4096 + 8), (129, 300, 64, 72, 128)] +
+         [(M, 128256, 4096, None, None) for M in (1, 257, 4099, 8191)])  # LLaMA-3-8B: 1002 vocabulary tiles; a perplexity chunk of 8191 rows
 
 
 @pytest.mark.parametrize('M,V,K,ldx,ldw', EDGES)
