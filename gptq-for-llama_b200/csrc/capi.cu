@@ -117,7 +117,20 @@ int gptq_rope_inplace(void* qk, int64_t token_stride, const int64_t* position_id
     if (!aligned(qk, 4) || token_stride % 2 != 0 || !aligned(position_ids, 8)) return GPTQ_ERR_ALIGN;
     if ((int64_t)bsz * seq == 0) return GPTQ_OK;
     if ((int64_t)bsz * seq > 0x7fffffffLL) return GPTQ_ERR_SHAPE;
-    return cuda_status(launch_rope(qk, token_stride, position_ids, pos_batch_stride, bsz, seq, rows, head_dim, base, static_cast<cudaStream_t>(stream)));
+    return cuda_status(launch_rope(qk, token_stride, position_ids, pos_batch_stride, bsz, seq, rows, head_dim, base, nullptr, static_cast<cudaStream_t>(stream)));
+}
+
+int gptq_rope_inplace_freq(void* qk, int64_t token_stride, const int64_t* position_ids, int64_t pos_batch_stride, int bsz, int seq, int rows, int head_dim,
+                           const float* inv_freq, gptq_stream_t stream) {
+    if (qk == nullptr || position_ids == nullptr || inv_freq == nullptr) return GPTQ_ERR_NULL;
+    if (bsz < 0 || seq < 0 || rows <= 0 || head_dim <= 0 || head_dim % 4 != 0) return GPTQ_ERR_SHAPE;
+    if (head_dim > 2 * kRopeMaxPairs) return GPTQ_ERR_UNSUPPORTED;  // the table travels in the launch parameters
+    if (!rope_table_ok(inv_freq, head_dim / 2)) return GPTQ_ERR_SHAPE;
+    if (token_stride < (int64_t)rows * head_dim || pos_batch_stride < seq) return GPTQ_ERR_SHAPE;
+    if (!aligned(qk, 4) || token_stride % 2 != 0 || !aligned(position_ids, 8)) return GPTQ_ERR_ALIGN;
+    if ((int64_t)bsz * seq == 0) return GPTQ_OK;
+    if ((int64_t)bsz * seq > 0x7fffffffLL) return GPTQ_ERR_SHAPE;
+    return cuda_status(launch_rope(qk, token_stride, position_ids, pos_batch_stride, bsz, seq, rows, head_dim, 1.f, inv_freq, static_cast<cudaStream_t>(stream)));
 }
 
 int gptq_rmsnorm_fwd(const void* x, int64_t ldx, const void* weight, void* y, int64_t ldy, int M, int N, float eps, gptq_stream_t stream) {

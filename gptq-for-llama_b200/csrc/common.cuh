@@ -105,12 +105,36 @@ __device__ __forceinline__ float warp_sum(float v) {
 __device__ __forceinline__ float swiglu(float a, float b) { return (a * (1.0f / (1.0f + expf(-a)))) * b; }
 
 // ---- RoPE (rotate_half_kernel, quant/fused_attn.py:8-58) --------------------------------------------------------------------
-// Both decode engines and gptq_rope_inplace rotate with these, so their q and k agree bit for bit.
+// Both decode engines and gptq_rope_inplace(_freq) rotate with these, so their q and k agree bit for bit.
 inline float rope_inv_base(float base, int head_dim) { return (float)(-2.0 * log((double)base) / (double)head_dim); }  // :91
 inline float attn_scale(int head_dim) { return 1.0f / sqrtf((float)head_dim); }                                        // SDPA's head_dim^-0.5
-// exp(i * inv_base): times the position, the angle of pair i (then its cosf and sinf); fp32 with the accurate expf (the reference insists
-// on libdevice exp, :42-43)
-__device__ __forceinline__ float rope_inv_freq(int i, float inv_base) { return expf((float)i * inv_base); }
+
+// The frequencies of one rotation, carried by value in the launch parameters (a captured graph replays them without a device buffer).
+// table == 0: pair i turns by exp(i * inv_base), the unscaled rule.  table == 1: by f[i], a host table of head_dim / 2 values (a scaled
+// rotation such as LLaMA-3.1's llama3 rule, computed by the host bit for bit as HF computes it; gptq_b200.ops.rope_inv_freq).
+constexpr int kRopeMaxPairs = 64;  // head_dim 128
+struct RopeFreqs {
+    float inv_base;
+    int table;
+    float f[kRopeMaxPairs];
+};
+// host: the rule of a call; inv_freq (HOST, head_dim / 2 entries, checked by rope_table_ok) or nullptr for the unscaled rule at `base`
+inline RopeFreqs rope_freqs(float base, int head_dim, const float* inv_freq) {
+    RopeFreqs r{};
+    r.inv_base = rope_inv_base(base, head_dim);
+    r.table = inv_freq != nullptr;
+    for (int i = 0; inv_freq != nullptr && i < head_dim / 2; ++i) r.f[i] = inv_freq[i];
+    return r;
+}
+// host: every entry of a table finite and > 0 (a frequency the angle rule below can use)
+inline bool rope_table_ok(const float* inv_freq, int n) {
+    for (int i = 0; i < n; ++i)
+        if (!(inv_freq[i] > 0.f) || !isfinite(inv_freq[i])) return false;
+    return true;
+}
+// The frequency of pair i; times the position, rounded once in fp32, it is the angle (then its cosf and sinf).  The unscaled rule is fp32
+// with the accurate expf (the reference insists on libdevice exp, :42-43).
+__device__ __forceinline__ float rope_inv_freq(int i, const RopeFreqs& r) { return r.table ? r.f[i] : expf((float)i * r.inv_base); }
 // x' = x c - y s ; y' = x s + y c, y at +head_dim/2 (:52-57): the reference's operation order, no FMA contraction (two roundings per term)
 __device__ __forceinline__ float rope_x(float x, float y, float c, float s) { return __fsub_rn(__fmul_rn(x, c), __fmul_rn(y, s)); }
 __device__ __forceinline__ float rope_y(float x, float y, float c, float s) { return __fadd_rn(__fmul_rn(x, s), __fmul_rn(y, c)); }

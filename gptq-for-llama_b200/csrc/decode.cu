@@ -49,7 +49,7 @@ __device__ __forceinline__ void load_key_dims(const __half* cache, const __half*
 }
 
 // RoPE(q, k) + KV append + attention over keys [split*256, min(split*256+256, pos+1)).
-//   rotation: rotate_half_kernel (quant/fused_attn.py:23-58): freq_i = exp(i * inv_base) * pos, fp32, results rounded to fp16
+//   rotation: rotate_half_kernel (quant/fused_attn.py:23-58): angle_i = rope_inv_freq(i) * pos (common.cuh), fp32, results rounded to fp16
 //   scores:   fp16 q.k with fp32 accumulation, * head_dim^-0.5, softmax in fp32, fp32 P.V  (SDPA, fused_attn.py:154-155)
 // grid (heads, nsplit, batch).  Partial (m, l, o[128]) per (batch, head, split) goes to `part`.
 // Grouped-query attention: qkv rows are [hidden q | n_kv_heads * 128 k | n_kv_heads * 128 v] and query head h reads K/V head h / g
@@ -57,7 +57,7 @@ __device__ __forceinline__ void load_key_dims(const __half* cache, const __half*
 // memory, never from the cache (a sibling's store may not have landed); only the group's first head stores it.
 __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half* __restrict__ qkv, int hidden, int n_kv_heads, __half* __restrict__ k_cache,
                                                                    __half* __restrict__ v_cache, const int32_t* __restrict__ positions, int n_heads, int max_seq,
-                                                                   int batch, float inv_base, float scale, float* __restrict__ part, int nsplit) {
+                                                                   int batch, const RopeFreqs rope, float scale, float* __restrict__ part, int nsplit) {
     const int head = blockIdx.x, split = blockIdx.y, b = blockIdx.z;
     grid_launch_dependents();
     grid_dependency_wait();
@@ -84,7 +84,7 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const __half*
     __half* vc = v_cache + ((size_t)(b * n_kv_heads + kv_head) * max_seq) * kHeadDim;
 
     if (tid < 64) {
-        const float f = rope_inv_freq(tid, inv_base) * (float)pos;
+        const float f = rope_inv_freq(tid, rope) * (float)pos;
         cs_s[tid] = cosf(f);
         cs_s[64 + tid] = sinf(f);
     }
@@ -418,13 +418,18 @@ extern "C" int gptq_llama_decode_launches(const gptq_llama_model* model, const g
     return n;
 }
 
-extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_llama_state* st, gptq_stream_t stream_) {
+extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_llama_state* st, gptq_stream_t stream) {
+    return gptq_llama_decode_step_rope(model, st, nullptr, stream);
+}
+
+extern "C" int gptq_llama_decode_step_rope(const gptq_llama_model* model, const gptq_llama_state* st, const float* inv_freq, gptq_stream_t stream_) {
     if (model == nullptr || st == nullptr) return GPTQ_ERR_NULL;
     const gptq_llama_model& m = *model;
     if (m.layers == nullptr || m.embed == nullptr || m.final_norm == nullptr || m.lm_head == nullptr) return GPTQ_ERR_NULL;
     if (st->k_cache == nullptr || st->v_cache == nullptr || st->tokens == nullptr || st->positions == nullptr || st->logits == nullptr || st->scratch == nullptr)
         return GPTQ_ERR_NULL;
     if (m.head_dim != kHeadDim) return GPTQ_ERR_UNSUPPORTED;  // LLaMA-7B/13B/33B/65B all use head_dim 128
+    if (inv_freq != nullptr && !rope_table_ok(inv_freq, kHeadDim / 2)) return GPTQ_ERR_SHAPE;
     const int Hq = m.n_heads * m.head_dim;  // = hidden, or this rank's share of it under tensor parallelism
     if ((st->tp == nullptr && Hq != m.hidden) || Hq < 1 || Hq > m.hidden || m.hidden % 32 != 0 || m.intermediate % 32 != 0 || m.n_layers < 1 || m.vocab < 1) return GPTQ_ERR_SHAPE;
     if (st->batch < 1 || st->batch > 8 || st->max_seq < 1) return GPTQ_ERR_SHAPE;
@@ -445,7 +450,7 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     uint8_t* sc = reinterpret_cast<uint8_t*>(st->scratch);
     // tensor-parallel ranks keep the persistent kernel's region at the START of the scratch area (peers address it by offset)
-    const cudaError_t mega = launch_decode_mega(m, *st, st->tp != nullptr ? sc : sc + L.mega, stream);
+    const cudaError_t mega = launch_decode_mega(m, *st, st->tp != nullptr ? sc : sc + L.mega, inv_freq, stream);
     if (mega == cudaSuccess) return GPTQ_OK;
     if (mega != cudaErrorCooperativeLaunchTooLarge && mega != cudaErrorInvalidConfiguration) return GPTQ_ERR_CUDA;
     // the step does not fit the persistent kernel, or the device cannot co-schedule its grid: per-op kernel chain below
@@ -455,7 +460,7 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
     __half* attn = reinterpret_cast<__half*>(sc + L.attn);
     float* part = reinterpret_cast<float*>(sc + L.part);
     const int B = st->batch, H = m.hidden;
-    const float inv_base = rope_inv_base(m.rope_base, m.head_dim);
+    const RopeFreqs rope = rope_freqs(m.rope_base, m.head_dim, inv_freq);
     const float scale = attn_scale(m.head_dim);
     const size_t layer_stride = (size_t)B * n_kv * st->max_seq * m.head_dim;
 
@@ -471,7 +476,7 @@ extern "C" int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_
         GPTQ_TRY(engine_linear(c[0], sc, L));
         GPTQ_TRY(launch_kernel(attn_decode_kernel, dim3(m.n_heads, L.nsplit, B), dim3(kAttnThreads), 0, stream, true, qkv, H, n_kv,
                                reinterpret_cast<__half*>(st->k_cache) + l * layer_stride, reinterpret_cast<__half*>(st->v_cache) + l * layer_stride,
-                               st->positions, m.n_heads, st->max_seq, B, inv_base, scale, part, L.nsplit));
+                               st->positions, m.n_heads, st->max_seq, B, rope, scale, part, L.nsplit));
         GPTQ_TRY(launch_kernel(attn_combine_kernel, dim3(m.n_heads, B), dim3(kHeadDim), 0, stream, true, part, st->positions, attn, H, m.n_heads, L.nsplit));
         for (int i = 1; i < 4; ++i) GPTQ_TRY(engine_linear(c[i], sc, L));
     }

@@ -139,7 +139,7 @@ struct MegaParams {
     // the width of the fused q | k | v output (3 Hq for multi-head attention)
     int n_kv_heads, kv_group, Nqkv;
     int tp_size, tp_rank, tp_exchange;  // tp_exchange: reduce locally first, then hand slices to the ranks (else: every team REDs into every rank)
-    float eps, inv_base, scale;
+    float eps, scale;
     const __half* embed;
     const __half* final_norm;
     const __half* lm_head;
@@ -176,6 +176,7 @@ struct MegaParams {
     // 64 mod 128 bytes puts the two lane groups of a quarter-warp on different banks).  Per-sequence vectors are [batch][n] with
     // n = H, Nqkv, I, V or 128 (rope_cs); resid, acc_* and rope_cs are sized for the batch.
     int batch, xs_stride;
+    RopeFreqs rope;  // this step's rotation rule (common.cuh); last, so that adding it moved no other field
 };
 
 // ---- work split ------------------------------------------------------------------------------------------------
@@ -1554,10 +1555,10 @@ __global__ void __launch_bounds__(kBlock, 1) llama_decode_mega_kernel(const __gr
         }
     };
 
-    // this step's RoPE angles, one row per sequence (quant/fused_attn.py:43,91): freq_i = exp(i * inv_base) * pos
+    // this step's RoPE angles, one row per sequence (quant/fused_attn.py:43,91): angle_i = rope_inv_freq(i) * pos
     if (blockIdx.x == 0 && tid < 64 * nbat) {
         const int s = tid >> 6, i = tid & 63;
-        const float f = rope_inv_freq(i, p.inv_base) * (float)step_pos(p, s);
+        const float f = rope_inv_freq(i, p.rope) * (float)step_pos(p, s);
         p.rope_cs[s * kHD + i] = cosf(f);
         p.rope_cs[s * kHD + 64 + i] = sinf(f);
     }
@@ -1805,7 +1806,7 @@ bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st) {
 
 size_t mega_scratch_bytes(const gptq_llama_model& m, int batch) { return mega_scratch(m, batch).total; }
 
-cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state& st, uint8_t* scratch, cudaStream_t stream) {
+cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state& st, uint8_t* scratch, const float* inv_freq, cudaStream_t stream) {
     static_assert(sizeof(MegaParams) < 32000, "kernel parameter space");
     MegaPlan pl;
     cudaError_t e = mega_step_plan(m, st, pl);
@@ -1824,7 +1825,7 @@ cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state
     p.n_stages = pl.n_stages;
     p.lm_rows = pl.lm_rows;
     p.eps = m.rms_eps;
-    p.inv_base = rope_inv_base(m.rope_base, m.head_dim);
+    p.rope = rope_freqs(m.rope_base, m.head_dim, inv_freq);
     p.scale = attn_scale(m.head_dim);
     p.embed = reinterpret_cast<const __half*>(m.embed);
     p.final_norm = reinterpret_cast<const __half*>(m.final_norm);

@@ -7,7 +7,7 @@ namespace {
 
 // rotate_half_kernel (quant/fused_attn.py:8-58): one block per token, threads over (row, i); fp32 math (common.cuh), fp16 store.
 __global__ void rope_kernel(__half* __restrict__ qk, int64_t token_stride, const int64_t* __restrict__ position_ids, int64_t pos_batch_stride, int seq,
-                            int rows, int head_dim, float inv_base) {
+                            int rows, int head_dim, const RopeFreqs rope) {
     const int token = blockIdx.x;
     const int b = token / seq, s = token % seq;
     const float pos = (float)__ldg(position_ids + (size_t)b * pos_batch_stride + s);
@@ -18,7 +18,7 @@ __global__ void rope_kernel(__half* __restrict__ qk, int64_t token_stride, const
     for (int idx = threadIdx.x; idx < rows * pairs_per_row; idx += blockDim.x) {
         const int row = idx / pairs_per_row;
         const int i = (idx - row * pairs_per_row) * 2;
-        const float f0 = rope_inv_freq(i, inv_base) * pos, f1 = rope_inv_freq(i + 1, inv_base) * pos;
+        const float f0 = rope_inv_freq(i, rope) * pos, f1 = rope_inv_freq(i + 1, rope) * pos;
         const float c0 = cosf(f0), s0 = sinf(f0), c1 = cosf(f1), s1 = sinf(f1);
         __half2* px = reinterpret_cast<__half2*>(base + (size_t)row * head_dim + i);
         __half2* py = reinterpret_cast<__half2*>(base + (size_t)row * head_dim + half_dim + i);
@@ -65,11 +65,11 @@ __global__ void __launch_bounds__(THREADS) rmsnorm_kernel(const __half* __restri
 }  // namespace
 
 cudaError_t launch_rope(void* qk, int64_t token_stride, const int64_t* position_ids, int64_t pos_batch_stride, int bsz, int seq, int rows, int head_dim,
-                        float base, cudaStream_t stream) {
+                        float base, const float* inv_freq, cudaStream_t stream) {
     const int work = rows * (head_dim / 4);
     const int threads = work >= 256 ? 256 : ((work + 31) / 32) * 32;
     rope_kernel<<<bsz * seq, threads, 0, stream>>>(reinterpret_cast<__half*>(qk), token_stride, position_ids, pos_batch_stride, seq, rows, head_dim,
-                                                    rope_inv_base(base, head_dim));
+                                                    rope_freqs(base, head_dim, inv_freq));
     return cudaGetLastError();
 }
 

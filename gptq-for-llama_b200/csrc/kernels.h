@@ -84,14 +84,14 @@ constexpr int kSampleMaxBatch = 8, kSampleMaxVocab = 131072;
 cudaError_t launch_sample_tokens(const void* logits, int64_t ld, int batch, int vocab, const int32_t* positions, const gptq_sampling& params,
                                  int32_t* next_tokens, cudaStream_t stream);
 
-// decode_mega.cu -- persistent single-kernel decode step (batch 1 to 8, int4 kernel-form layers)
+// decode_mega.cu -- persistent single-kernel decode step (batch 1 to 8, int4 kernel-form layers); inv_freq as for launch_rope
 bool mega_supported(const gptq_llama_model& m, const gptq_llama_state& st);
 size_t mega_scratch_bytes(const gptq_llama_model& m, int batch);
-cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state& st, uint8_t* scratch, cudaStream_t stream);
+cudaError_t launch_decode_mega(const gptq_llama_model& m, const gptq_llama_state& st, uint8_t* scratch, const float* inv_freq, cudaStream_t stream);
 
-// elementwise.cu
+// elementwise.cu -- inv_freq: a HOST table of head_dim / 2 frequencies (head_dim <= 128), or nullptr for the unscaled rule at `base` (common.cuh)
 cudaError_t launch_rope(void* qk, int64_t token_stride, const int64_t* position_ids, int64_t pos_batch_stride, int bsz, int seq, int rows, int head_dim,
-                        float base, cudaStream_t stream);
+                        float base, const float* inv_freq, cudaStream_t stream);
 cudaError_t launch_rmsnorm(const void* x, int64_t ldx, const void* weight, void* y, int64_t ldy, int M, int N, float eps, cudaStream_t stream);
 
 // pack.cu

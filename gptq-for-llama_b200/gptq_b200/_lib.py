@@ -75,6 +75,7 @@ SIGNATURES = {
     'gptq_fused_mlp_fwd': (c_int, [c_void_p, c_int64, _QW, _QW, c_void_p, c_int64, c_int, c_void_p, c_size_t, c_void_p]),
     'gptq_qlinear_transpose_fwd': (c_int, [c_void_p, c_int64, _QW, c_void_p, c_int64, c_int, c_void_p]),
     'gptq_rope_inplace': (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_float, c_void_p]),
+    'gptq_rope_inplace_freq': (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_int, ctypes.POINTER(c_float), c_void_p]),
     'gptq_rmsnorm_fwd': (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int, c_int, c_float, c_void_p]),
     'gptq_pack_qweight': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     'gptq_pack_qzeros': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
@@ -83,6 +84,7 @@ SIGNATURES = {
     'gptq_dequant': (c_int, [_QW, c_void_p, c_int64, c_void_p]),
     'gptq_llama_scratch_bytes': (c_size_t, [ctypes.POINTER(LlamaModel), c_int, c_int]),
     'gptq_llama_decode_step': (c_int, [ctypes.POINTER(LlamaModel), ctypes.POINTER(LlamaState), c_void_p]),
+    'gptq_llama_decode_step_rope': (c_int, [ctypes.POINTER(LlamaModel), ctypes.POINTER(LlamaState), ctypes.POINTER(c_float), c_void_p]),
     'gptq_llama_decode_launches': (c_int, [ctypes.POINTER(LlamaModel), ctypes.POINTER(LlamaState)]),
     'gptq_llama_persistent_scratch_offset': (c_size_t, [ctypes.POINTER(LlamaModel), c_int, c_int]),
     'gptq_lm_head_logprob_workspace_bytes': (c_size_t, [c_int, c_int]),

@@ -29,13 +29,21 @@ LLAMA_SHAPES = {  # hidden, intermediate, layers, heads (SURVEY.md section 8)
     # grouped-query attention: their K/V head counts are in KV_HEADS
     '70b': (8192, 28672, 80, 64),        # LLaMA-2-70B
     '34b': (8192, 22016, 48, 64),        # CodeLlama-34B (RoPE base 1e6)
-    'llama3-8b': (4096, 14336, 32, 32),  # LLaMA-3-8B (RoPE base 5e5, vocabulary 128256)
+    'llama3-8b': (4096, 14336, 32, 32),  # LLaMA-3-8B (RoPE base 5e5, vocabulary 128256); LLaMA-3.1-8B with LLAMA3_1_ROPE_SCALING
+    'llama3.2-3b': (3072, 8192, 28, 24),  # LLaMA-3.2-3B (RoPE base 5e5, LLAMA3_2_ROPE_SCALING, vocabulary 128256, lm_head tied to the embedding)
     'tiny-gqa2': (512, 1024, 2, 4),      # persistent single-kernel path, 2 query heads per K/V head
     'tiny-gqa1': (512, 1024, 2, 4),      # persistent, one K/V head for all 4 query heads
     'tiny-gqa2-chain': (512, 704, 2, 4),  # intermediate not a multiple of 256: the kernel-chain engine
     'tiny-gqa1-chain': (512, 704, 2, 4),
 }
-KV_HEADS = {'70b': 8, '34b': 8, 'llama3-8b': 8, 'tiny-gqa2': 2, 'tiny-gqa1': 1, 'tiny-gqa2-chain': 2, 'tiny-gqa1-chain': 1}  # other shapes: one per head
+KV_HEADS = {'70b': 8, '34b': 8, 'llama3-8b': 8, 'llama3.2-3b': 8, 'tiny-gqa2': 2, 'tiny-gqa1': 1, 'tiny-gqa2-chain': 2, 'tiny-gqa1-chain': 1}  # other shapes: one per head
+
+# The llama3 RoPE scaling of the published LLaMA-3.x checkpoints (their config.json's rope_scaling; RoPE base 5e5).  LLaMA-3.1-8B is 'llama3-8b'
+# with LLAMA3_1_ROPE_SCALING; LLaMA-3.1-70B and 3.3-70B are '70b' with vocabulary 128256 and LLAMA3_1_ROPE_SCALING / LLAMA3_3_ROPE_SCALING.
+LLAMA3_1_ROPE_SCALING = {'rope_type': 'llama3', 'factor': 8.0, 'low_freq_factor': 1.0, 'high_freq_factor': 4.0, 'original_max_position_embeddings': 8192}
+LLAMA3_2_ROPE_SCALING = dict(LLAMA3_1_ROPE_SCALING, factor=32.0)
+LLAMA3_3_ROPE_SCALING = LLAMA3_1_ROPE_SCALING
+LLAMA3_ROPE_BASE = 500000.0
 
 
 def kv_heads(size):
@@ -94,16 +102,26 @@ class LlamaDecoder:
     """Owns the weights, the KV cache and the captured graph; `step()` decodes one token per sequence."""
 
     def __init__(self, layers, embed, final_norm, lm_head, n_heads, rms_eps=1e-6, rope_base=10000.0, batch=1, max_seq=2048, use_graph=True, head_dim=None,
-                 tp=None, n_kv_heads=None):
+                 tp=None, n_kv_heads=None, rope_scaling=None):
         """tp = (rank, size, vocab_begin, vocab_end[, reduce_mode]): this process holds one tensor-parallel shard (see shard_for_rank / gptq_llama_tp): `layers`,
         `lm_head` and `n_heads` are the LOCAL ones, head_dim must be given, and torch.distributed must be initialised (the scratch and logits
         buffers of the ranks are exchanged as CUDA IPC handles).
         n_kv_heads: K/V heads of grouped-query attention (None: n_heads, multi-head attention).  It must divide n_heads, and every layer's fused
         qkv must be (n_heads + 2 n_kv_heads) * head_dim wide (q, then k, then v heads; the width is how the kernels learn the count).
-        The KV cache holds n_kv_heads heads.  Tensor parallelism needs n_kv_heads == n_heads."""
+        The KV cache holds n_kv_heads heads.  Tensor parallelism needs n_kv_heads == n_heads.
+        rope_scaling: HF's rope_scaling dict of a scaled rotation (llama3: LLaMA-3.1 / 3.2 / 3.3, e.g. LLAMA3_1_ROPE_SCALING), or the fp32
+        frequency table [head_dim / 2] such a dict gives (ops.rope_inv_freq; the quant attention modules carry it).  The table is built once
+        (`rope_inv_freq`) and every rotation follows it: both decode engines (gptq_llama_decode_step_rope, in the captured graphs too) and the
+        RoPE of prefill, extend and score; rope_base is then unused.  None: the unscaled rotation at rope_base."""
         self.dev = embed.device
         self.tp = tp
         self.head_dim = head_dim or embed.shape[1] // n_heads
+        table = rope_scaling if rope_scaling is None or isinstance(rope_scaling, torch.Tensor) else ops.rope_inv_freq(rope_base, self.head_dim, rope_scaling)
+        self.rope_inv_freq = None if table is None else table.detach().to('cpu', torch.float32).contiguous()
+        if self.rope_inv_freq is not None and (self.rope_inv_freq.shape != (self.head_dim // 2, ) or not bool((self.rope_inv_freq > 0).all())
+                                               or not bool(torch.isfinite(self.rope_inv_freq).all())):
+            raise ValueError(f'the RoPE frequency table must hold {self.head_dim // 2} finite values > 0')
+        self._rope_table = None if table is None else (ctypes.c_float * (self.head_dim // 2))(*self.rope_inv_freq.tolist())  # what the C ABI reads
         self.layers = layers  # list of dicts: qkv, o, gate, up, down (QLayerWeights), input_norm, post_norm (fp16 tensors)
         self.n_kv_heads = n_heads if n_kv_heads is None else int(n_kv_heads)
         if self.n_kv_heads < 1 or n_heads % self.n_kv_heads != 0:
@@ -227,7 +245,7 @@ class LlamaDecoder:
     # ------------------------------------------------------------------------------------------
     def _enqueue(self, stream, sample=False):
         """One decode step on `stream`; with `sample`, followed by gptq_sample_tokens under set_sampling's parameters."""
-        check(lib.gptq_llama_decode_step(ctypes.byref(self.model), ctypes.byref(self.state), ctypes.c_void_p(stream.cuda_stream)))
+        check(lib.gptq_llama_decode_step_rope(ctypes.byref(self.model), ctypes.byref(self.state), self._rope_table, ctypes.c_void_p(stream.cuda_stream)))
         if sample:
             self._enqueue_sample(stream)
 
@@ -375,7 +393,7 @@ class LlamaDecoder:
             qkv = ops.matmul248(ops.rmsnorm(x, ly['input_norm'], self.model.rms_eps), *ly['qkv'].parts(), ly['qkv'].bits,
                                 groupsize=ly['qkv'].hint).view(1, total, nh + 2 * nkv, hd)  # q | k | v heads
             # q and k are the first nh + nkv rows of head_dim of every token: one RoPE call rotates both
-            ops.rotate_half_(qkv[:, :, :nh + nkv].unsqueeze(2), pos, base=self.model.rope_base)
+            ops.rotate_half_(qkv[:, :, :nh + nkv].unsqueeze(2), pos, base=self.model.rope_base, inv_freq=self.rope_inv_freq)
             q_rows, k_rows, v_rows = qkv[0].split([nh, nkv, nkv], dim=1)  # [total, heads, hd]
             if starts is None:
                 atts = []
@@ -698,12 +716,18 @@ def synthetic_llama_tp(size_name, rank, world, bits=4, groupsize=128, vocab=3200
 
 def from_hf_quant_model(model, batch=1, max_seq=2048, **kw):
     """Build a decoder from an HF LlamaForCausalLM that went through the reference's load_quant recipe with this
-    repo's quant package (make_quant_linear -> load_state_dict -> make_quant_attn / make_quant_norm / make_fused_mlp)."""
+    repo's quant package (make_quant_linear -> load_state_dict -> make_quant_attn / make_quant_norm / make_fused_mlp).  The rotation (base, and
+    the frequency table of a llama3-scaled model) is the one the attention modules carry; a tied lm_head is not copied."""
     import quant
     L = []
-    rope_bases = {layer.self_attn.rope_base for layer in model.model.layers if isinstance(layer.self_attn, quant.QuantLlamaAttention)}
+    attns = [layer.self_attn for layer in model.model.layers if isinstance(layer.self_attn, quant.QuantLlamaAttention)]
+    rope_bases = {a.rope_base for a in attns}
     if len(rope_bases) > 1:
         raise ValueError(f'the attention layers disagree on the RoPE base: {sorted(rope_bases)}')
+    tables = {None if a.rope_inv_freq is None else tuple(a.rope_inv_freq.tolist()) for a in attns}
+    if len(tables) > 1:
+        raise ValueError('the attention layers disagree on the RoPE frequency table (rope_inv_freq)')
+    table = tables.pop() if tables else None
     for layer in model.model.layers:
         attn, mlp = layer.self_attn, layer.mlp
         if not isinstance(attn, quant.QuantLlamaAttention):
@@ -713,6 +737,9 @@ def from_hf_quant_model(model, batch=1, max_seq=2048, **kw):
             dict(qkv=attn.qkv_proj.weights(), o=attn.o_proj.weights(), gate=gate, up=up, down=mlp.down_proj.weights(),
                  input_norm=layer.input_layernorm.weight.data.half().contiguous(), post_norm=layer.post_attention_layernorm.weight.data.half().contiguous()))
     cfg = model.config
-    return LlamaDecoder(L, model.model.embed_tokens.weight.data.half(), model.model.norm.weight.data.half().contiguous(), model.lm_head.weight.data.half(),
+    embed = model.model.embed_tokens.weight.data.half()
+    tied = model.lm_head.weight.data_ptr() == model.model.embed_tokens.weight.data_ptr()  # LLaMA-3.2-3B (tie_word_embeddings)
+    return LlamaDecoder(L, embed, model.model.norm.weight.data.half().contiguous(), embed if tied else model.lm_head.weight.data.half(),
                         cfg.num_attention_heads, rms_eps=cfg.rms_norm_eps, rope_base=rope_bases.pop(), batch=batch, max_seq=max_seq,
-                        n_kv_heads=model.model.layers[0].self_attn.num_key_value_heads, **kw)  # (make_quant_attn read it from the config)
+                        n_kv_heads=model.model.layers[0].self_attn.num_key_value_heads,  # (make_quant_attn read it from the config)
+                        rope_scaling=None if table is None else torch.tensor(table, dtype=torch.float32), **kw)

@@ -12,6 +12,7 @@ torch is plumbing here (device memory, current stream); all arithmetic happens i
 """
 import ctypes
 import functools
+import math
 
 import torch
 
@@ -145,8 +146,60 @@ def fused_mlp(x, gate, up, bits, groupsize: int = 0):
     return out
 
 
-def rotate_half_(qk, position_ids, config=None, base: float = 10000.0):
-    """In-place RoPE on qk[bsz, seq, 2, heads, head_dim] (may be a strided view of the qkv output)."""
+LLAMA3_KEYS = ('factor', 'low_freq_factor', 'high_freq_factor', 'original_max_position_embeddings')
+
+
+def rope_inv_freq(base: float, head_dim: int, rope_scaling):
+    """The fp32 frequencies [head_dim / 2] of a scaled rotation, bit for bit the tensor HF builds for the same config
+    (transformers.modeling_rope_utils._compute_llama3_parameters, the same fp32 operations in the same order), or None for an unscaled one
+    (rope_scaling None, or its rope type 'default': the kernels then compute exp(i * -2 ln(base) / head_dim) themselves).
+
+    The llama3 rule (LLaMA-3.1 / 3.2 / 3.3): with inv_freq = 1 / base^(2i / head_dim) and wavelength 2 pi / inv_freq, a frequency whose
+    wavelength is below original_max_position_embeddings / high_freq_factor is kept, one above original_max_position_embeddings /
+    low_freq_factor is divided by factor, and one in between is blended: (1 - s) inv_freq / factor + s inv_freq with
+    s = (original_max_position_embeddings / wavelength - low_freq_factor) / (high_freq_factor - low_freq_factor).
+    rope_scaling must carry every key of LLAMA3_KEYS with factor > 0, 0 < low_freq_factor < high_freq_factor and
+    original_max_position_embeddings > 0; any other rope type, or a dict without those, raises ValueError."""
+    if rope_scaling is None:
+        return None
+    rope_type = rope_scaling.get('rope_type', rope_scaling.get('type', 'default'))
+    if rope_type == 'default':
+        return None
+    if rope_type != 'llama3':
+        raise ValueError(f"RoPE type {rope_type!r} is not supported: only 'default' and 'llama3' rotary embeddings are computed")
+    missing = [k for k in LLAMA3_KEYS if rope_scaling.get(k) is None]
+    if missing:
+        raise ValueError(f'llama3 RoPE scaling needs {", ".join(missing)}')
+    if not all(isinstance(rope_scaling[k], (int, float)) and not isinstance(rope_scaling[k], bool) for k in LLAMA3_KEYS):
+        raise ValueError(f'llama3 RoPE scaling: {", ".join(LLAMA3_KEYS)} must be numbers, got {rope_scaling}')
+    factor, low, high, old_context = (float(rope_scaling[k]) for k in LLAMA3_KEYS)
+    if not all(math.isfinite(v) for v in (factor, low, high, old_context, float(base))):
+        raise ValueError(f'llama3 RoPE scaling: every value must be finite, got {rope_scaling} at base {base}')
+    if not (factor > 0 and 0 < low < high and old_context > 0 and base > 0):
+        raise ValueError(f'llama3 RoPE scaling needs factor > 0, 0 < low_freq_factor < high_freq_factor and original_max_position_embeddings > 0 '
+                         f'(and base > 0), got {rope_scaling} at base {base}')
+    if head_dim % 2 or head_dim < 2:
+        raise ValueError(f'head_dim must be a positive even number, got {head_dim}')
+    # HF keeps original_max_position_embeddings as the config holds it (an int in every published config); its operands are restated as such
+    old_context = rope_scaling['original_max_position_embeddings']
+    inv_freq = 1.0 / (float(base)**(torch.arange(0, head_dim, 2, dtype=torch.int64).to(dtype=torch.float) / head_dim))
+    wavelen = 2 * math.pi / inv_freq
+    scaled = torch.where(wavelen > old_context / rope_scaling['low_freq_factor'], inv_freq / rope_scaling['factor'], inv_freq)
+    smooth = (old_context / wavelen - rope_scaling['low_freq_factor']) / (rope_scaling['high_freq_factor'] - rope_scaling['low_freq_factor'])
+    smoothed = (1 - smooth) * scaled / rope_scaling['factor'] + smooth * scaled
+    medium = ~(wavelen < old_context / rope_scaling['high_freq_factor']) * ~(wavelen > old_context / rope_scaling['low_freq_factor'])
+    return torch.where(medium, smoothed, scaled).contiguous()
+
+
+def _host_table(inv_freq):
+    """A frequency table (tensor or sequence, [head_dim / 2]) as the C array the ABI reads on the host."""
+    vals = inv_freq.detach().to('cpu', torch.float32).reshape(-1).tolist() if isinstance(inv_freq, torch.Tensor) else [float(v) for v in inv_freq]
+    return (ctypes.c_float * len(vals))(*vals)
+
+
+def rotate_half_(qk, position_ids, config=None, base: float = 10000.0, inv_freq=None):
+    """In-place RoPE on qk[bsz, seq, 2, heads, head_dim] (may be a strided view of the qkv output).  inv_freq: the fp32 frequencies
+    [head_dim / 2] of a scaled rotation (rope_inv_freq; gptq_rope_inplace_freq), which replace the unscaled rule at `base`."""
     _require_cuda(qk, position_ids)
     batch_size, seq_len, qandk, num_heads, head_dim = qk.shape
     # same argument checks as the reference (quant/fused_attn.py:69-74)
@@ -159,10 +212,17 @@ def rotate_half_(qk, position_ids, config=None, base: float = 10000.0):
         raise ValueError('qk must be float16')
     if position_ids.dtype != torch.int64:
         position_ids = position_ids.long()
+    if inv_freq is not None and len(inv_freq) != head_dim // 2:
+        raise ValueError(f'inv_freq has {len(inv_freq)} entries, head_dim {head_dim} needs {head_dim // 2}')
     with torch.cuda.device(qk.device):
-        check(
-            lib.gptq_rope_inplace(qk.data_ptr(), qk.stride(1), position_ids.data_ptr(), position_ids.stride(0), batch_size, seq_len, qandk * num_heads,
-                                  head_dim, float(base), _stream(qk)))
+        if inv_freq is None:
+            check(
+                lib.gptq_rope_inplace(qk.data_ptr(), qk.stride(1), position_ids.data_ptr(), position_ids.stride(0), batch_size, seq_len, qandk * num_heads,
+                                      head_dim, float(base), _stream(qk)))
+        else:
+            check(
+                lib.gptq_rope_inplace_freq(qk.data_ptr(), qk.stride(1), position_ids.data_ptr(), position_ids.stride(0), batch_size, seq_len,
+                                           qandk * num_heads, head_dim, _host_table(inv_freq), _stream(qk)))
 
 
 def rmsnorm(x, weight, eps: float):

@@ -26,10 +26,9 @@ def triton_rotate_half_(qk, position_ids, config=None):
 
 
 def rope_base_from_config(config):
-    """The RoPE base (theta) an HF LLaMA config asks for: rope_parameters['rope_theta'] (transformers >= 5), else rope_theta
-    (transformers 4.31 - 4.x), else 10000.  The kernels rotate by theta^(-2i/d) * pos on integer positions only, so a config
-    whose rope type is anything but 'default' (linear, dynamic, yarn, llama3, ...) raises ValueError instead of decoding
-    as if it were unscaled."""
+    """The base of an unscaled rotation: the RoPE base (theta) an HF LLaMA config asks for, rope_parameters['rope_theta'] (transformers >= 5),
+    else rope_theta (transformers 4.31 - 4.x), else 10000.  A config whose rope type is anything but 'default' (linear, dynamic, yarn,
+    llama3, ...) raises ValueError instead of decoding as if it were unscaled; rope_from_config also serves llama3."""
     params = getattr(config, 'rope_parameters', None)
     if params is None:  # transformers 4.x: rope_theta beside an optional rope_scaling dict ('type' before 4.45, 'rope_type' after)
         scaling = getattr(config, 'rope_scaling', None) or {}
@@ -39,6 +38,30 @@ def rope_base_from_config(config):
         raise ValueError(f"RoPE type {rope_type!r} is not supported: only 'default' (unscaled) rotary embeddings are computed")
     base = params.get('rope_theta')
     return 10000.0 if base is None else float(base)
+
+
+def _rope_params(config):
+    """(rope_theta or None, the rope parameters dict) of an HF config under its three conventions: rope_parameters (transformers >= 5), or
+    rope_theta beside an optional rope_scaling dict keyed by 'rope_type' (4.45 - 4.x) or by 'type' (before 4.45)."""
+    params = getattr(config, 'rope_parameters', None)
+    if params is None:
+        return getattr(config, 'rope_theta', None), dict(getattr(config, 'rope_scaling', None) or {})
+    return params.get('rope_theta'), dict(params)
+
+
+def rope_from_config(config):
+    """(base, inv_freq) of the rotation an HF LLaMA config asks for.  inv_freq is None for the 'default' (unscaled) rope type, which the
+    kernels compute from the base; for 'llama3' (LLaMA-3.1 / 3.2 / 3.3) it is the fp32 table [head_dim / 2] HF builds (ops.rope_inv_freq),
+    and the base is the one the table was built from.  Every other rope type (linear, dynamic, yarn, ...) raises ValueError."""
+    theta, params = _rope_params(config)
+    base = 10000.0 if theta is None else float(theta)
+    rope_type = params.get('rope_type', params.get('type', 'default'))
+    if rope_type == 'default':
+        return base, None
+    if rope_type != 'llama3':
+        raise ValueError(f"RoPE type {rope_type!r} is not supported: only 'default' and 'llama3' rotary embeddings are computed")
+    head_dim = getattr(config, 'head_dim', None) or config.hidden_size // config.num_attention_heads
+    return base, ops.rope_inv_freq(base, head_dim, params)
 
 
 def kv_heads_from_config(config):
@@ -52,7 +75,8 @@ class QuantLlamaAttention(nn.Module):
     reads K/V head h / (num_heads / num_key_value_heads)).  qkv_proj is the fused q | k | v projection of num_heads + 2 num_key_value_heads
     heads; the cache holds num_key_value_heads heads."""
 
-    def __init__(self, hidden_size, num_heads, qkv_proj, o_proj, layer_idx=None, rope_base=10000.0, num_key_value_heads=None):
+    def __init__(self, hidden_size, num_heads, qkv_proj, o_proj, layer_idx=None, rope_base=10000.0, num_key_value_heads=None, rope_inv_freq=None):
+        """rope_inv_freq: the fp32 frequencies [head_dim / 2] of a scaled rotation (rope_from_config), None for the unscaled one at rope_base."""
         super().__init__()
         self.hidden_size = hidden_size
         self.num_heads = num_heads
@@ -67,6 +91,9 @@ class QuantLlamaAttention(nn.Module):
             raise ValueError(f'num_key_value_heads ({self.num_key_value_heads}) must divide num_heads ({num_heads})')
         self.qkv_proj = qkv_proj
         self.o_proj = o_proj
+        # a plain fp32 host tensor, not a registered buffer: the kernel reads the table on the host at every call, and module.half() or .cuda()
+        # would round it to fp16 or make each call a device-to-host copy
+        self.rope_inv_freq = None if rope_inv_freq is None else torch.as_tensor(rope_inv_freq, dtype=torch.float32, device='cpu').clone()
 
     def forward(self, hidden_states, past_key_value=None, attention_mask=None, position_ids=None, output_attentions=False, use_cache=False,
                 past_key_values=None, position_embeddings=None, **kwargs):
@@ -87,7 +114,8 @@ class QuantLlamaAttention(nn.Module):
         nh, nkv = self.num_heads, self.num_key_value_heads
         qkv_states = self.qkv_proj(hidden_states)
         qkv_states = qkv_states.view(bsz, q_len, nh + 2 * nkv, self.head_dim)  # q | k | v heads
-        ops.rotate_half_(qkv_states[:, :, :nh + nkv].unsqueeze(2), position_ids, base=self.rope_base)  # q and k rotated in place (:126)
+        scaled = {} if self.rope_inv_freq is None else dict(inv_freq=self.rope_inv_freq)
+        ops.rotate_half_(qkv_states[:, :, :nh + nkv].unsqueeze(2), position_ids, base=self.rope_base, **scaled)  # q and k rotated in place (:126)
 
         query_states, key_states, value_states = (t.transpose(1, 2) for t in torch.split(qkv_states, [nh, nkv, nkv], dim=2))
         del qkv_states
@@ -144,7 +172,7 @@ def fuse_qkv(q_proj, k_proj, v_proj):
 
 def make_quant_attn(model):
     """Replace all LlamaAttention modules with QuantLlamaAttention modules, fusing the q, k, v projections (k and v are narrower than q under
-    grouped-query attention).  Only the 'default' RoPE type is accepted (rope_base_from_config)."""
+    grouped-query attention).  The 'default' and 'llama3' RoPE types are accepted (rope_from_config)."""
     if not LlamaAttention:
         return
     targets = [name for name, m in model.named_modules() if isinstance(m, LlamaAttention)]
@@ -156,11 +184,11 @@ def make_quant_attn(model):
         hidden_size = getattr(m, 'hidden_size', None) or cfg.hidden_size
         num_heads = getattr(m, 'num_heads', None) or cfg.num_attention_heads
         kv_heads = getattr(m, 'num_key_value_heads', None) or kv_heads_from_config(cfg if cfg is not None else model.config)
-        rope_base = rope_base_from_config(cfg if cfg is not None else model.config)
+        rope_base, inv_freq = rope_from_config(cfg if cfg is not None else model.config)
         qkv_layer = fuse_qkv(m.q_proj, m.k_proj, m.v_proj)
-        # the rotary embedding module is dropped: RoPE is computed in the kernel from position_ids and the config's base
+        # the rotary embedding module is dropped: RoPE is computed in the kernel from position_ids and the config's base or frequency table
         attn = QuantLlamaAttention(hidden_size, num_heads, qkv_layer, m.o_proj, layer_idx=getattr(m, 'layer_idx', None), rope_base=rope_base,
-                                   num_key_value_heads=kv_heads)
+                                   num_key_value_heads=kv_heads, rope_inv_freq=inv_freq)
         parent_name, _, child_name = name.rpartition('.')
         parent = model.get_submodule(parent_name) if parent_name else model
         setattr(parent, child_name, attn)

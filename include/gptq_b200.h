@@ -39,8 +39,9 @@ extern "C" {
 
 #define GPTQ_B200_ABI_VERSION 6 /* 2: act-order input gathers; 3: gptq_llama_persistent_scratch_offset; 4: tensor parallelism (gptq_llama_tp, gptq_ipc_*);
                                    5: persistent path at batch 2..8 ([batch][hidden] residual rows in the persistent region);
-                                   6: gptq_lm_head_logprob (scoring); gptq_cached_attention, gptq_sample_tokens and gptq_cached_attention_gqa
-                                   added later without a change to any existing struct or signature */
+                                   6: gptq_lm_head_logprob (scoring); gptq_cached_attention, gptq_sample_tokens, gptq_cached_attention_gqa,
+                                   gptq_rope_inplace_freq and gptq_llama_decode_step_rope added later without a change to any existing struct
+                                   or signature */
 
 typedef void* gptq_stream_t; /* cudaStream_t */
 
@@ -102,6 +103,14 @@ int gptq_qlinear_transpose_fwd(const void* g, int64_t ldg, const gptq_qweight* w
  * between batches; tokens = bsz*seq. */
 int gptq_rope_inplace(void* qk, int64_t token_stride, const int64_t* position_ids, int64_t pos_batch_stride, int bsz, int seq, int rows, int head_dim,
                       float base, gptq_stream_t stream);
+/* The same rotation with the frequencies of a scaled RoPE (LLaMA-3.1 / 3.2 / 3.3's llama3 rule, or any other table): pair i of a row at
+ * position p turns by the angle fp32(inv_freq[i] * (float)p), rounded once, through cosf / sinf, which is the angle HF computes from the same
+ * fp32 table.  inv_freq is a HOST array of head_dim / 2 floats, read during the call and copied into the launch parameters (a captured graph
+ * replays it; the array may be freed once the call returns).  It is required (GPTQ_ERR_NULL), each entry must be finite and > 0
+ * (GPTQ_ERR_SHAPE, checked before any CUDA call), and head_dim must be at most 128 (GPTQ_ERR_UNSUPPORTED).  Everything else as
+ * gptq_rope_inplace, whose unscaled rule is exp(i * -2 ln(base) / head_dim) in fp32. */
+int gptq_rope_inplace_freq(void* qk, int64_t token_stride, const int64_t* position_ids, int64_t pos_batch_stride, int bsz, int seq, int rows, int head_dim,
+                           const float* inv_freq, gptq_stream_t stream);
 
 /* y[M,N] = x * rsqrt(mean(x^2) + eps) * weight, fp32 math, fp16 store.
  * Replaces TritonLlamaRMSNorm.forward / rms_norm_fwd_fused (quant/triton_norm.py:50-67, :7-39). */
@@ -196,6 +205,12 @@ typedef struct gptq_llama_state {
 
 size_t gptq_llama_scratch_bytes(const gptq_llama_model* model, int batch, int max_seq);
 int gptq_llama_decode_step(const gptq_llama_model* model, const gptq_llama_state* state, gptq_stream_t stream);
+/* The decode step with a scaled RoPE: both engines rotate q and the appended k with the frequencies inv_freq, a HOST array of head_dim / 2
+ * (= 64) floats, under gptq_rope_inplace_freq's angle rule, so the step appends exactly the cache rows gptq_rope_inplace_freq writes at the
+ * same position.  model->rope_base is then unused.  NULL: model->rope_base's unscaled rule (gptq_llama_decode_step is this call with NULL).
+ * A table entry that is not finite and > 0 gives GPTQ_ERR_SHAPE before any CUDA call.  The table is copied into the launch parameters, so a
+ * captured step replays it.  gptq_llama_decode_launches does not depend on the rotation. */
+int gptq_llama_decode_step_rope(const gptq_llama_model* model, const gptq_llama_state* state, const float* inv_freq, gptq_stream_t stream);
 /* Number of kernels one gptq_llama_decode_step launches for this model/state: 1 when the persistent single-kernel
  * path applies (batch 1 to 8, every layer int4 in kernel form -- act-order layers with input gathers included -- and a shape
  * whose staging buffers fit the device's shared memory at this batch; tensor parallelism at batch 1 only), else the
