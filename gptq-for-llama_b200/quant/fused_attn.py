@@ -25,37 +25,34 @@ def triton_rotate_half_(qk, position_ids, config=None):
     ops.rotate_half_(qk, position_ids)
 
 
-def rope_base_from_config(config):
-    """The base of an unscaled rotation: the RoPE base (theta) an HF LLaMA config asks for, rope_parameters['rope_theta'] (transformers >= 5),
-    else rope_theta (transformers 4.31 - 4.x), else 10000.  A config whose rope type is anything but 'default' (linear, dynamic, yarn,
-    llama3, ...) raises ValueError instead of decoding as if it were unscaled; rope_from_config also serves llama3."""
-    params = getattr(config, 'rope_parameters', None)
-    if params is None:  # transformers 4.x: rope_theta beside an optional rope_scaling dict ('type' before 4.45, 'rope_type' after)
-        scaling = getattr(config, 'rope_scaling', None) or {}
-        params = {'rope_theta': getattr(config, 'rope_theta', None), 'rope_type': scaling.get('rope_type', scaling.get('type', 'default'))}
-    rope_type = params.get('rope_type', 'default')
-    if rope_type != 'default':
-        raise ValueError(f"RoPE type {rope_type!r} is not supported: only 'default' (unscaled) rotary embeddings are computed")
-    base = params.get('rope_theta')
-    return 10000.0 if base is None else float(base)
-
-
-def _rope_params(config):
-    """(rope_theta or None, the rope parameters dict) of an HF config under its three conventions: rope_parameters (transformers >= 5), or
-    rope_theta beside an optional rope_scaling dict keyed by 'rope_type' (4.45 - 4.x) or by 'type' (before 4.45)."""
+def _rope_config(config):
+    """(base, rope type, rope parameters dict) of an HF LLaMA config under its three conventions: rope_parameters (transformers >= 5), or
+    rope_theta beside an optional rope_scaling dict keyed by 'rope_type' (4.45 - 4.x) or by 'type' (before 4.45).  The base defaults to
+    10000 and the rope type to 'default'."""
     params = getattr(config, 'rope_parameters', None)
     if params is None:
-        return getattr(config, 'rope_theta', None), dict(getattr(config, 'rope_scaling', None) or {})
-    return params.get('rope_theta'), dict(params)
+        theta, params = getattr(config, 'rope_theta', None), dict(getattr(config, 'rope_scaling', None) or {})
+    else:
+        theta, params = params.get('rope_theta'), dict(params)
+    return 10000.0 if theta is None else float(theta), params.get('rope_type', params.get('type', 'default')), params
+
+
+def rope_base_from_config(config):
+    """The base of an unscaled rotation: the RoPE base (theta) an HF LLaMA config asks for (_rope_config).  A config whose rope type is
+    anything but 'default' (linear, dynamic, yarn, llama3, ...) raises ValueError instead of decoding as if it were unscaled;
+    rope_from_config also serves llama3."""
+    base, rope_type, _ = _rope_config(config)
+    if rope_type != 'default':
+        raise ValueError(f"RoPE type {rope_type!r} is not supported: only 'default' (unscaled) rotary embeddings are computed")
+    return base
 
 
 def rope_from_config(config):
-    """(base, inv_freq) of the rotation an HF LLaMA config asks for.  inv_freq is None for the 'default' (unscaled) rope type, which the
-    kernels compute from the base; for 'llama3' (LLaMA-3.1 / 3.2 / 3.3) it is the fp32 table [head_dim / 2] HF builds (ops.rope_inv_freq),
-    and the base is the one the table was built from.  Every other rope type (linear, dynamic, yarn, ...) raises ValueError."""
-    theta, params = _rope_params(config)
-    base = 10000.0 if theta is None else float(theta)
-    rope_type = params.get('rope_type', params.get('type', 'default'))
+    """(base, inv_freq) of the rotation an HF LLaMA config asks for (_rope_config).  inv_freq is None for the 'default' (unscaled) rope type,
+    which the kernels compute from the base; for 'llama3' (LLaMA-3.1 / 3.2 / 3.3) it is the fp32 table [head_dim / 2] HF builds
+    (ops.rope_inv_freq), and the base is the one the table was built from.  Every other rope type (linear, dynamic, yarn, ...) raises
+    ValueError."""
+    base, rope_type, params = _rope_config(config)
     if rope_type == 'default':
         return base, None
     if rope_type != 'llama3':

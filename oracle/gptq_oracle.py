@@ -177,17 +177,20 @@ def fused_mlp_fwd(x, gate, up, bits: int) -> torch.Tensor:
     return c.reshape(x.shape[:-1] + (c.shape[-1], ))
 
 
-def rope_inplace(qk: torch.Tensor, position_ids: torch.Tensor, base: float = 10000.0) -> None:
+def rope_inplace(qk: torch.Tensor, position_ids: torch.Tensor, base: float = 10000.0, inv_freq=None) -> None:
     """``rotate_half_kernel`` / ``triton_rotate_half_`` (quant/fused_attn.py:8-93), in place.
 
     qk: fp16 ``[bsz, seq, 2, heads, head_dim]`` (a view is fine).  :43 ``freq_i =
     exp(i * INV_BASE) * pos`` with INV_BASE = -2 ln(base)/head_dim (:91), fp32 cos/sin (:44-45);
     x' = x cos - y sin, y' = x sin + y cos with y at +head_dim/2 (:52-57), fp16 store.
+    inv_freq: the fp32 frequency table ``[head_dim/2]`` of a scaled rotation (no counterpart in the
+    reference), which replaces ``exp(i * INV_BASE)``: ``freq_i = fp32(inv_freq[i] * pos)``.
     """
     bsz, seq, two, heads, hd = qk.shape
     half = hd // 2
-    inv_base = np.float32(-2.0 * math.log(base) / hd)
-    freq = torch.exp(torch.arange(half, dtype=torch.float32) * inv_base)[None, None, :] * position_ids[:, :, None].float()
+    if inv_freq is None:
+        inv_freq = torch.exp(torch.arange(half, dtype=torch.float32) * np.float32(-2.0 * math.log(base) / hd))
+    freq = torch.as_tensor(inv_freq, dtype=torch.float32).cpu()[None, None, :] * position_ids[:, :, None].float()
     cos = torch.cos(freq)[:, :, None, None, :]
     sin = torch.sin(freq)[:, :, None, None, :]
     x = qk[..., :half].float()

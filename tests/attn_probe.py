@@ -27,7 +27,7 @@ import math
 import numpy as np
 import torch
 
-from gpu_util import ulp16
+from gpu_util import fp16_ulp_distance, report, ulp16
 
 HD = 128      # head dim
 UNIT = 32     # keys per work unit of the persistent kernel (kKeysPerUnit)
@@ -146,12 +146,14 @@ def resid_buffers(dec):
 
 
 class Probe:
-    """The probe model on a LlamaDecoder (1 layer, n_kv_heads K/V heads: default engine.kv_heads(size)).  learn() is pass 1 of a (tokens,
+    """The probe model on a LlamaDecoder (1 layer, n_kv_heads K/V heads: default engine.kv_heads(size); RoPE at rope_base, or with the
+    frequency table of rope_scaling, LlamaDecoder's argument).  learn() is pass 1 of a (tokens,
     positions) step: it reads the appended K and V rows of every K/V head (k_new, v_new) and from them each query head's rotated q (q_rot:
     the K row of its K/V head masked to its pairs); run() is pass 2: it plants the cache, poisons the rows at and after each position with
     NaN, steps, checks that exactly row pos of every K/V head was written, bit-identical to pass 1, and returns (x_in, x_out) [B, H] fp16."""
 
-    def __init__(self, size, batch=1, max_seq=2048, act_order=False, vocab=64, seed=0, lm_head=None, rope_base=10000.0, n_kv_heads=None):
+    def __init__(self, size, batch=1, max_seq=2048, act_order=False, vocab=64, seed=0, lm_head=None, rope_base=10000.0, n_kv_heads=None,
+                 rope_scaling=None):
         from gptq_b200 import engine
         H, I, _, nh = engine.LLAMA_SHAPES[size]
         nkv = engine.kv_heads(size) if n_kv_heads is None else n_kv_heads
@@ -167,8 +169,9 @@ class Probe:
         if lm_head is None:
             lm_head = (torch.randn(vocab, H, generator=torch.Generator().manual_seed(seed + 2)) * 0.02).half()
         self.dec = engine.LlamaDecoder([L], embed, torch.ones(H, dtype=torch.float16, device=dev), lm_head.to(dev), nh, rms_eps=0.0, batch=batch,
-                                       max_seq=max_seq, rope_base=rope_base, n_kv_heads=nkv)
-        self.H, self.nh, self.nkv, self.g, self.B, self.max_seq, self.rope_base = H, nh, nkv, nh // nkv, batch, max_seq, rope_base
+                                       max_seq=max_seq, rope_base=rope_base, n_kv_heads=nkv, rope_scaling=rope_scaling)
+        self.H, self.nh, self.nkv, self.g, self.B, self.max_seq = H, nh, nkv, nh // nkv, batch, max_seq
+        self.rope = dict(base=rope_base, inv_freq=self.dec.rope_inv_freq)  # the rotation: O.rope_inplace, ops.rotate_half_, check_rope_row
         self.mask = pair_mask(self.w['support']).to(dev)
         self.persistent = self.dec.launches_per_step() == 1
         self.nb = 2 * torch.cuda.get_device_properties(dev).multi_processor_count
@@ -424,18 +427,131 @@ def emulate_persistent(q, K, V, ranges):
 
 
 # ----------------------------------------------------------------------------- RoPE of the appended K row
-def check_rope_row(k_row, k_exact, pos, rope_base):
-    """The appended K rows [nkv, 128] (fp16) against fp64 RoPE of the exact k [nkv * 128] (exact_qv) at base rope_base, the angle computed in fp32 as the
-    reference formula does (quant/fused_attn.py:43): within 1 ulp16, plus a 4-ulp difference in the fp32 angle and in cos / sin.  Returns the
-    worst |err| / bound."""
+def rope_angles32(pos, base=10000.0, inv_freq=None):
+    """The fp32 RoPE angles [64] at pos, as the kernels and O.rope_inplace compute them: fp32(f_i * pos), where f_i is the table's
+    inv_freq[i], else fp32 exp(i * fp32(-2 ln(base) / 128)) (quant/fused_attn.py:43)."""
     f = np.float32
-    inv_base = f(-2.0 * math.log(rope_base) / HD)
-    th = (np.exp(np.arange(64, dtype=f) * inv_base).astype(f) * f(pos)).astype(np.float64)
+    freq = np.exp(np.arange(64, dtype=f) * f(-2.0 * math.log(base) / HD)).astype(f) if inv_freq is None else np.asarray(inv_freq, dtype=f)
+    return (freq * f(pos)).astype(f)
+
+
+def check_rope_row(k_row, k_exact, pos, base=10000.0, inv_freq=None):
+    """The rotated rows [rows, 128] (fp16; the appended K rows [nkv, 128]) against fp64 RoPE of the exact rows [rows * 128] (exact_qv) at
+    the fp32 angles of rope_angles32 (the rotation at `base`, or the table's): within 1 ulp16, plus a 4-ulp difference in the fp32 angle and
+    in cos / sin.  Returns the worst |err| / bound."""
+    th = rope_angles32(pos, base, inv_freq).astype(np.float64)
     x = k_exact.view(-1, HD)[:, :64].numpy()
     y = k_exact.view(-1, HD)[:, 64:].numpy()
     c, s = np.cos(th), np.sin(th)
     ref = torch.from_numpy(np.concatenate([x * c - y * s, x * s + y * c], 1))
-    dth = 4 * np.spacing(th.astype(f)).astype(np.float64) + 4 * U24
+    dth = 4 * np.spacing(th.astype(np.float32)).astype(np.float64) + 4 * U24
     slack = torch.from_numpy(np.tile((np.abs(x) + np.abs(y)) * dth, 2))
     bound = ulp16(ref) + slack
     return ((k_row.double().cpu() - ref).abs() / bound).max().item()
+
+
+def prefill_row(probe, tok, pos):
+    """The K rows [nkv, 128] of position pos as the prefill writes them: the exact k of the probe (exact_qv) rotated by ops.rotate_half_
+    with the probe's rotation."""
+    from gptq_b200 import ops
+    k = exact_qv(probe.w, probe.dec.embed[tok])[1].half().view(1, 1, 1, probe.nkv, HD).cuda()
+    ops.rotate_half_(k, torch.tensor([[pos]], device='cuda'), **probe.rope)
+    return k.view(probe.nkv, HD)
+
+
+# ----------------------------------------------------------------------------- GPU sweeps of the probe
+class Worst:
+    def __init__(self, what):
+        self.what, self.ratio, self.where = what, 0.0, ''
+
+    def update(self, ratio_t, where):
+        r = ratio_t.max().item() if torch.is_tensor(ratio_t) else float(ratio_t)
+        if torch.is_tensor(ratio_t) and not r <= 1:
+            idx = [int(i) for i in torch.nonzero(~(ratio_t <= 1))[0]]
+            where = f'{where} head {idx[0]} dim {idx[1]}'
+        if not r <= self.ratio:
+            self.ratio, self.where = r, where
+
+    def done(self):
+        report(self.ratio, f'{self.what} (worst at {self.where})' if self.ratio > 1 else self.what)
+
+
+def anchors(probe, toks, positions, gen, what):
+    """Equal scores and zero-sum values (pos 0: the lone new key): x_out must be x_in (fp16(x_in + v_new) at pos 0) bit for bit."""
+    plants = [(k[:, None, :].expand(-1, p, -1).contiguous(), zero_sum_values(v, p, gen)) for k, v, p in zip(probe.k_new, probe.v_new, positions)]
+    x_in, x_out = probe.run(toks, positions, plants)
+    for b, p in enumerate(positions):
+        want = x_in[b] if p > 0 else (x_in[b].double() + probe.v_new[b].repeat_interleave(probe.g, 0).reshape(-1).double()).half()
+        if not torch.equal(x_out[b], want):
+            d = fp16_ulp_distance(x_out[b], want)
+            i = int(torch.nonzero(d)[0])
+            raise AssertionError(f'{what} seq {b} pos {p}: {int((d > 0).sum())} elements off, up to {int(d.max())} ulp; first at head {i // HD} '
+                                 f'dim {i % HD}: {x_out[b, i].item()} vs {want[i].item()}')
+
+
+def bounded(probe, toks, positions, plants, worst, what):
+    x_in, x_out = probe.run(toks, positions, plants)
+    for b, p in enumerate(positions):
+        K = torch.cat([plants[b][0], probe.k_new[b][:, None, :]], 1).repeat_interleave(probe.g, 0)
+        V = torch.cat([plants[b][1], probe.v_new[b][:, None, :]], 1).repeat_interleave(probe.g, 0)
+        att, E = softmax_ref(probe.q_rot[b], K, V)
+        x_ref = x_in[b].double().view(-1, HD) + att
+        out = x_out[b].double().view(-1, HD)
+        assert torch.isfinite(out).all(), f'{what} seq {b} pos {p}: non-finite output'
+        worst.update((out - x_ref).abs() / x_bound(att, x_ref, E), f'{what} seq {b} pos {p}')
+
+
+def heavy_passes(probe, positions, rotate=None):
+    """Heavy key sets per pass: [pass][sequence][head] -> keys.  rotate = offset: one pass, the edges dealt from that offset."""
+    ranges = team_ranges(positions, probe.nh, probe.nb) if probe.persistent else {}
+    per_seq = []
+    for b, p in enumerate(positions):
+        edges = sorted(set().union(*[edge_keys(p, ranges.get((b, h), ())) for h in range(probe.nh)]))
+        deal = deal_heavy(edges, probe.nh, offset=rotate or 0)
+        per_seq.append(deal[:1] if rotate is not None else deal)
+    n = max(len(d) for d in per_seq)
+    return [[d[j % len(d)] for d in per_seq] for j in range(n)]
+
+
+def rotation_passes(nh, T):
+    """8 passes of nh heads x 8 keys in which every key t < T is heavy once: pass t % 8, head (t // 8) % nh."""
+    out = [[[] for _ in range(nh)] for _ in range(8)]
+    for t in range(T):
+        out[t % 8][(t // 8) % nh].append(t)
+    return out
+
+
+def sweep(probe, position_sets, profiles, gen, worst, rope, toks=lambda i, b: 7 * i + 3 * b, rotate_heavy=False, full_rotation=()):
+    """Position set i of `position_sets` with the tokens toks(i, b) % vocab: pass 1 (probe.learn), the appended K rows against fp64 RoPE
+    (check_rope_row) and bit for bit against the prefill's rotation (prefill_row), the bit-exact anchors, then each profile, bounded."""
+    vocab = probe.dec.vocab
+    for i, positions in enumerate(position_sets):
+        tk = [toks(i, b) % vocab for b in range(probe.B)]
+        what = f'toks {tk} positions {positions}'
+        probe.learn(tk, positions)
+        for b, p in enumerate(positions):  # the appended K rows (q_rot, masked) against fp64 RoPE of the exact k and the prefill's rotation
+            k_exact = exact_qv(probe.w, probe.dec.embed[tk[b]])[1]
+            rope.update(check_rope_row(probe.k_new[b], k_exact, p, **probe.rope), f'{what} seq {b}')
+            assert torch.equal(probe.k_new[b], prefill_row(probe, tk[b], p)), f'{what} seq {b}: the step and the prefill rotate differently'
+        anchors(probe, tk, positions, gen, what)
+        for kind in profiles:
+            if kind == 'heavy':
+                passes = heavy_passes(probe, positions, rotate=(i * 8 * probe.nh) if rotate_heavy else None)
+                if len(positions) == 1 and positions[0] in full_rotation:
+                    passes += [[r] for r in rotation_passes(probe.nh, positions[0])]
+                for heavy in passes:
+                    plants = [profile('heavy', q, p, gen, heavy=hv, g=probe.g) for q, p, hv in zip(probe.q_rot, positions, heavy)]
+                    bounded(probe, tk, positions, plants, worst[kind], what + ' heavy')
+            else:
+                plants = [profile(kind, q, p, gen, g=probe.g) for q, p in zip(probe.q_rot, positions)]
+                bounded(probe, tk, positions, plants, worst[kind], f'{what} {kind}')
+
+
+def run_sweeps(probe, name, position_sets, profiles=PROFILES, seed=1234, **kw):
+    """sweep over every position set, with the worst |err| / bound of each profile and of the RoPE rows printed (pytest -s)."""
+    gen = torch.Generator(device='cuda:0').manual_seed(seed)
+    worst = {k: Worst(f'{name} {k}') for k in profiles}
+    rope = Worst(f'{name} appended K row vs fp64 RoPE')
+    sweep(probe, position_sets, profiles, gen, worst, rope, **kw)
+    for w in list(worst.values()) + [rope]:
+        w.done()

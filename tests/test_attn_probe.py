@@ -50,9 +50,9 @@ def test_qkv_products_are_exact_in_any_order(H, act, nkv):
 
 def _rope32(x, pos, base):
     """float32 RoPE of rows x [n, 128] rounded to fp16, in the kernels' operation order (x c - y s, x s + y c, two roundings per term) and
-    with the angle of check_rope_row."""
+    with the angle of check_rope_row (rope_angles32)."""
     f = np.float32
-    th = (np.exp(np.arange(64, dtype=f) * f(-2.0 * np.log(base) / P.HD)).astype(f) * f(pos)).astype(f)
+    th = P.rope_angles32(pos, base)
     c, s = np.cos(th).astype(f), np.sin(th).astype(f)
     a, b = x[:, :64].numpy().astype(f), x[:, 64:].numpy().astype(f)
     return torch.from_numpy(np.concatenate([a * c - b * s, a * s + b * c], 1).astype(np.float16))

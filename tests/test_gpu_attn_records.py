@@ -7,8 +7,7 @@ gptq_llama_persistent_scratch_offset(); _mega_layout follows mega_scratch in csr
 import pytest
 import torch
 
-from llama_oracle import LlamaOracle
-from gpu_util import assert_rel_close
+from llama_oracle import LlamaOracle, check_steps
 
 pytestmark = pytest.mark.gpu
 
@@ -125,9 +124,4 @@ def test_fresh_engine_first_step_matches_oracle():
     dec = engine.synthetic_llama('tiny256', bits=4, groupsize=64, vocab=512, seed=5, max_seq=64, use_graph=False)
     assert dec.launches_per_step() == 1 and _counter(dec) == (0, 0)
     toks = [3, 9, 27]
-    refs = LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0).logits(toks)
-    for pos, tok in enumerate(toks):
-        dec.set_input(tok, pos)
-        dec.step()
-        torch.cuda.synchronize()
-        assert_rel_close(dec.logits[0], refs[pos], rel=2e-2, what=f'pos {pos}')
+    check_steps(dec, LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0), [toks], lambda k, b, pos: f'pos {pos}')

@@ -4,7 +4,7 @@ import pytest
 import torch
 
 from gpu_util import assert_rel_close
-from llama_oracle import LlamaOracle
+from llama_oracle import LlamaOracle, check_steps
 
 pytestmark = pytest.mark.gpu
 
@@ -56,15 +56,7 @@ def test_batch_columns_match_oracle(size, bits, act, batch):
     assert dec.launches_per_step() == 1
     assert (dec.perms[0]['qkv'] is not None) == act
     toks = torch.randint(0, 512, (batch, 6), generator=torch.Generator().manual_seed(batch)).tolist()
-    oracle = LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0)
-    refs = [oracle.logits(t) for t in toks]
-    for pos in range(6):
-        dec.set_input([t[pos] for t in toks], pos)
-        dec.step()
-        torch.cuda.synchronize()
-        for b in range(batch):
-            assert_rel_close(dec.logits[b], refs[b][pos], rel=2e-2, what=f'{size} bits={bits} act={act} B={batch} seq={b} pos={pos}')
-            assert int(dec.next_tokens[b]) == int(dec.logits[b].float().argmax())
+    check_steps(dec, LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0), toks, lambda k, b, pos: f'{size} bits={bits} act={act} B={batch} seq={b} pos={pos}')
 
 
 @pytest.mark.parametrize('size,bits,act,positions', [('7b', 4, False, [0, 31, 32, 255, 256, 1023, 2046, 2047]), ('13b', 3, True, [0, 255, 1023, 2047])])

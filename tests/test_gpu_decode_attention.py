@@ -8,6 +8,8 @@ v, identity o_proj, zero MLP: the residual after a step is fp16(x_in + fp16(att)
 * Bounded profiles (attn_probe.PROFILES): x_out against x_in + att of a float64 softmax over the kernel's own q_rot, K and V rows, per
   element within attn_probe.x_bound.  Heavy keys are put at 0, at the last planted key, on both sides of every unit and split edge and at
   both ends of every team range; at the longest 7B context the heavy sets rotate until every key has been heavy in some head.
+* The appended K row of every step against fp64 RoPE (attn_probe.check_rope_row) and bit for bit against the prefill's rotation of the
+  same exact k (attn_probe.prefill_row).
 * The cache rows at and after each position hold NaN before the step: the kernel must write the new row and never read a later one.  After
   the step the planted rows are bitwise unchanged and the later rows still NaN: exactly row pos of every K/V head was written.
 * Grouped-query shapes (tiny-gqa*, LLaMA-3-8B, LLaMA-2-70B, CodeLlama-34B, and one K/V head at 7B and tiny): the query heads of a group
@@ -20,102 +22,10 @@ import pytest
 import torch
 
 import attn_probe as P
-from gpu_util import check_fp64_bound, fp16_ulp_distance, report
+from attn_probe import run_sweeps
+from gpu_util import check_fp64_bound
 
 pytestmark = pytest.mark.gpu
-
-
-class Worst:
-    def __init__(self, what):
-        self.what, self.ratio, self.where = what, 0.0, ''
-
-    def update(self, ratio_t, where):
-        r = ratio_t.max().item() if torch.is_tensor(ratio_t) else float(ratio_t)
-        if torch.is_tensor(ratio_t) and not r <= 1:
-            idx = [int(i) for i in torch.nonzero(~(ratio_t <= 1))[0]]
-            where = f'{where} head {idx[0]} dim {idx[1]}'
-        if not r <= self.ratio:
-            self.ratio, self.where = r, where
-
-    def done(self):
-        report(self.ratio, f'{self.what} (worst at {self.where})' if self.ratio > 1 else self.what)
-
-
-def anchors(probe, toks, positions, gen, what):
-    """Equal scores and zero-sum values (pos 0: the lone new key): x_out must be x_in (fp16(x_in + v_new) at pos 0) bit for bit."""
-    plants = [(k[:, None, :].expand(-1, p, -1).contiguous(), P.zero_sum_values(v, p, gen)) for k, v, p in zip(probe.k_new, probe.v_new, positions)]
-    x_in, x_out = probe.run(toks, positions, plants)
-    for b, p in enumerate(positions):
-        want = x_in[b] if p > 0 else (x_in[b].double() + probe.v_new[b].repeat_interleave(probe.g, 0).reshape(-1).double()).half()
-        if not torch.equal(x_out[b], want):
-            d = fp16_ulp_distance(x_out[b], want)
-            i = int(torch.nonzero(d)[0])
-            raise AssertionError(f'{what} seq {b} pos {p}: {int((d > 0).sum())} elements off, up to {int(d.max())} ulp; first at head {i // P.HD} '
-                                 f'dim {i % P.HD}: {x_out[b, i].item()} vs {want[i].item()}')
-
-
-def bounded(probe, toks, positions, plants, worst, what):
-    x_in, x_out = probe.run(toks, positions, plants)
-    for b, p in enumerate(positions):
-        K = torch.cat([plants[b][0], probe.k_new[b][:, None, :]], 1).repeat_interleave(probe.g, 0)
-        V = torch.cat([plants[b][1], probe.v_new[b][:, None, :]], 1).repeat_interleave(probe.g, 0)
-        att, E = P.softmax_ref(probe.q_rot[b], K, V)
-        x_ref = x_in[b].double().view(-1, P.HD) + att
-        out = x_out[b].double().view(-1, P.HD)
-        assert torch.isfinite(out).all(), f'{what} seq {b} pos {p}: non-finite output'
-        worst.update((out - x_ref).abs() / P.x_bound(att, x_ref, E), f'{what} seq {b} pos {p}')
-
-
-def heavy_passes(probe, positions, rotate=None):
-    """Heavy key sets per pass: [pass][sequence][head] -> keys.  rotate = offset: one pass, the edges dealt from that offset."""
-    ranges = P.team_ranges(positions, probe.nh, probe.nb) if probe.persistent else {}
-    per_seq = []
-    for b, p in enumerate(positions):
-        edges = sorted(set().union(*[P.edge_keys(p, ranges.get((b, h), ())) for h in range(probe.nh)]))
-        deal = P.deal_heavy(edges, probe.nh, offset=rotate or 0)
-        per_seq.append(deal[:1] if rotate is not None else deal)
-    n = max(len(d) for d in per_seq)
-    return [[d[j % len(d)] for d in per_seq] for j in range(n)]
-
-
-def rotation_passes(nh, T):
-    """8 passes of nh heads x 8 keys in which every key t < T is heavy once: pass t % 8, head (t // 8) % nh."""
-    out = [[[] for _ in range(nh)] for _ in range(8)]
-    for t in range(T):
-        out[t % 8][(t // 8) % nh].append(t)
-    return out
-
-
-def sweep(probe, position_sets, profiles, gen, worst, rope, tok0=0, rotate_heavy=False, full_rotation=()):
-    vocab = probe.dec.vocab
-    for i, positions in enumerate(position_sets):
-        toks = [(tok0 + 7 * i + 3 * b) % vocab for b in range(probe.B)]
-        what = f'toks {toks} positions {positions}'
-        probe.learn(toks, positions)
-        for b, p in enumerate(positions):  # the appended K rows (q_rot, masked) against fp64 RoPE of the exact k
-            k_exact = P.exact_qv(probe.w, probe.dec.embed[toks[b]])[1]
-            rope.update(P.check_rope_row(probe.k_new[b], k_exact, p, probe.rope_base), f'{what} seq {b}')
-        anchors(probe, toks, positions, gen, what)
-        for kind in profiles:
-            if kind == 'heavy':
-                passes = heavy_passes(probe, positions, rotate=(i * 8 * probe.nh) if rotate_heavy else None)
-                if len(positions) == 1 and positions[0] in full_rotation:
-                    passes += [[r] for r in rotation_passes(probe.nh, positions[0])]
-                for heavy in passes:
-                    plants = [P.profile('heavy', q, p, gen, heavy=hv, g=probe.g) for q, p, hv in zip(probe.q_rot, positions, heavy)]
-                    bounded(probe, toks, positions, plants, worst[kind], what + ' heavy')
-            else:
-                plants = [P.profile(kind, q, p, gen, g=probe.g) for q, p in zip(probe.q_rot, positions)]
-                bounded(probe, toks, positions, plants, worst[kind], f'{what} {kind}')
-
-
-def run_sweeps(probe, name, position_sets, profiles=P.PROFILES, **kw):
-    gen = torch.Generator(device='cuda:0').manual_seed(1234)
-    worst = {k: Worst(f'{name} {k}') for k in profiles}
-    rope = Worst(f'{name} appended K row vs fp64 RoPE')
-    sweep(probe, position_sets, profiles, gen, worst, rope, **kw)
-    for w in list(worst.values()) + [rope]:
-        w.done()
 
 
 def label(probe, size):
@@ -127,10 +37,10 @@ def label(probe, size):
 def every_position(probe, name, seed):
     """Every position 0..599 at batch 1: heavy keys at every position (rotating over the edges), one more profile in turn."""
     gen = torch.Generator(device='cuda:0').manual_seed(seed)
-    worst = {k: Worst(f'{name} {k}') for k in P.PROFILES}
-    rope = Worst(f'{name} appended K row vs fp64 RoPE')
+    worst = {k: P.Worst(f'{name} {k}') for k in P.PROFILES}
+    rope = P.Worst(f'{name} appended K row vs fp64 RoPE')
     for i in range(600):
-        sweep(probe, [[i]], ('heavy', P.PROFILES[1 + i % 6]), gen, worst, rope, tok0=i, rotate_heavy=True)
+        P.sweep(probe, [[i]], ('heavy', P.PROFILES[1 + i % 6]), gen, worst, rope, toks=lambda j, b: i + 7 * j + 3 * b, rotate_heavy=True)
     for w in list(worst.values()) + [rope]:
         w.done()
 

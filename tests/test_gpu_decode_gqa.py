@@ -4,7 +4,7 @@ the prefill / extend / scoring pass, gptq_cached_attention_gqa and the quant mod
   * both engines against the CPU reference decoder at g = 2 and with one K/V head (g = 4), int4, act-order and 3-bit, batch 1 and batch 4 at
     ragged positions;
   * LLaMA-2-70B (g = 8), CodeLlama-34B (RoPE base 1e6, context 16384) and LLaMA-3-8B (base 5e5, vocabulary 128256) layers, two of them, on
-    the persistent kernel, block by block against the reference (llama_oracle.check_last_layer_blocks) on a random cache;
+    the persistent kernel, block by block against the reference on a random cache (llama_oracle.check_blocks_on_random_cache);
   * the shared new row: the g query heads of a group all use row pos, one of them stores it; every K/V head's row pos is the reference's
     rotated k, no other cache row changes, and prefill, extend and token-by-token decode write the same rows;
   * gptq_cached_attention_gqa against the float64 reference with the K/V heads repeated, and the MHA symbol unchanged;
@@ -20,41 +20,13 @@ import pytest
 import torch
 
 from gpu_util import assert_rel_close, check_cached_attention, fill_quant_linear, make_kv_cache
-from llama_oracle import CODELLAMA, KV_ROW_TOL, LlamaOracle, assert_no_failures, check, check_extend_against_stepping, check_last_layer_blocks, check_scores, \
-    step_all
-from oracle import gptq_oracle as O
+from llama_oracle import CODELLAMA, KV_ROW_TOL, LlamaOracle, assert_no_failures, check, check_blocks_on_random_cache, check_extend_against_stepping, \
+    check_scores, check_steps, step_all
 
 pytestmark = pytest.mark.gpu
 
 LLAMA2_70B = (10000.0, 1e-5)
 LLAMA3 = (5e5, 1e-5)
-
-
-class GqaOracle(LlamaOracle):
-    """LlamaOracle with n_kv_heads K/V heads: the fused qkv output is q | k | v of nh | nkv | nkv heads, RoPE rotates the first nh + nkv
-    heads, query head h attends with K/V head h // (nh // nkv).  attention() returns the new K / V rows of the nkv heads."""
-
-    def __init__(self, *a, n_kv_heads, **kw):
-        super().__init__(*a, **kw)
-        self.n_kv_heads = n_kv_heads
-
-    @classmethod
-    def from_decoder(cls, dec, *, eps, base):
-        return cls(dec.layers, dec.embed, dec.final_norm, dec.lm_head, dec.n_heads, eps=eps, base=base, n_kv_heads=dec.n_kv_heads)
-
-    def attention(self, li, x, pos, k_prefix=None, v_prefix=None, exact=False):
-        n, nh, nkv, hd = x.shape[0], self.n_heads, self.n_kv_heads, self.head_dim
-        g = nh // nkv
-        qkv = self._linear(li, 'qkv', O.rmsnorm_fwd(x, self._layer(li)['input_norm'], self.eps), exact).view(1, n, nh + 2 * nkv, hd).clone()
-        O.rope_inplace(qkv[:, :, None, :nh + nkv], torch.arange(pos, pos + n)[None, :], base=self.base)
-        q, k, v = (t.transpose(0, 1) for t in qkv[0].split([nh, nkv, nkv], 1))  # [heads, n, hd]
-        K = torch.cat([k_prefix[:, :pos], k], 1) if pos else k
-        V = torch.cat([v_prefix[:, :pos], v], 1) if pos else v
-        qg = q.float().reshape(nkv, g, n, hd)  # query head kvh * g + j
-        s = (qg @ K.float()[:, None].transpose(-1, -2)) * hd**-0.5  # [nkv, g, n, pos + n]
-        s = s.masked_fill(torch.ones(n, pos + n, dtype=torch.bool).triu(pos + 1), float('-inf'))
-        att = (torch.softmax(s, -1) @ V.float()[:, None]).reshape(nh, n, hd).half().transpose(0, 1).reshape(n, self.hidden)
-        return x + self._linear(li, 'o', att, exact), k, v
 
 
 def _decoder(size, **kw):
@@ -75,13 +47,7 @@ def test_decode_steps_match_oracle(size, bits, act):
     """Six decode steps against the reference decoder (bound of test_gpu_engine.py::test_decode_steps_match_oracle)."""
     dec = _decoder(size, bits=bits, groupsize=64, act_order=act, vocab=512, seed=bits, max_seq=64)
     toks = torch.randint(0, 512, (6, ), generator=torch.Generator().manual_seed(0)).tolist()
-    ref = GqaOracle.from_decoder(dec, eps=1e-6, base=10000.0).logits(toks)
-    for pos, tok in enumerate(toks):
-        dec.set_input(tok, pos)
-        dec.step()
-        torch.cuda.synchronize()
-        assert_rel_close(dec.logits[0], ref[pos], rel=2e-2, what=f'{size} bits={bits} act={act} pos={pos}')
-        assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
+    check_steps(dec, LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0), [toks], lambda k, b, pos: f'{size} bits={bits} act={act} pos={pos}')
 
 
 @pytest.mark.parametrize('size', SIZES)
@@ -92,55 +58,27 @@ def test_batch4_ragged_positions(size):
     lens = [5, 40, 2, 33]
     gen = torch.Generator().manual_seed(3)
     seqs = [torch.randint(0, 300, (n, ), generator=gen).tolist() for n in lens]
-    oracle = GqaOracle.from_decoder(dec, eps=1e-6, base=10000.0)
-    refs = [oracle.logits(s) for s in seqs]
-    for k in range(max(lens)):
-        pos = [min(k, n - 1) for n in lens]
-        dec.set_input([s[p] for s, p in zip(seqs, pos)], pos)
-        dec.step()
-        torch.cuda.synchronize()
-        for b in range(4):
-            assert_rel_close(dec.logits[b], refs[b][pos[b]], rel=2e-2, what=f'{size} step {k} sequence {b} pos {pos[b]}')
+    check_steps(dec, LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0), seqs, lambda k, b, pos: f'{size} step {k} sequence {b} pos {pos}')
 
 
-def _real_shape_blocks(size, positions, max_seq, rope, vocab=32000):
+def _check_gqa_layers(size, positions, max_seq, rope, vocab=32000):
     """Two layers of a real GQA shape on the persistent kernel, a random cache, one step at each position, block by block against the
     reference (the appended K rows against the exact linears, as test_gpu_engine_fullsize.py does where one-ulp roundings matter)."""
-    from gptq_b200 import engine
     base, eps = rope
-    dec2 = _decoder(size, bits=4, groupsize=128, vocab=vocab, seed=11, max_seq=max_seq, n_layers=2, rms_eps=eps, rope_base=base)
-    dec1 = engine.LlamaDecoder(dec2.layers[:1], dec2.embed, dec2.final_norm, dec2.lm_head, dec2.n_heads, max_seq=max_seq, rms_eps=eps, rope_base=base,
-                               n_kv_heads=dec2.n_kv_heads)
-    assert dec1.launches_per_step() == 1
-    gen = torch.Generator(device=dec2.dev).manual_seed(111)
-    dec2.k_cache.copy_((torch.randn(dec2.k_cache.shape, device=dec2.dev, generator=gen) * 0.5).half())
-    dec2.v_cache.copy_((torch.randn(dec2.v_cache.shape, device=dec2.dev, generator=gen) * 0.5).half())
-    k0, v0 = dec2.k_cache.clone(), dec2.v_cache.clone()
-    kc, vc = k0.cpu(), v0.cpu()
-    oracle = GqaOracle.from_decoder(dec2, eps=eps, base=base)
-    for i, pos in enumerate(positions):
-        tok = (17 * i + 3) % vocab
-        what = f'{size} base={base:g} pos={pos}'
-        # every position starts from the same cache: a step rewrites row pos, which a later, short context would read
-        for dec in (dec1, dec2):
-            dec.k_cache.copy_(k0[:len(dec.layers)])
-            dec.v_cache.copy_(v0[:len(dec.layers)])
-        check_last_layer_blocks(dec1, oracle, tok, pos, kc, vc, what + ' (1 layer)', False)
-        check_last_layer_blocks(dec2, oracle, tok, pos, kc, vc, what + ' (2 layers)', False)
-        assert_no_failures()
-    return dec2, oracle
+    dec = _decoder(size, bits=4, groupsize=128, vocab=vocab, seed=11, max_seq=max_seq, n_layers=2, rms_eps=eps, rope_base=base)
+    return dec, check_blocks_on_random_cache(dec, positions, f'{size} base={base:g}', eps=eps, base=base, cache_seed=111, k_row_vs_reference=False)
 
 
 def test_llama2_70b_layers():
-    _real_shape_blocks('70b', [0, 31, 32, 2047, 4095], 4096, LLAMA2_70B)
+    _check_gqa_layers('70b', [0, 31, 32, 2047, 4095], 4096, LLAMA2_70B)
 
 
 def test_codellama_34b_layers_at_16k():
-    _real_shape_blocks('34b', [16383], 16384, CODELLAMA)
+    _check_gqa_layers('34b', [16383], 16384, CODELLAMA)
 
 
 def test_llama3_8b_layers_greedy_sampled_and_scored():
-    dec, oracle = _real_shape_blocks('llama3-8b', [0, 2047], 2048, LLAMA3, vocab=128256)
+    dec, oracle = _check_gqa_layers('llama3-8b', [0, 2047], 2048, LLAMA3, vocab=128256)
     assert dec.vocab == 128256
     # greedy and sampled generation over the whole vocabulary (sampling takes up to 131072 ids)
     prompt = [5, 128255, 77, 1000]
@@ -167,7 +105,7 @@ def test_shared_new_row(size):
     """After a step at pos (batch 2, positions 37 and 5): row pos of every K/V head of layer 0 is the reference's rotated k and v (the layer's
     input is the embedding row), the rows before pos are what they were and the NaN-poisoned rows after pos are untouched."""
     dec = _decoder(size, bits=4, groupsize=64, vocab=300, seed=9, max_seq=64, batch=2)
-    oracle = GqaOracle.from_decoder(dec, eps=1e-6, base=10000.0)
+    oracle = LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0)
     gen = torch.Generator(device=dec.dev).manual_seed(5)
     dec.k_cache.copy_((torch.randn(dec.k_cache.shape, device=dec.dev, generator=gen) * 0.5).half())
     dec.v_cache.copy_((torch.randn(dec.v_cache.shape, device=dec.dev, generator=gen) * 0.5).half())
@@ -207,7 +145,6 @@ def test_prefill_extend_and_decode_write_the_same_rows(size):
     dec.step()
     torch.cuda.synchronize()
     assert_rel_close(dec.logits[0], ref_logits, rel=2e-2, what=f'{size}: logits after prefill + 1 decode step')
-    dec.reset()
     check_extend_against_stepping(dec, prompt, 17, f'{size} extend')
 
 
@@ -284,7 +221,7 @@ def test_hf_route():
         assert_rel_close(step.logits[0, 0], ref[8], rel=2e-2, what='QuantLlamaAttention step on the cache')
     dec = engine.from_hf_quant_model(model, max_seq=16)
     assert dec.n_kv_heads == 2 and dec.launches_per_step() == 1
-    oracle = GqaOracle.from_decoder(dec, eps=model.config.rms_norm_eps, base=10000.0).logits(ids[0, :6].tolist())
+    oracle = LlamaOracle.from_decoder(dec, eps=model.config.rms_norm_eps, base=10000.0).logits(ids[0, :6].tolist())
     for pos in range(6):
         dec.set_input(int(ids[0, pos]), pos)
         dec.step()

@@ -4,7 +4,7 @@ import pytest
 import torch
 
 from gpu_util import assert_rel_close, tiny_quant_llama
-from llama_oracle import CODELLAMA, LLAMA1, LlamaOracle, scale_down_embedding_row
+from llama_oracle import CODELLAMA, LLAMA1, LlamaOracle, check_steps, scale_down_embedding_row
 
 pytestmark = pytest.mark.gpu
 
@@ -35,14 +35,7 @@ def test_decode_steps_match_oracle(size, bits, act, use_graph, rope):
     toks = torch.randint(0, 512, (6, ), generator=gen).tolist()
     if rope != LLAMA1:
         scale_down_embedding_row(dec.embed, toks[0], 8)
-    ref = LlamaOracle.from_decoder(dec, eps=eps, base=base).logits(toks)
-    for pos, tok in enumerate(toks):
-        dec.tokens.fill_(tok)
-        dec.positions.fill_(pos)
-        dec.step()
-        torch.cuda.synchronize()
-        assert_rel_close(dec.logits[0], ref[pos], rel=2e-2, what=f'{size} bits={bits} act={act} base={base:g} eps={eps:g} pos={pos}')
-        assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
+    check_steps(dec, LlamaOracle.from_decoder(dec, eps=eps, base=base), [toks], lambda k, b, pos: f'{size} bits={bits} act={act} base={base:g} eps={eps:g} pos={pos}')
 
 
 @pytest.mark.parametrize('gs,rope', [pytest.param(-1, LLAMA1, id='-1'), pytest.param(32, LLAMA1, id='32'), pytest.param(32, CODELLAMA, id='32-codellama')])
@@ -69,13 +62,7 @@ def test_hf_checkpoint_groupsizes_decode_on_the_persistent_kernel(gs, rope):
         for name in ('qkv', 'o', 'gate', 'up', 'down'):
             K = kl[name].g_idx.numel()
             assert kl[name].hint == (K if gs == -1 else gs), f'{name}: groupsize hint {kl[name].hint}'
-    ref = LlamaOracle.from_decoder(dec, eps=eps, base=base).logits(toks)
-    for pos, tok in enumerate(toks):
-        dec.set_input(tok, pos)
-        dec.step()
-        torch.cuda.synchronize()
-        assert_rel_close(dec.logits[0], ref[pos], rel=2e-2, what=f'gs={gs} base={base:g} eps={eps:g} pos={pos}')
-        assert int(dec.next_tokens[0]) == int(dec.logits[0].float().argmax())
+    check_steps(dec, LlamaOracle.from_decoder(dec, eps=eps, base=base), [toks], lambda k, b, pos: f'gs={gs} base={base:g} eps={eps:g} pos={pos}')
 
 
 @pytest.mark.parametrize('size', ['tiny', 'tiny256'])
@@ -84,14 +71,8 @@ def test_long_context_attention_splits(size):
     from gptq_b200 import engine
     dec = engine.synthetic_llama(size, bits=4, groupsize=128, vocab=256, seed=1, max_seq=640)
     toks = torch.randint(0, 256, (530, ), generator=torch.Generator().manual_seed(1)).tolist()
-    ref = LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0).logits(toks)
-    for pos, tok in enumerate(toks):
-        dec.tokens.fill_(tok)
-        dec.positions.fill_(pos)
-        dec.step()
-        if pos in (0, 255, 256, 257, 511, 512, 529):
-            torch.cuda.synchronize()
-            assert_rel_close(dec.logits[0], ref[pos], rel=3e-2, what=f'pos={pos}')
+    check_steps(dec, LlamaOracle.from_decoder(dec, eps=1e-6, base=10000.0), [toks], lambda k, b, pos: f'pos={pos}', rel=3e-2,
+                checked=(0, 255, 256, 257, 511, 512, 529))
 
 
 def test_generate_is_deterministic_and_matches_stepwise():

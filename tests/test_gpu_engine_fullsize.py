@@ -20,55 +20,32 @@ end-to-end bound on the logits against the oracle run from the embedding.
 import pytest
 import torch
 
-from llama_oracle import END_TO_END_TOL, LlamaOracle, assert_no_failures, check, check_last_layer_blocks, scale_down_embedding_row
+from llama_oracle import check_blocks_on_random_cache
 
 pytestmark = pytest.mark.gpu
 
 
 def _run_case(size, bits, act, positions, vocab, seed, gs=128, max_seq=2048, rms_eps=1e-6, rope_base=10000.0, small_embedding=False,
               k_row_vs_reference=True):
-    """Both decoders and every oracle call take max_seq, rms_eps and rope_base from the arguments.  small_embedding: the token of the first
-    position has its embedding row scaled by 2^-8 (mean square about 4e-6, near the epsilon), so that the 1-layer checks see the epsilon.
-    k_row_vs_reference=False holds the appended K rows to the exact linears only (see the comment in the loop)."""
+    """The decoder, its twin and every oracle call take max_seq, rms_eps and rope_base from the arguments; the end-to-end check runs too
+    (llama_oracle.check_blocks_on_random_cache).  k_row_vs_reference=False holds the appended K rows to the exact linears only.
+
+    The K row is rotated after the fp16 rounding of k, so a one-ulp difference in k before RoPE can land on a small element of the rotated
+    row, whose bound is relative to the row's rms: whether the reference's per-weight fp16 rounding does that is a matter of the random draw,
+    not of the groupsize.  The draw of the gs -1 case does it: at context 2047, layer 1, one K-row element is 1.15 of its bound from the
+    reference rounding, while the kernel equals Exact there (measured: fp64 9.289385, kernel and Exact 9.2890625, the nearest fp16; reference
+    rounding 9.296875).  That case holds its K rows to Exact only, and so does the LLaMA-2-13B case: at context 4095, layer 0, one K-row
+    element is 1.05 of its bound from the reference rounding (|err| 2.93e-3, row rms 1.12) while the whole row stays within 0.39 of its bound
+    from Exact."""
     from gptq_b200 import engine
-    dec2 = engine.synthetic_llama(size, bits=bits, groupsize=gs, act_order=act, vocab=vocab, seed=seed, max_seq=max_seq, n_layers=2, rms_eps=rms_eps,
-                                  rope_base=rope_base)
-    assert dec2.launches_per_step() == 1, 'the persistent kernel must be the path under test'
-    for name, ly in dec2.klayers[0].items():
+    dec = engine.synthetic_llama(size, bits=bits, groupsize=gs, act_order=act, vocab=vocab, seed=seed, max_seq=max_seq, n_layers=2, rms_eps=rms_eps,
+                                 rope_base=rope_base)
+    for name, ly in dec.klayers[0].items():
         if hasattr(ly, 'qweight'):
             assert ly.hint == (ly.g_idx.numel() if gs == -1 else gs), f'{name}: groupsize hint {ly.hint}'
-    if small_embedding:
-        scale_down_embedding_row(dec2.embed, 3, 8)  # the token of the first position (17 * 0 + 3)
-    dec1 = engine.LlamaDecoder(dec2.layers[:1], dec2.embed, dec2.final_norm, dec2.lm_head, dec2.n_heads, max_seq=max_seq, rms_eps=rms_eps, rope_base=rope_base)
-    assert dec1.launches_per_step() == 1
-    gen = torch.Generator(device=dec2.dev).manual_seed(seed + 100)
-    dec2.k_cache.copy_((torch.randn(dec2.k_cache.shape, device=dec2.dev, generator=gen) * 0.5).half())
-    dec2.v_cache.copy_((torch.randn(dec2.v_cache.shape, device=dec2.dev, generator=gen) * 0.5).half())
-    kc, vc = dec2.k_cache.cpu(), dec2.v_cache.cpu()
-    oracle = LlamaOracle.from_decoder(dec2, eps=rms_eps, base=rope_base)
-    for i, pos in enumerate(positions):
-        tok = (17 * i + 3) % vocab
-        what = f'{size} int{bits} g{gs} act={act} eps={rms_eps:g} base={rope_base:g} pos={pos}'
-        dec1.k_cache.copy_(dec2.k_cache[:1])
-        dec1.v_cache.copy_(dec2.v_cache[:1])
-        # The K row is rotated after the fp16 rounding of k, so a one-ulp difference in k before RoPE can land on a small element of the
-        # rotated row, whose bound is relative to the row's rms: whether the reference's per-weight fp16 rounding does that is a matter of
-        # the random draw, not of the groupsize.  The draw of the gs -1 case does it: at context 2047, layer 1, one K-row element is
-        # 1.15 of its bound from the reference rounding, while the kernel equals Exact there (measured: fp64 9.289385, kernel and Exact
-        # 9.2890625, the nearest fp16; reference rounding 9.296875).  That case holds its K rows to Exact only, and so does the LLaMA-2-13B
-        # case: at context 4095, layer 0, one K-row element is 1.05 of its bound from the reference rounding (|err| 2.93e-3, row rms 1.12)
-        # while the whole row stays within 0.39 of its bound from Exact.
-        k_row = k_row_vs_reference and gs != -1
-        check_last_layer_blocks(dec1, oracle, tok, pos, kc, vc, what + ' (1 layer)', k_row)
-        logits2 = check_last_layer_blocks(dec2, oracle, tok, pos, kc, vc, what + ' (2 layers)', k_row)
-        # end to end from the embedding
-        x = dec2.embed[tok].cpu()[None, :].clone()
-        for li in range(2):
-            x = oracle.mlp(li, oracle.attention(li, x, pos, kc[li, 0], vc[li, 0])[0])
-        check(logits2, oracle.head(x)[0], rel=END_TO_END_TOL, what=what + ': logits after 2 layers, end to end')
-        dec2.k_cache.copy_(kc)  # every position starts from the same cache
-        dec2.v_cache.copy_(vc)
-    assert_no_failures()
+    check_blocks_on_random_cache(dec, positions, f'{size} int{bits} g{gs} act={act} eps={rms_eps:g} base={rope_base:g}', eps=rms_eps, base=rope_base,
+                                 cache_seed=seed + 100, k_row_vs_reference=k_row_vs_reference and gs != -1, small_embedding=small_embedding,
+                                 end_to_end=True)
 
 
 def test_mega_kernel_7b_int4_g128_matches_oracle():

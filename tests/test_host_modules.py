@@ -133,6 +133,8 @@ def test_rope_base_from_config():
             rope_base_from_config(LlamaConfig(rope_parameters={'rope_type': rope_type, 'factor': 2.0, 'rope_theta': 1e4}))
         with pytest.raises(ValueError, match=rope_type):
             rope_base_from_config(SimpleNamespace(rope_theta=1e4, rope_scaling={'type': rope_type, 'factor': 4.0}))
+        with pytest.raises(ValueError, match=rope_type):  # rope_parameters with only the legacy 'type' key
+            rope_base_from_config(SimpleNamespace(rope_parameters={'type': rope_type, 'factor': 2.0, 'rope_theta': 1e4}))
 
 
 def test_make_quant_attn_takes_the_rope_base_from_the_config():
